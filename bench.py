@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 visualDet3D hot path (contract: see the task brief / DESIGN.md).
+"""bench.py — headline benchmark of the visualDet3D hot path on the GPU (H100, sm_90a; see DESIGN.md).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config stereo|gac|monoflex|km3d|yolo3d] [--batch B]
+                    [--dump-outputs DIR]
     torchrun --nproc-per-node N bench.py --gpus N ...        (one rank per GPU, NCCL)
 
 Default workload (= BASELINE.json configs[1] / the `metric`): a "step" = one YOLOStereo3D forward (backbone -> cost volumes -> neck ->
@@ -15,9 +16,11 @@ post-optimisation of its shipped config on, monoflex / km3d = configs[3], yolo3d
                (crop / resize / normalise) -> forward -> all-gather -> D2H of the records; `e2e_f32` = the same with float32 network
                inputs (4x the H2D bytes), the form round 1 reported
   roofline     scale-4 PSMCosine kernel (dominant cost-volume kernel; stereo only): algorithmic bytes / CUDA-event time vs measured HBM peak
-  cpu_baseline / --impl reference : the UNMODIFIED reference (oracle/_ref/visualDet3D or /root/reference, loaded by oracle/refload.py)
-               running its own PyTorch forward on this host's cores (`kind: "reference"`); falls back to the oracle port (`"port"`)
-               only when no copy of the reference package travelled to this box
+  cpu_baseline / --impl reference : the UNMODIFIED reference (when oracle/refload.py finds a copy of the package) running its own PyTorch
+               forward on this host's cores (`kind: "reference"`); otherwise the oracle port (`"port"`)
+  --dump-outputs DIR   after the timed steps, the last timed step's outputs as DIR/<name>.npy: the record block the device step returns
+               (records.npy, float32 [B, 1 + kmax * 13]) and its per-detection columns (scores / boxes / classes / image, float32 / float64).
+               Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -43,7 +46,6 @@ CONFIGS = {
     "yolo3d": ("synthetic_288x1280_mono_images_per_sec", "images/s", 288, 1280, 1, "Yolo3D (ResNet-18, DCNv2 head) forward, batch {B} mono 288x1280 per GPU"),
 }
 FRAME_HW = (375, 1242)                                           # a KITTI camera frame; crop_top below gives the network aspect ratio
-PSM4_NCU_TRAFFIC_B8 = 137_400_000                                # DRAM bytes per launch of the scale-4 PSMCosine kernel at B = 8 (ncu)
 
 
 def measured_peaks():
@@ -54,11 +56,11 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "datasheet"                                    # H100 SXM HBM3, NVIDIA data sheet (not a measured rate)
 
 
 class ClockSampler:
-    """SM clock / power / throttle-reason sampling DURING the timed region (B200_PROFILING.md): NVML polled every 5 ms from a
+    """SM clock / power / throttle-reason sampling DURING the timed region: NVML polled every 5 ms from a
     thread (nvidia_ml_py), falling back to `nvidia-smi -lms` when NVML is not importable."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
     BITS = {"hw_slowdown": 0x8, "sw_power_cap": 0x4, "sw_thermal_slowdown": 0x20, "hw_thermal_slowdown": 0x40}
@@ -316,6 +318,7 @@ def main():
     ap.add_argument("--batch", type=int, default=None, help="samples per GPU per step (default: 8; yolo3d 1)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-mode", action="store_true", help="device-resident steps only (for ncu): no e2e leg, no CPU baseline")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -331,7 +334,7 @@ def main():
     from visualdet3d_b200.pipeline import StreamedInference
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device (the GPU path has no CPU fallback; use --impl reference for the CPU arm)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -456,12 +459,14 @@ def main():
         barrier()
         e0.record()
         e_fwd = torch.cuda.Event(enable_timing=True)
+        last = None
         for i in range(args.steps):
-            step_device(i)
+            last = step_device(i)
         e_fwd.record()                            # this rank's own forwards are done (per_rank.forward_ms_per_step: shows a slow GPU)
         drain()                                   # the last all-gathers are inside the timed region
         e1.record()
         barrier()
+        last_records = last[1].clone() if args.dump_outputs else None      # the buffer is reused by later steps
         launches = _lib.launch_count() + graph_launches() - g0          # kernels launched directly + kernels inside the replayed graphs
         ms_dev = e0.elapsed_time(e1)
         ms_fwd = e0.elapsed_time(e_fwd)
@@ -527,7 +532,7 @@ def main():
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": text.format(B=B) + ", random-init seeded weights", "name": args.config,
                    "global_batch": B * world, "parallelism": f"dp{world}",
-                   "l2": "activations + weights of one step exceed the 126 MB L2 several times over; no explicit flush",
+                   "l2": "activations + weights of one step exceed the 50 MB L2 several times over; no explicit flush",
                    "warmup_steps_run": args.warmup,
                    "conv_engine": os.environ.get("VD3D_CONV_ENGINE", "default"),
                    "cuda_graphs": ("one graph per record buffer / staging slot (graphs.GraphedStep); the stereo device-resident leg stays eager for the "
@@ -550,22 +555,39 @@ def main():
         psm_avg_ms = statistics.mean(psm_ms) if psm_ms else None
         achieved = (psm_bytes / 1e9) / (psm_avg_ms / 1e3) if psm_avg_ms else None
         tc = os.environ.get("VD3D_PSM_ENGINE", "tc") == "tc" and os.environ.get("VD3D_CONV_ENGINE", "tc16") == "tc16"
-        out["roofline"] = {"kernel": "psm_cosine_tc_kernel (scale-4 PSMCosine, tcgen05 on fp16 hi/lo planes)" if tc
+        out["roofline"] = {"kernel": "psm_cosine_tc_kernel (scale-4 PSMCosine, wgmma on fp16 hi/lo planes)" if tc
                            else "psm_cosine_nhwc_v4_kernel<64> (scale-4 PSMCosine, SIMT)",
                            "bound": "hbm", "achieved": achieved, "peak": peak, "peak_kind": peak_kind, "unit": "GB/s",
-                           "frac": (achieved / peak) if achieved else None, "avg_launch_ms": psm_avg_ms, "algorithmic_bytes_per_launch": psm_bytes,
-                           # dram__bytes_read.sum + dram__bytes_write.sum of this kernel at B = 8 from the committed `ncu --set full` capture
-                           "traffic": (PSM4_NCU_TRAFFIC_B8 if (B == 8 and tc) else None),
-                           "traffic_source": "ncu --set full, one launch, profiles/r01_ncu_psm_cosine_tc.txt (round 2 re-capture, profiles/r02_ncu_misc.txt row 10: 125.9 MB read + 11.3 MB written)"}
+                           "frac": (achieved / peak) if achieved else None, "avg_launch_ms": psm_avg_ms, "algorithmic_bytes_per_launch": psm_bytes}
         # the other cost-volume kernels, timed in situ the same way (SURVEY.md 8(d) algorithmic bytes per pair x batch)
         alg = {"psm8": 4 * (H // 8) * (W // 8) * (2 * 128 + 24) * B, "concat_volume": (2 * 8 * (H // 16) * (W // 16) * 4 + 16 * 12 * (H // 16) * (W // 16) * 4) * B}
         out["cost_volume_in_situ"] = {k: {"avg_launch_ms": statistics.mean(v), "algorithmic_bytes": alg[k], "GB_per_s": alg[k] / 1e9 / (statistics.mean(v) / 1e3),
                                           "frac_of_hbm_peak": alg[k] / 1e9 / (statistics.mean(v) / 1e3) / peak} for k, v in situ.items() if k in alg and v}
     if not args.no_cpu_baseline and world == 1:          # the CPU arm is timed on rank 0 at N = 1 only (the driver runs --impl reference for every N)
         out["cpu_baseline"] = cpu_baseline_subprocess(args.config, B)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_records)
     print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(path: str, records):
+    """DIR/<name>.npy of the last timed step (rank 0's batch): the record block and its per-detection columns."""
+    import numpy as np
+    from visualdet3d_b200 import parallel
+    os.makedirs(path, exist_ok=True)
+    rec = records.float().cpu()
+    np.save(os.path.join(path, "records.npy"), rec.numpy().astype(np.float32))
+    dets = parallel.unpack_records(rec)
+    cols = {"scores": [], "boxes": [], "classes": [], "image": []}
+    for b, (s, bx, c) in enumerate(dets):
+        cols["scores"].append(s.numpy().astype(np.float32))
+        cols["boxes"].append(bx.numpy().astype(np.float32).reshape(len(s), -1))
+        cols["classes"].append(c.numpy().astype(np.float64))
+        cols["image"].append(np.full(len(s), b, dtype=np.float64))
+    for k, v in cols.items():
+        np.save(os.path.join(path, k + ".npy"), np.concatenate(v) if v else np.zeros(0))
 
 
 def E_overflow() -> bool:

@@ -1,5 +1,5 @@
 /*
- * vd3d_b200.h — C ABI of libvd3d_b200.so: hand-written sm_100a kernels for visualDet3D's inference hot path.
+ * vd3d_b200.h — C ABI of libvd3d_b200.so: hand-written sm_90a (H100) kernels for visualDet3D's inference hot path.
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host; `stream` is a cudaStream_t passed as void*.
@@ -53,19 +53,19 @@ int vd3d_conv2d_nhwc(const float* in, int B, int H, int W, int Cin, int in_cs, i
                      const float* res, int res_cs, int res_co,
                      float* out, int Cout, int out_cs, int out_co, int relu, void* stream);
 
-/* ---- dense convolution (tcgen05 tensor cores, "3xTF32" split accumulation) --------------------------------------
- * Same op as vd3d_conv2d_nhwc for stride-1 convs with Cin % 32 == 0 and Cout % 16 == 0, on the 5th-gen tensor cores:
- * operands staged by TMA (4-D box per filter tap, zero padding = TMA out-of-bounds fill), tcgen05.mma kind::tf32 with the
- * fp32 accumulator in TMEM.  fp32-grade accuracy comes from splitting every operand v = hi + lo with
+/* ---- dense convolution (wgmma tensor cores, "3xTF32" split accumulation) ----------------------------------------
+ * Same op as vd3d_conv2d_nhwc for stride-1 convs with Cin % 32 == 0 and Cout % 16 == 0, on the Hopper tensor cores:
+ * operands staged by TMA (4-D box per filter tap, zero padding = TMA out-of-bounds fill), wgmma kind tf32 with the
+ * fp32 accumulator in registers.  fp32-grade accuracy comes from splitting every operand v = hi + lo with
  * hi = v & 0xFFFFE000 (what the MMA reads when handed v) and accumulating A*Whi + Alo*Whi + A*Wlo (passes = 3).
  *   in / in_lo   : NHWC activation and its lo companion (in_lo may be NULL when passes == 1)
  *   w_hi / w_lo  : [Cout][KH*KW*Cin] (k = (kh*KW + kw)*Cin + ci), BN folded, split on the host
  *   out / out_lo : NHWC result and (optional) its lo companion, written by the epilogue
- *   bn           : output-channel tile (multiple of 16, <= 256); 0 = vd3d_tc_pick_bn(Cout)
+ *   bn           : output-channel tile (multiple of 16, <= 256; tiles wider than 128 run as two equal halves); 0 = vd3d_tc_pick_bn(Cout)
  * passes == 1 is plain single-pass TF32 (diagnostics only: ~1e-3 relative error, not parity-grade). */
 int vd3d_tc_pick_bn(int Cout);
 /* tile width of the persistent fp16-split engine (default of vd3d_conv2d_tc16 when bn == 0): Cout split evenly into
- * ceil(Cout / 256) tiles of 16-column granules; tiles wider than 128 run as CTA pairs (cta_group::2, UMMA M = 256) */
+ * ceil(Cout / 128) tiles of 16-column granules (128 columns: the widest accumulator the consumer warpgroups hold in registers) */
 int vd3d_tc_pick_bn_persistent(int Cout);
 int vd3d_conv2d_tc(const float* in, const float* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
                    const float* w_hi, const float* w_lo, const float* bias, int KH, int KW, int pad, int dil,
@@ -111,7 +111,7 @@ int vd3d_conv2d_tc16_stem_pool(const void* in_hi, const void* in_lo, int B, int 
                                const void* w_hi, const void* w_lo, float out_scale, const float* bias,
                                float* pool_out, int Cout, int pool_cs, int pool_co, void* stream);
 /* The ResNet stem as one persistent kernel (csrc/stem_pool.cu): conv 7x7 / stride 2 / pad 3 (<= 4 -> 64 channels) + folded BN + ReLU +
- * MaxPool2d(3, 2, 1) (R/networks/backbones/resnet.py:120-122,186-189).  Replaces vd3d_conv2d_tc16_stem_pool: no window re-reads (the UMMA
+ * MaxPool2d(3, 2, 1) (R/networks/backbones/resnet.py:120-122,186-189).  Replaces vd3d_conv2d_tc16_stem_pool: no window re-reads (the wgmma
  * descriptor walks the overlapping 8-pixel windows inside one staged image row), no atomics, pooled tensor written as fp32 (`out`, may be
  * NULL) and / or fp16 (hi, lo) planes (may be NULL) NHWC [B][Hq][Wq][out_cs], channels [out_co, out_co + 64).
  * in_hi / in_lo: row planes [B][H][Wp][4] made by vd3d_image_to_h16_rows with xoff = vd3d_stem_pool_xoff() and Wp = vd3d_stem_pool_row_pitch(W)
@@ -317,7 +317,7 @@ int vd3d_look_ground_sample(const float* x, int B, int H, int W, int C, int x_cs
                             float baseline, float relative_elevation,
                             float* out, float* out_lo, int out_cs, void* stream);
 
-/* Fused (modulated) deformable convolution: the bilinear gather writes the fp16 (hi, lo) A operand of the tcgen05 GEMM straight into
+/* Fused (modulated) deformable convolution: the bilinear gather writes the fp16 (hi, lo) A operand of the wgmma GEMM straight into
  * shared memory (SWIZZLE_128B K-major layout + fence.proxy.async), so the column tensor of the reference (deform_conv_cuda.cpp:539-556)
  * never exists in HBM.  x: NHWC fp32; om: NHWC at output resolution holding the offsets (channel off_co + 2k = dh, + 1 = dw) and, when
  * has_mask, the modulation (msk_co + k; mask_sigmoid applies the sigmoid of ModulatedDeformConvPack.forward); weights: the fp16 (hi, lo)

@@ -34,7 +34,7 @@ def _so_path(name: str) -> str:
 def copy_package() -> None:
     """The reference's Python package, copied verbatim next to its compiled extensions (oracle/_ref/visualDet3D, git-ignored, ships to
     the GPU box with the snapshot): `bench.py --impl reference` then times the REAL reference on the box's host cores and the seam
-    tests run its unmodified modules against the B200 ops.  Nothing under oracle/_ref is ever imported by the product package."""
+    tests run its unmodified modules against the project's ops.  Nothing under oracle/_ref is ever imported by the product package."""
     import shutil
     src, dst = os.path.join(REF, "visualDet3D"), os.path.join(OUT, "visualDet3D")
     if not os.path.isdir(src):
@@ -57,7 +57,7 @@ def build(verbose: bool = False) -> None:
     todo = [n for n in SOURCES if not os.path.exists(_so_path(n))]
     if not todo:
         return
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     os.environ.setdefault("CUDA_HOME", "/usr/local/cuda")
     from torch.utils import cpp_extension
     for name in todo:

@@ -118,11 +118,12 @@ def test_host_side_tile_and_layout_helpers():
     for cout in (16, 24, 64, 72, 128, 144, 256, 288, 384, 608, 1152, 1408, 2048):
         bn = lib.vd3d_tc_pick_bn_persistent(cout)
         cp = (cout + 15) // 16 * 16
-        assert bn % 16 == 0 and 16 <= bn <= 256
+        assert bn % 16 == 0 and 16 <= bn <= 128
         n_tiles = (cp + bn - 1) // bn
-        assert n_tiles == (cp + 255) // 256                      # as few tiles as 256 accumulator columns allow ...
+        assert n_tiles == (cp + 127) // 128                      # as few tiles as 128 accumulator columns (the widest tile) allow ...
         assert n_tiles * bn - cp < 16 * n_tiles                  # ... split evenly (less than one 16-column granule of padding per tile)
-    assert lib.vd3d_tc_pick_bn_persistent(1408) == 240 and lib.vd3d_tc_pick_bn_persistent(64) == 64
+    assert lib.vd3d_tc_pick_bn_persistent(1408) == 128 and lib.vd3d_tc_pick_bn_persistent(608) == 128 and lib.vd3d_tc_pick_bn_persistent(144) == 80
+    assert lib.vd3d_tc_pick_bn_persistent(64) == 64
     # stem rows: `pad` zero pixels on the left, the image, and the 16-pixel window of the last output column; even pixel count
     for (W, KW, s, pad) in ((1280, 7, 2, 3), (320, 7, 2, 3), (53, 7, 2, 3), (96, 3, 2, 1)):
         Wp = lib.vd3d_stem_row_pitch(W, KW, s, pad)

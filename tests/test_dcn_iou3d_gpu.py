@@ -1,5 +1,6 @@
-"""-m gpu: the two op families the reference builds under make.sh (DCN v1/v2, iou3d) against (a) the reference's OWN
-compiled extensions (oracle/_ref, built by oracle/build_ref.py from the reference sources) and (b) CPU restatements."""
+"""-m gpu: the two op families the reference builds under make.sh (DCN v1/v2, iou3d) against (a) what the reference's OWN compiled
+extensions (oracle/_ref, built by oracle/build_ref.py from the reference sources) return for the same seeded inputs, stored in
+tests/golden/ref_ops.npz by tests/golden/make_golden_ref_ops.py, and (b) CPU restatements."""
 import os
 
 import numpy as np
@@ -7,16 +8,34 @@ import pytest
 import torch
 
 import torch_port as tp
+from conftest import GOLDEN
 
 pytestmark = pytest.mark.gpu
+N_SAMPLE = 2048                  # stored values per large reference tensor (a fixed seeded sample of positions)
+RECORD = {} if os.environ.get("VD3D_RECORD_REF") else None      # make_golden_ref_ops.py: run the real extensions and record
+_STORED = {}
 
 
-def ref_ext(name):
-    import build_ref
-    try:
-        return build_ref.load(name)
-    except FileNotFoundError as e:
-        pytest.skip(str(e))
+def sample(t):
+    a = t.detach().reshape(-1).cpu().numpy()
+    if a.size <= N_SAMPLE:
+        return a
+    return a[np.sort(np.random.default_rng(a.size).choice(a.size, N_SAMPLE, replace=False))]
+
+
+def ref_out(key, run, full=False):
+    """The reference extension's output `key` (flattened; sampled unless `full`; `key + "_absmax"` = max |.| of the whole tensor): from
+    tests/golden/ref_ops.npz, or, while that file is being written, run(ext) on the real extension (ext(name) loads one)."""
+    if RECORD is None:
+        if not _STORED:
+            _STORED.update(np.load(os.path.join(GOLDEN, "ref_ops.npz")))
+        return _STORED[key]
+    if run is not None:
+        import build_ref
+        t = run(build_ref.load)
+        RECORD[key] = t.detach().reshape(-1).cpu().numpy() if full else sample(t)
+        RECORD[key + "_absmax"] = np.float64(float(t.abs().max()))
+    return RECORD[key]
 
 
 def rand_boxes(n, g, spread=10.0):
@@ -28,14 +47,18 @@ def rand_boxes(n, g, spread=10.0):
 
 def test_iou3d_pairwise_vs_reference_extension_and_clipping():
     from visualdet3d_b200.ops import iou3d
-    ref = ref_ext("ref_iou3d_cuda")
     g = torch.Generator().manual_seed(0)
     a, b = rand_boxes(70, g).cuda(), rand_boxes(45, g).cuda()
-    for mine, theirs in ((iou3d.boxes_overlap_bev_gpu, ref.boxes_overlap_bev_gpu), (iou3d.boxes_iou_bev_gpu, ref.boxes_iou_bev_gpu)):
-        o1 = torch.zeros(70, 45, device="cuda"); o2 = torch.zeros(70, 45, device="cuda")
-        assert mine(a, b, o1) == 1 and theirs(a, b, o2) == 1
+
+    def theirs(name):
+        o2 = torch.zeros(70, 45, device="cuda")
+        return lambda ext: (getattr(ext("ref_iou3d_cuda"), name)(a, b, o2), o2)[1]
+    for mine, name in ((iou3d.boxes_overlap_bev_gpu, "boxes_overlap_bev_gpu"), (iou3d.boxes_iou_bev_gpu, "boxes_iou_bev_gpu")):
+        o1 = torch.zeros(70, 45, device="cuda")
+        assert mine(a, b, o1) == 1
+        o2 = ref_out(name, theirs(name), full=True)
         torch.cuda.synchronize()
-        np.testing.assert_allclose(o1.cpu().numpy(), o2.cpu().numpy(), rtol=1e-4, atol=1e-5)
+        np.testing.assert_allclose(o1.cpu().numpy().reshape(-1), o2, rtol=1e-4, atol=1e-5)
     ov = torch.zeros(70, 45, device="cuda")
     iou3d.boxes_overlap_bev_gpu(a, b, ov)
     ac, bc, ovc = a.cpu().numpy(), b.cpu().numpy(), ov.cpu().numpy()
@@ -51,13 +74,16 @@ def test_iou3d_pairwise_vs_reference_extension_and_clipping():
 @pytest.mark.parametrize("n", [1, 63, 64, 65, 300])
 def test_iou3d_nms_vs_reference_extension(n):
     from visualdet3d_b200.ops import iou3d
-    ref = ref_ext("ref_iou3d_cuda")
     g = torch.Generator().manual_seed(n)
     boxes = rand_boxes(n, g, spread=8.0).cuda()
-    for mine, theirs in ((iou3d.nms_gpu, ref.nms_gpu), (iou3d.nms_normal_gpu, ref.nms_normal_gpu)):
-        k1, k2 = torch.zeros(n, dtype=torch.int64), torch.zeros(n, dtype=torch.int64)
-        n1, n2 = mine(boxes, k1, 0.3), theirs(boxes, k2, 0.3)
-        assert n1 == n2 and torch.equal(k1[:n1], k2[:n2])            # bit-exact keep indices
+
+    def theirs(name):
+        k2 = torch.zeros(n, dtype=torch.int64)
+        return lambda ext: k2[:getattr(ext("ref_iou3d_cuda"), name)(boxes, k2, 0.3)]
+    for mine, name in ((iou3d.nms_gpu, "nms_gpu"), (iou3d.nms_normal_gpu, "nms_normal_gpu")):
+        k1 = torch.zeros(n, dtype=torch.int64)
+        n1, k2 = mine(boxes, k1, 0.3), ref_out(f"{name}_{n}", theirs(name), full=True)
+        assert n1 == len(k2) and np.array_equal(k1[:n1].numpy(), k2)            # bit-exact keep indices
     assert iou3d.nms_gpu(boxes[:0], torch.zeros(0, dtype=torch.int64), 0.3) == 0
     with pytest.raises(RuntimeError):
         iou3d.nms_gpu(boxes.cpu(), torch.zeros(n, dtype=torch.int64), 0.3)
@@ -99,20 +125,22 @@ def test_modulated_deform_conv_vs_reference_extension(case):
     xc, wc, bc, oc, mc = x.cuda(), w.cuda(), bias.cuda(), off.cuda(), mask.cuda()
     out = torch.empty(B, Co, Ho, Wo, device="cuda")
     dcn.modulated_deform_conv_forward(xc, wc, bc, xc.new_empty(0), oc, mc, out, xc.new_empty(0), k, k, s, s, p, p, d, d, 1, dg, True)
-    ref = ref_ext("ref_deform_conv_ext")
     out_ref = torch.empty(B, Co, Ho, Wo, device="cuda")
-    ref.modulated_deform_conv_forward(xc, wc, bc, xc.new_empty(0), oc, mc, out_ref, xc.new_empty(0), k, k, s, s, p, p, d, d, 1, dg, True)
+    key = f"dcn_v2_{DCN_CASES.index(case)}"
+    out_ref = ref_out(key, lambda ext: (ext("ref_deform_conv_ext").modulated_deform_conv_forward(
+        xc, wc, bc, xc.new_empty(0), oc, mc, out_ref, xc.new_empty(0), k, k, s, s, p, p, d, d, 1, dg, True), out_ref)[1])
     torch.cuda.synchronize()
-    np.testing.assert_allclose(out.cpu().numpy(), out_ref.cpu().numpy(), rtol=1e-4, atol=2e-5)
+    np.testing.assert_allclose(sample(out), out_ref, rtol=1e-4, atol=2e-5)
     if dg == 1:
         cpu = tp.modulated_deform_conv(x, off, mask, w, bias, s, p, d)
         np.testing.assert_allclose(out.cpu().numpy(), cpu.numpy(), rtol=1e-4, atol=2e-5)
     # DCN v1 (no mask, no bias)
     o1 = torch.empty(B, Co, Ho, Wo, device="cuda"); o2 = torch.empty(B, Co, Ho, Wo, device="cuda")
     assert dcn.deform_conv_forward(xc, wc, oc, o1, xc.new_empty(0), xc.new_empty(0), k, k, s, s, p, p, d, d, 1, dg, B) == 1
-    ref.deform_conv_forward(xc, wc, oc, o2, xc.new_empty(0), xc.new_empty(0), k, k, s, s, p, p, d, d, 1, dg, B)
+    o2 = ref_out(key.replace("v2", "v1"), lambda ext: (ext("ref_deform_conv_ext").deform_conv_forward(
+        xc, wc, oc, o2, xc.new_empty(0), xc.new_empty(0), k, k, s, s, p, p, d, d, 1, dg, B), o2)[1])
     torch.cuda.synchronize()
-    np.testing.assert_allclose(o1.cpu().numpy(), o2.cpu().numpy(), rtol=1e-4, atol=2e-5)
+    np.testing.assert_allclose(sample(o1), o2, rtol=1e-4, atol=2e-5)
 
 
 @pytest.mark.parametrize("case", DCN_CASES)
@@ -132,44 +160,58 @@ def test_deform_conv_backward_vs_reference_extension(case):
     mask = torch.sigmoid(torch.randn(B, k * k * dg, Ho, Wo, generator=g))
     gout = torch.randn(B, Co, Ho, Wo, generator=g)
     xc, wc, bc, oc, mc, gc = x.cuda(), w.cuda(), bias.cuda(), off.cuda(), mask.cuda(), gout.cuda()
-    ref = ref_ext("ref_deform_conv_ext")
     e = lambda: xc.new_empty(0)
+    ci = DCN_CASES.index(case)
 
-    def close(a, b, what):
-        scale = float(b.abs().max()) + 1e-12
-        err = float((a - b).abs().max()) / scale
+    def close(a, b, what, factor=1.0):           # b: the reference tensor's key; scale = max |.| of the whole reference tensor
+        ref = ref_out(f"dcn_bwd_{ci}_{b[0]}", b[1]).astype(np.float64) * factor
+        scale = float(ref_out(f"dcn_bwd_{ci}_{b[0]}_absmax", None)) * factor + 1e-12
+        err = float(np.abs(sample(a).astype(np.float64) - ref).max()) / scale
         assert err < 1e-4, (what, err)
         return err
 
+    def run_ref(v1):
+        def run(ext):
+            if "grads" not in memo:
+                ref = ext("ref_deform_conv_ext")
+                gi, gw, gb = torch.zeros_like(xc), torch.zeros_like(wc), torch.zeros_like(bc)
+                go, gm = torch.zeros_like(oc), torch.zeros_like(mc)
+                ref.modulated_deform_conv_backward(xc, wc, bc, e(), oc, mc, e(), gi, gw, gb, go, gm, gc, k, k, s, s, p, p, d, d, 1, dg, True)
+                g1i, g1o, g1w = torch.zeros_like(xc), torch.zeros_like(oc), torch.zeros_like(wc)
+                ref.deform_conv_backward_input(xc, oc, gc, g1i, g1o, wc, e(), k, k, s, s, p, p, d, d, 1, dg, B)
+                ref.deform_conv_backward_parameters(xc, oc, gc, g1w, e(), e(), k, k, s, s, p, p, d, d, 1, dg, 0.5, B)
+                torch.cuda.synchronize()
+                memo["grads"] = (gi, gw, gb, go, gm, g1i, g1o, g1w)
+            return memo["grads"][v1]
+        return run
+    memo = {}
+    names = ("grad_input", "grad_weight", "grad_bias", "grad_offset", "grad_mask", "v1_grad_input", "v1_grad_offset", "v1_grad_weight")
+    ref = {n: (n, run_ref(i)) for i, n in enumerate(names)}
+
     # ---- DCNv2 ----
-    res = []
-    for ext in (dcn, ref):
-        gi, gw, gb = torch.zeros_like(xc), torch.zeros_like(wc), torch.zeros_like(bc)
-        go, gm = torch.zeros_like(oc), torch.zeros_like(mc)
-        ext.modulated_deform_conv_backward(xc, wc, bc, e(), oc, mc, e(), gi, gw, gb, go, gm, gc, k, k, s, s, p, p, d, d, 1, dg, True)
-        torch.cuda.synchronize()
-        res.append((gi, gw, gb, go, gm))
-    errs = [close(a, b, n) for a, b, n in zip(res[0], res[1], ("grad_input", "grad_weight", "grad_bias", "grad_offset", "grad_mask"))]
-    # accumulate-into contracts: a second call doubles grad_input / grad_weight / grad_bias, re-assigns grad_offset / grad_mask
-    gi, gw, gb, go, gm = [t.clone() for t in res[0]]
+    gi, gw, gb = torch.zeros_like(xc), torch.zeros_like(wc), torch.zeros_like(bc)
+    go, gm = torch.zeros_like(oc), torch.zeros_like(mc)
     dcn.modulated_deform_conv_backward(xc, wc, bc, e(), oc, mc, e(), gi, gw, gb, go, gm, gc, k, k, s, s, p, p, d, d, 1, dg, True)
-    close(gi, 2 * res[1][0], "grad_input x2"), close(gw, 2 * res[1][1], "grad_weight x2"), close(go, res[1][3], "grad_offset again")
+    torch.cuda.synchronize()
+    res = (gi, gw, gb, go, gm)
+    errs = [close(a, ref[n], n) for a, n in zip(res, names[:5])]
+    # accumulate-into contracts: a second call doubles grad_input / grad_weight / grad_bias, re-assigns grad_offset / grad_mask
+    gi, gw, gb, go, gm = [t.clone() for t in res]
+    dcn.modulated_deform_conv_backward(xc, wc, bc, e(), oc, mc, e(), gi, gw, gb, go, gm, gc, k, k, s, s, p, p, d, d, 1, dg, True)
+    close(gi, ref["grad_input"], "grad_input x2", 2.0), close(gw, ref["grad_weight"], "grad_weight x2", 2.0), close(go, ref["grad_offset"], "grad_offset again")
     # ---- DCNv1 ----
-    r1 = []
-    for ext in (dcn, ref):
-        gi, go, gw = torch.zeros_like(xc), torch.zeros_like(oc), torch.zeros_like(wc)
-        assert ext.deform_conv_backward_input(xc, oc, gc, gi, go, wc, e(), k, k, s, s, p, p, d, d, 1, dg, B) == 1
-        assert ext.deform_conv_backward_parameters(xc, oc, gc, gw, e(), e(), k, k, s, s, p, p, d, d, 1, dg, 0.5, B) == 1
-        torch.cuda.synchronize()
-        r1.append((gi, go, gw))
-    errs += [close(a, b, n) for a, b, n in zip(r1[0], r1[1], ("v1 grad_input", "v1 grad_offset", "v1 grad_weight (scale 0.5)"))]
+    gi, go, gw = torch.zeros_like(xc), torch.zeros_like(oc), torch.zeros_like(wc)
+    assert dcn.deform_conv_backward_input(xc, oc, gc, gi, go, wc, e(), k, k, s, s, p, p, d, d, 1, dg, B) == 1
+    assert dcn.deform_conv_backward_parameters(xc, oc, gc, gw, e(), e(), k, k, s, s, p, p, d, d, 1, dg, 0.5, B) == 1
+    torch.cuda.synchronize()
+    errs += [close(a, ref[n], n) for a, n in zip((gi, go, gw), names[5:])]
     print(case, "max relative errors", ["%.1e" % v for v in errs])
 
 
 @pytest.mark.parametrize("case", [(2, 64, 24, 40, 64, 1, 1, 0.5), (1, 128, 20, 28, 64, 1, 1, 0.5), (2, 64, 17, 23, 256, 1, 1, 0.5), (1, 64, 21, 30, 128, 2, 1, 0.5),
                                   (1, 192, 9, 50, 96, 1, 2, 0.5), (2, 64, 33, 47, 64, 1, 1, 5.0), (1, 256, 13, 21, 128, 1, 1, 2.0)])
 def test_fused_deform_conv_matches_unfused_and_reference(case, monkeypatch):
-    """csrc/dcn_fused.cu (bilinear gather written straight into the swizzled shared-memory operand of the tcgen05 GEMM) against
+    """csrc/dcn_fused.cu (bilinear gather written straight into the swizzled shared-memory operand of the wgmma GEMM) against
     (a) the unfused path (fp16 column planes in HBM + 1x1 conv): bit-identical, same K order and gather arithmetic;
     (b) the reference's own compiled extension on the same tensors: rtol 1e-4."""
     from visualdet3d_b200 import engine as E
@@ -204,13 +246,13 @@ def test_fused_deform_conv_matches_unfused_and_reference(case, monkeypatch):
     # reference extension: offsets / mask from the same offset conv, computed by torch
     om = torch.nn.functional.conv2d(x, ow, ob, stride=s, padding=d, dilation=d)
     off, mask = om[:, :18].contiguous().cuda(), torch.sigmoid(om[:, 18:]).contiguous().cuda()
-    ref = ref_ext("ref_deform_conv_ext")
     xc = x.cuda()
     out_ref = torch.empty(B, Co, Ho, Wo, device="cuda")
-    ref.modulated_deform_conv_forward(xc, w.cuda(), bias.cuda(), xc.new_empty(0), off, mask, out_ref, xc.new_empty(0), 3, 3, s, s, d, d, d, d, 1, 1, True)
-    want = torch.relu(out_ref + res.t.permute(0, 3, 1, 2))
+    out_ref = ref_out(f"fused_{int(2 * sum(case))}", lambda ext: (ext("ref_deform_conv_ext").modulated_deform_conv_forward(
+        xc, w.cuda(), bias.cuda(), xc.new_empty(0), off, mask, out_ref, xc.new_empty(0), 3, 3, s, s, d, d, d, d, 1, 1, True), out_ref)[1])
+    want = np.maximum(out_ref + sample(res.t.permute(0, 3, 1, 2)), 0.0)
     got = outs[0][0][..., 4:4 + Co].permute(0, 3, 1, 2)
-    np.testing.assert_allclose(got.cpu().numpy(), want.cpu().numpy(), rtol=1e-4, atol=5e-5)
+    np.testing.assert_allclose(sample(got), want, rtol=1e-4, atol=5e-5)
 
 
 def test_dcn_error_behaviour_and_pack_module():

@@ -154,7 +154,7 @@ def test_concat_volume_conv3d_vs_oracle():
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# tcgen05 conv engine
+# wgmma conv engine
 # ----------------------------------------------------------------------------------------------------------------
 def _trunc13(t):
     return (t.contiguous().view(torch.int32) & -8192).view(torch.float32)
@@ -238,7 +238,7 @@ TC16_MODES = {"default": ("0", "1", "0", "2"), "auto": ("0", "1", "0", "1"), "pe
 
 
 def _tc16_mode(monkeypatch, mode):
-    """default: persistent kernel, CTA pairs (cta_group::2, UMMA M = 256) for tiles wider than 128 columns and input-halo reuse
+    """Engine switches of the Blackwell build (on H100 every mode runs the one persistent wgmma kernel; the modes stay as inputs): persistent kernel, CTA pairs for tiles wider than 128 columns and input-halo reuse
     (A staged once per channel chunk for the nine taps) for those paired 3x3 stride-1 convs; auto / persistent / pair: halo reuse
     for every 3x3 stride-1 conv with automatic pairing / one CTA per SM / CTA pairs everywhere;
     *-generic: per-tap input boxes for every conv (no halo reuse); tile: one CTA per output tile (round-1 kernel);
@@ -395,7 +395,7 @@ def test_conv2d_tc16_strided_and_ragged_channels(case, mode, monkeypatch):
 
 @pytest.mark.parametrize("mode", ["default", "auto", "persistent", "pair", "auto-generic", "persistent-generic", "pair-generic"])
 def test_conv2d_tc16_persistent_many_tiles(mode, monkeypatch):
-    """more output tiles than SMs (every CTA loops several times, the TMA ring and the TMEM chunk buffers wrap across tiles),
+    """more output tiles than SMs (every CTA loops several times, the TMA ring and the chunk promotion wrap across tiles),
     an odd number of M tiles (the second CTA of the last pair is dead) and several N tiles; checked against the exact-fp32
     SIMT engine of the same library."""
     E = _E()
@@ -506,7 +506,7 @@ def test_stem_with_fused_maxpool_is_bit_identical(shape):
 @pytest.mark.parametrize("shape", [(2, 3, 64, 96), (3, 3, 70, 154), (1, 3, 34, 30), (2, 3, 96, 320), (16, 3, 96, 160), (2, 3, 384, 1280), (1, 3, 75, 515), (5, 3, 21, 1010)])
 @pytest.mark.parametrize("f32_out", [True, False])
 def test_stem_row_strip_kernel_is_bit_identical(shape, f32_out):
-    """csrc/stem_pool.cu (conv1 + BN + ReLU + MaxPool2d(3, 2, 1) as one row-strip kernel: overlapping windows through a no-swizzle UMMA
+    """csrc/stem_pool.cu (conv1 + BN + ReLU + MaxPool2d(3, 2, 1) as one row-strip kernel: overlapping windows through a no-swizzle wgmma
     descriptor, max-pool in registers, pooled tensor as fp16 planes [+ fp32]) against the stem kernel followed by the max-pool kernel: bit for
     bit, for one and several strips / row segments, odd conv and pooled sizes, image rows above / below the image, a channel slice, repeated calls."""
     E = _E()
@@ -553,7 +553,7 @@ ROW_CONV_CASES = [
 
 @pytest.mark.parametrize("case", ROW_CONV_CASES)
 def test_row_conv_vs_fp64(case):
-    """csrc/row_conv.cu (few-channel convs as row-strip tcgen05 kernels: overlapping windows through a no-swizzle UMMA descriptor on fp16 (hi, lo)
+    """csrc/row_conv.cu (few-channel convs as row-strip wgmma kernels: overlapping windows through a no-swizzle wgmma descriptor on fp16 (hi, lo)
     row planes) against an fp64 convolution of the same fp32 inputs: < 2e-5 (the bound of the fp16-split engine), fp32 output and planes, output
     written at a column offset of a wider, zero-bordered buffer (the next row conv's input form), neighbouring channels untouched."""
     E = _E()

@@ -191,7 +191,7 @@ def test_lo_companions_are_fresh_everywhere(det_bundle, monkeypatch):
 
 
 def test_engines_agree(det_bundle):
-    """The tcgen05 engines (fp16-split default, 3xTF32) and the exact-fp32 SIMT engine give the same detections (sets) and
+    """The wgmma engines (fp16-split default, 3xTF32) and the exact-fp32 SIMT engine give the same detections (sets) and
     values within 1e-3."""
     import os
     from visualdet3d_b200 import synth

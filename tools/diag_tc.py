@@ -1,4 +1,4 @@
-"""Diagnostic for the tcgen05 conv engine: isolates which of the three passes / which k-block pattern is wrong."""
+"""Diagnostic for the wgmma conv engine: isolates which of the three passes / which k-block pattern is wrong."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch, torch.nn.functional as F

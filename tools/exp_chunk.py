@@ -1,7 +1,7 @@
-"""Promotion-chunk sweep of the fp16-split conv engine (VD3D_TC_CHUNK = k-blocks accumulated in TMEM between two promotions into the fp32
+"""Promotion-chunk sweep of the fp16-split conv engine (VD3D_TC_CHUNK = k-blocks accumulated by the tensor core between two promotions into the fp32
 registers): error against the REFERENCE fixture at the BASELINE shape (tests/golden/stereo3d_384x1280.npz, the unmodified reference's
-outputs on the same seeded inputs) and the step time at batch 8.  The TMEM accumulator is updated with truncation (DESIGN 3.1), so longer
-chunks are faster (fewer tcgen05.ld + add rounds) and less accurate.
+outputs on the same seeded inputs) and the step time at batch 8.  The MMA accumulator is updated with truncation (DESIGN 3.1), so longer
+chunks are faster (fewer promotion rounds) and less accurate.
 
     python tools/exp_chunk.py [--chunks 4,6,9,12,18,36]
 """

@@ -69,5 +69,3 @@ for dbg, lab in ((64, "knock-out: 1/12 of the MMAs (first K step, one pass), all
     run(lab, {"VD3D_TC_DEBUG": dbg}, MK)
 for ch in (2, 9, 36):
     run(f"chunk = {ch} k-blocks per promotion", {"VD3D_TC_CHUNK": ch}, MK)
-for nb in (2, 3):
-    run(f"TMEM buffers = {nb}", {"VD3D_TC_NBUF": nb}, MK)

@@ -1,4 +1,4 @@
-"""visualdet3d_b200 — B200-native (sm_100a) inference forward for visualDet3D's dense 3D-detection hot path.
+"""visualdet3d_b200 — GPU-native (H100, sm_90a) inference forward for visualDet3D's dense 3D-detection hot path.
 
 Only what the path needs lives here: ``csrc/`` (hand-written CUDA kernels behind a C ABI, ``include/vd3d_b200.h``),
 the ctypes binding (``_lib``), the host-side mirror of the reference's registry / detector interface

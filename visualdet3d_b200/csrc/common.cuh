@@ -1,4 +1,4 @@
-// Shared host/device helpers for libvd3d_b200 (sm_100a only).
+// Shared host/device helpers for libvd3d_b200 (sm_90a: H100).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,7 +45,7 @@ constexpr float kFp16Overflow = 65520.0f;      // smallest magnitude that rounds
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM: persistent grids and tile-cost models
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ float amax4(float m, const float4& a) { return fmaxf(fmaxf(m, fmaxf(fabsf(a.x), fabsf(a.y))), fmaxf(fabsf(a.z), fabsf(a.w))); }

@@ -1,7 +1,7 @@
 // SIMT fp32 implicit-GEMM convolution on NHWC activations (exact fp32 FMA accumulation).
 //
 // This is the reference-accuracy engine: every dense conv of the path can run here, and the small-channel /
-// HBM-bound layers (3-, 8-, 24-, 72-channel convs) always do.  The big GEMM-shaped layers move to the tcgen05
+// HBM-bound layers (3-, 8-, 24-, 72-channel convs) always do.  The big GEMM-shaped layers move to the wgmma
 // engine (conv2d_tc.cu) once that is parity-green against this kernel.
 //
 //   M = B*Ho*Wo output pixels, N = Cout, K = KH*KW*Cin.   CTA tile 128 x BN, K-chunk 16, 256 threads,

@@ -1,16 +1,21 @@
-// tcgen05 implicit-GEMM convolution (stride 1) on NHWC fp32 activations with fp32-grade accuracy ("3xTF32").
+// Implicit-GEMM convolution (NHWC activations) on the Hopper tensor cores (wgmma) with fp32-grade accuracy.
 //
 //   D[m, n] = sum_{tap, c} A[pixel(m) + tap, c] * W[n, tap, c]          M = B*Ho*Wo, N = Cout, K = KH*KW*Cin
 //
-// * The tensor core (kind::tf32) reads 32-bit operands from shared memory and uses their top 19 bits.  Every value v
-//   is therefore used as  v = hi + lo  with  hi = v & 0xFFFFE000 (what the MMA sees when handed v itself) and
-//   lo = v - hi (exact in fp32, kept in a second tensor by the producer).  Three MMAs per k-step accumulate
-//   A*Whi + Alo*Whi + A*Wlo in the fp32 TMEM accumulator; the dropped Alo*Wlo term is ~2^-22 relative.
-// * No im2col: for k-block (tap, 32-channel chunk) the A operand is ONE 4-D TMA box [32 c][16 w][8 h][1 b] of the
-//   input shifted by the tap offset; conv zero padding is TMA out-of-bounds fill.  128-byte swizzle on both operands.
-// * Warp roles: warp 0 = TMA producer (one lane), warp 1 = MMA issuer (one lane) + TMEM owner, warps 2..5 = epilogue
-//   (TMEM -> registers -> bias / residual / ReLU -> value and its `lo` part -> global, channel-slice aware).
-// * One 128-pixel x BN-channel output tile per CTA; multi-stage mbarrier ring between TMA and MMA.
+// * fp16 split (the default engine, vd3d_conv2d_tc16*): every value v is kept as fp16 planes hi = rn16(v), lo = rn16(v - hi); three
+//   kind::f16 products per K step (A_lo W_hi + A_hi W_lo + A_hi W_hi) carry 22 significant bits.
+//   3xTF32 (vd3d_conv2d_tc): the tensor core reads 32-bit operands and uses their top 19 bits, so every value v is used as v = hi + lo with
+//   hi = v & 0xFFFFE000 (what the MMA sees when handed v itself) and lo = v - hi (exact in fp32, kept in a second tensor by the producer);
+//   three products A*Whi + Alo*Whi + A*Wlo, the dropped Alo*Wlo term is ~2^-22 relative.
+// * No im2col: for k-block (tap, channel chunk) the A operand is ONE 4-D TMA box [chunk][16 w][8 h][1 b] of the input shifted by the tap
+//   offset; conv zero padding is TMA out-of-bounds fill.  Swizzled K-major operands (128-byte rows; 64-byte rows for the 32-element stem window).
+// * Persistent: one CTA per SM strides over the 128-pixel x BN-channel output tiles (unit_tile: M fastest inside L2-sized M blocks).
+//   Warp 8 = TMA producer (one lane) feeding a multi-stage mbarrier ring; warps 0..7 = two consumer warpgroups.  Warpgroup w issues the
+//   wgmma of tile rows 64 w .. 64 w + 63 as soon as a stage has landed, keeps one k-block in flight, frees a stage when its MMAs are done,
+//   promotes every chunk (wg_promote) and at the end of the tile stages its accumulator in shared memory for the epilogue (tcp_store_tile),
+//   while the producer is already filling the ring with the next tile's operands.
+// * K order: channel chunk outermost, taps inside, and the same chunking for every tile width: a layer gives bit-identical results
+//   whichever tile width the host picks.
 #include "tc_conv.cuh"
 #include <unordered_map>
 #include <string>
@@ -20,453 +25,68 @@
 namespace vd3d {
 
 // ----------------------------------------------------------------------------------------------------------------
-// epilogue warps (4 warps <-> TMEM lane quadrants (warp % 4)): promote every accumulated chunk into registers, then
-// scale / bias / residual / ReLU and write the value plus the companions the next tensor-core conv reads.
-// ----------------------------------------------------------------------------------------------------------------
-template <int NG>
-__device__ __forceinline__ void tc_epilogue(const TcParams& p, uint32_t tmem_base, uint64_t* tmem_full, uint64_t* tmem_empty, int NC,
-                                            int warp, int lane, int b, int h0, int w0, int n0) {
-    const int q = warp & 3;
-    float acc[NG][32];
-#pragma unroll
-    for (int g = 0; g < NG; ++g)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[g][i] = 0.f;
-    for (int ci = 0; ci < NC; ++ci) {
-        const int buf = ci & 1, use = ci >> 1;
-        mbar_wait(&tmem_full[buf], use & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int g = 0; g < NG; ++g) {
-            if (g * 32 < p.BN) {
-                uint32_t v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * p.BN + g * 32), v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) acc[g][i] += __uint_as_float(v[i]);
-            }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty[buf])) : "memory");
-    }
-    const int r = q * 32 + lane;                   // accumulator row = tile pixel
-    const int ho = h0 + r / TC_TW, wo = w0 + r % TC_TW;
-    const bool ok = ho < p.Ho && wo < p.Wo;
-    const long long pix = ((long long)b * p.Ho + ho) * p.Wo + wo;
-    float* op = p.out + pix * p.out_cs + p.out_co;
-    float* olo = p.out_lo ? p.out_lo + pix * p.out_cs + p.out_co : nullptr;
-    __half* oh = p.out_h16_hi ? reinterpret_cast<__half*>(p.out_h16_hi) + pix * p.out_cs + p.out_co : nullptr;
-    __half* ol16 = p.out_h16_lo ? reinterpret_cast<__half*>(p.out_h16_lo) + pix * p.out_cs + p.out_co : nullptr;
-    const float osc = p.out_scale;
-    const float* rp = (p.res && !(p.dbg & 32)) ? p.res + pix * p.res_cs + p.res_co : nullptr;
-    float amax = 0.f;
-    if (ok) {
-#pragma unroll
-        for (int g = 0; g < NG; ++g) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-                const int n = n0 + g * 32 + i;
-                if (g * 32 + i < p.BN && n < p.Cout) {          // Cout % 4 == 0
-                    float4 a = make_float4(acc[g][i] * osc, acc[g][i + 1] * osc, acc[g][i + 2] * osc, acc[g][i + 3] * osc);
-                    if (p.bias) { float4 bb = ldg4(p.bias + n); a.x += bb.x; a.y += bb.y; a.z += bb.z; a.w += bb.w; }
-                    if (rp) { float4 rr = ldg4(rp + n); a.x += rr.x; a.y += rr.y; a.z += rr.z; a.w += rr.w; }
-                    if (p.relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f); }
-                    *reinterpret_cast<float4*>(op + n) = a;
-                    if (olo) {
-                        float4 l;
-                        l.x = a.x - __uint_as_float(__float_as_uint(a.x) & 0xFFFFE000u);
-                        l.y = a.y - __uint_as_float(__float_as_uint(a.y) & 0xFFFFE000u);
-                        l.z = a.z - __uint_as_float(__float_as_uint(a.z) & 0xFFFFE000u);
-                        l.w = a.w - __uint_as_float(__float_as_uint(a.w) & 0xFFFFE000u);
-                        *reinterpret_cast<float4*>(olo + n) = l;
-                    }
-                    if (oh) {      // fp16 hi/lo planes for the next fp16-split conv: hi = rn16(v), lo = rn16(v - hi)
-                        amax = amax4(amax, a);
-                        __half hx = __float2half_rn(a.x), hy = __float2half_rn(a.y), hz = __float2half_rn(a.z), hw = __float2half_rn(a.w);
-                        __half lx = __float2half_rn(a.x - __half2float(hx)), ly = __float2half_rn(a.y - __half2float(hy));
-                        __half lz = __float2half_rn(a.z - __half2float(hz)), lw = __float2half_rn(a.w - __half2float(hw));
-                        __half2 h01 = __halves2half2(hx, hy), h23 = __halves2half2(hz, hw), l01 = __halves2half2(lx, ly), l23 = __halves2half2(lz, lw);
-                        uint2 hv, lv;
-                        hv.x = *reinterpret_cast<uint32_t*>(&h01); hv.y = *reinterpret_cast<uint32_t*>(&h23);
-                        lv.x = *reinterpret_cast<uint32_t*>(&l01); lv.y = *reinterpret_cast<uint32_t*>(&l23);
-                        *reinterpret_cast<uint2*>(oh + n) = hv;
-                        *reinterpret_cast<uint2*>(ol16 + n) = lv;
-                    }
-                }
-            }
-        }
-    }
-    note_fp16_range(amax, p.range_flag);
-}
-
-// ----------------------------------------------------------------------------------------------------------------
-// kernel
-//
-// Accumulation precision: the tensor core adds every MMA result into the TMEM accumulator with truncation (measured on
-// B200: ~0.5 ulp(|acc|) of bias per accumulation, i.e. 4e-4 relative after the 4752 accumulations of a 1408-channel 3x3
-// conv).  The K loop is therefore cut into chunks of `chunk` k-blocks: each chunk is accumulated in one of TWO TMEM
-// buffers starting from zero, then "promoted": the epilogue warps read it (tcgen05.ld) and add it with round-to-nearest
-// into per-thread fp32 registers while the MMA warp is already filling the other buffer.
-// ----------------------------------------------------------------------------------------------------------------
-template <int NG>   // NG = number of 32-column groups of the accumulator held in registers (BN <= 32*NG)
-__global__ void __launch_bounds__(TC_THREADS, 1)
-conv2d_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAlo,
-                 const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // 1024-byte aligned operand ring: [stage][A | Alo | Whi | Wlo]
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t b_bytes = (uint32_t)p.BN * 128u;
-    const uint32_t stage_bytes = 2u * TC_A_BYTES + 2u * b_bytes;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* full = bars;                        // [stages]  TMA -> MMA
-    uint64_t* empty = bars + p.stages;            // [stages]  MMA -> TMA
-    uint64_t* tmem_full = bars + 2 * p.stages;    // [2]       MMA -> epilogue (chunk accumulated)
-    uint64_t* tmem_empty = tmem_full + 2;         // [2]       epilogue -> MMA (chunk promoted)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int tile = blockIdx.x;
-    const int tw = tile % p.tiles_w; tile /= p.tiles_w;
-    const int th = tile % p.tiles_h; const int b = tile / p.tiles_h;
-    const int w0 = tw * TC_TW, h0 = th * TC_TH;
-    const int n0 = blockIdx.y * p.BN;
-    const int cchunks = p.cin_pad / p.bk;
-    const int KB = p.KH * p.KW * cchunks;
-    const int NC = (KB + p.chunk - 1) / p.chunk;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {   // TMEM allocation (whole warp, .sync.aligned)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // ================= TMA producer =================
-            for (int kb = 0; kb < KB; ++kb) {
-                const int s = kb % p.stages, ph = (kb / p.stages) & 1;
-                mbar_wait(&empty[s], ph ^ 1);
-                const int tap = kb / cchunks, c0 = (kb - tap * cchunks) * p.bk;
-                const int kh = tap / p.KW, kw = tap - kh * p.KW;
-                uint8_t* st = smem + (size_t)s * stage_bytes;
-                mbar_expect_tx(&full[s], p.passes == 3 ? stage_bytes : (TC_A_BYTES + b_bytes));
-                const int wi = w0 * p.stride - p.pad + kw * p.dil, hi = h0 * p.stride - p.pad + kh * p.dil;
-                tma_load_4d(st, &mapA, &full[s], c0, wi, hi, b);
-                tma_load_2d(st + 2 * TC_A_BYTES, &mapWhi, &full[s], tap * p.cin_pad + c0, n0);
-                if (p.passes == 3) {
-                    tma_load_4d(st + TC_A_BYTES, &mapAlo, &full[s], c0, wi, hi, b);
-                    tma_load_2d(st + 2 * TC_A_BYTES + b_bytes, &mapWlo, &full[s], tap * p.cin_pad + c0, n0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ================= MMA issuer =================
-            int kb = 0;
-            for (int ci = 0; ci < NC; ++ci) {
-                const int buf = ci & 1, use = ci >> 1;
-                mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);          // the epilogue has promoted this buffer's previous chunk
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.BN);
-                const int kend = min(KB, kb + p.chunk);
-                for (bool first = true; kb < kend; ++kb) {
-                    const int s = kb % p.stages, ph = (kb / p.stages) & 1;
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-                    const uint64_t dA = make_sdesc(sa), dAlo = make_sdesc(sa + TC_A_BYTES);
-                    const uint64_t dB = make_sdesc(sa + 2 * TC_A_BYTES), dBlo = make_sdesc(sa + 2 * TC_A_BYTES + b_bytes);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t off = (uint64_t)((k * 32) >> 4);     // one MMA K-step = 32 bytes (8 tf32 / 16 fp16) inside the swizzle row
-                        if (p.f16) {
-                            if (p.passes == 3) {   // small terms first, then the main product
-                                umma_f16(d_tmem, dAlo + off, dB + off, p.idesc, first ? 0u : 1u);
-                                umma_f16(d_tmem, dA + off, dBlo + off, p.idesc, 1);
-                                umma_f16(d_tmem, dA + off, dB + off, p.idesc, 1);
-                            } else {
-                                umma_f16(d_tmem, dA + off, dB + off, p.idesc, first ? 0u : 1u);
-                            }
-                        } else if (p.passes == 3) {
-                            umma_tf32(d_tmem, dAlo + off, dB + off, p.idesc, first ? 0u : 1u);
-                            umma_tf32(d_tmem, dA + off, dBlo + off, p.idesc, 1);
-                            umma_tf32(d_tmem, dA + off, dB + off, p.idesc, 1);
-                        } else {
-                            umma_tf32(d_tmem, dA + off, dB + off, p.idesc, first ? 0u : 1u);
-                        }
-                        first = false;
-                    }
-                    umma_commit(&empty[s]);          // frees the smem stage once the MMAs above have read it
-                }
-                umma_commit(&tmem_full[buf]);        // chunk complete
-            }
-        }
-    } else {
-        tc_epilogue<NG>(p, tmem_base, tmem_full, tmem_empty, NC, warp, lane, b, h0, w0, n0);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-    }
-}
-
-// ----------------------------------------------------------------------------------------------------------------
-// Halo kernel: 3x3 / pad 1 / dilation 1 convolution on fp16 (hi, lo) operands with the A operand REUSED across taps.
-//
-// The generic kernel re-fetches the (shifted) 128-pixel A box for every tap, which makes the conv L2->shared-memory
-// bound (64 KB per k-block per CTA against ~42 B/clk/SM of L2 bandwidth).  Here the input halo of the tile is staged
-// ONCE per 64-channel chunk and the nine taps address it through shifted UMMA descriptors:
-//   h_mode 2 (full halo)   smem item = [10 halo rows][2 half rows][10 px][128 B]; (row r, half g) is one TMA box
-//                          {64 c, 10 w, 1 h}.  Tap (ky, kx) starts at ky*2560 + kx*128 and steps 1280 B per 8-pixel
-//                          group (m = r*16 + g*8 + i, as in the generic kernel).  A bytes per chunk: 200 px instead of 1152.
-//   h_mode 1 (vertical)    one item per (chunk, kx) = box {64 c, 16 w, 10 h} shifted by kx-1; tap ky starts at ky*2048,
-//                          groups 1024 B apart (every descriptor 1024-byte aligned).  480 px per chunk.
-// Swizzling is a function of the absolute shared-memory address bits for both TMA and the MMA, so 128-byte shifts of the
-// start address keep the two consistent.
-// Warp roles: 0 = A producer, 1 = MMA issuer + TMEM owner, 2..5 = epilogue, 6 = B (weights) producer; the A ring (h_sa
-// items) and the B ring (h_sb taps) are independent.
-// ----------------------------------------------------------------------------------------------------------------
-constexpr int TCH_THREADS = 224;
-constexpr int TCH_PLANE = 25600;             // bytes of one A plane item (full halo: 10 rows x 2560 B; vertical halo uses 20480 of it)
-
-template <int NG>
-__global__ void __launch_bounds__(TCH_THREADS, 1)
-conv2d_tc_halo_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAlo,
-                      const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t b_bytes = (uint32_t)p.BN * 128u;
-    const uint32_t a_item = 2u * TCH_PLANE;              // hi plane, lo plane
-    const uint32_t b_stage = 2u * b_bytes;               // Whi, Wlo
-    uint8_t* smemA = smem;
-    uint8_t* smemB = smem + (size_t)p.h_sa * a_item;     // 51200 * h_sa is a multiple of 1024
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smemB + (size_t)p.h_sb * b_stage);
-    uint64_t* fullA = bars;
-    uint64_t* emptyA = fullA + p.h_sa;
-    uint64_t* fullB = emptyA + p.h_sa;
-    uint64_t* emptyB = fullB + p.h_sb;
-    uint64_t* tmem_full = emptyB + p.h_sb;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int tile = blockIdx.x;
-    const int tw = tile % p.tiles_w; tile /= p.tiles_w;
-    const int th = tile % p.tiles_h; const int b = tile / p.tiles_h;
-    const int w0 = tw * TC_TW, h0 = th * TC_TH;
-    const int n0 = blockIdx.y * p.BN;
-    const int cchunks = p.cin_pad / 64;
-    const int items = p.h_mode == 2 ? cchunks : cchunks * 3;
-    const int KB = items * p.h_taps;                      // = 9 * cchunks
-    const int NC = (KB + p.chunk - 1) / p.chunk;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < p.h_sa; ++s) { mbar_init(&fullA[s], 1); mbar_init(&emptyA[s], 1); }
-        for (int s = 0; s < p.h_sb; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // ================= A producer: one halo item per 64-channel chunk (mode 2) or per (chunk, kx) (mode 1) =================
-            for (int it = 0; it < items; ++it) {
-                const int s = it % p.h_sa, ph = (it / p.h_sa) & 1;
-                mbar_wait(&emptyA[s], ph ^ 1);
-                uint8_t* st = smemA + (size_t)s * a_item;
-                if (p.h_mode == 2) {
-                    const int c0 = it * 64;
-                    mbar_expect_tx(&fullA[s], 2u * 20u * 1280u);
-                    for (int r = 0; r < 10; ++r)
-                        for (int g = 0; g < 2; ++g) {
-                            const uint32_t off = (uint32_t)r * 2560u + (uint32_t)g * 1280u;
-                            tma_load_4d(st + off, &mapA, &fullA[s], c0, w0 - 1 + 8 * g, h0 - 1 + r, b);
-                            tma_load_4d(st + TCH_PLANE + off, &mapAlo, &fullA[s], c0, w0 - 1 + 8 * g, h0 - 1 + r, b);
-                        }
-                } else {
-                    const int ch = it / 3, kx = it - ch * 3;
-                    mbar_expect_tx(&fullA[s], 2u * 20480u);
-                    tma_load_4d(st, &mapA, &fullA[s], ch * 64, w0 - 1 + kx, h0 - 1, b);
-                    tma_load_4d(st + TCH_PLANE, &mapAlo, &fullA[s], ch * 64, w0 - 1 + kx, h0 - 1, b);
-                }
-            }
-        }
-    } else if (warp == 6) {
-        if (lane == 0) {
-            // ================= B producer: one (tap, chunk) weight block per k-block =================
-            for (int kb = 0; kb < KB; ++kb) {
-                const int s = kb % p.h_sb, ph = (kb / p.h_sb) & 1;
-                mbar_wait(&emptyB[s], ph ^ 1);
-                const int it = kb / p.h_taps, t = kb - it * p.h_taps;
-                int tap, c0;
-                if (p.h_mode == 2) { tap = t; c0 = it * 64; }
-                else { const int ch = it / 3, kx = it - ch * 3; tap = t * 3 + kx; c0 = ch * 64; }
-                uint8_t* st = smemB + (size_t)s * b_stage;
-                mbar_expect_tx(&fullB[s], b_stage);
-                tma_load_2d(st, &mapWhi, &fullB[s], tap * p.cin_pad + c0, n0);
-                tma_load_2d(st + b_bytes, &mapWlo, &fullB[s], tap * p.cin_pad + c0, n0);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ================= MMA issuer =================
-            bool first = true;
-            for (int kb = 0; kb < KB; ++kb) {
-                const int ci = kb / p.chunk, buf = ci & 1;
-                if (kb - ci * p.chunk == 0) {
-                    mbar_wait(&tmem_empty[buf], ((ci >> 1) & 1) ^ 1);
-                    tc_fence_after();
-                    first = true;
-                }
-                const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.BN);
-                const int it = kb / p.h_taps, t = kb - it * p.h_taps;
-                const int sa = it % p.h_sa, sb = kb % p.h_sb;
-                if (t == 0) mbar_wait(&fullA[sa], (it / p.h_sa) & 1);
-                mbar_wait(&fullB[sb], (kb / p.h_sb) & 1);
-                tc_fence_after();
-                uint32_t aoff;
-                if (p.h_mode == 2) { const int ky = t / 3, kx = t - ky * 3; aoff = (uint32_t)ky * p.h_rp + (uint32_t)kx * 128u; }
-                else aoff = (uint32_t)t * p.h_rp;
-                const uint32_t a0 = smem_u32(smemA + (size_t)sa * a_item) + aoff;
-                const uint32_t b0 = smem_u32(smemB + (size_t)sb * b_stage);
-                const uint64_t dA = make_sdesc(a0, p.h_sbo), dAlo = make_sdesc(a0 + TCH_PLANE, p.h_sbo);
-                const uint64_t dB = make_sdesc(b0), dBlo = make_sdesc(b0 + b_bytes);
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const uint64_t off = (uint64_t)((k * 32) >> 4);
-                    umma_f16(d_tmem, dAlo + off, dB + off, p.idesc, first ? 0u : 1u);      // small terms first, then the main product
-                    umma_f16(d_tmem, dA + off, dBlo + off, p.idesc, 1);
-                    umma_f16(d_tmem, dA + off, dB + off, p.idesc, 1);
-                    first = false;
-                }
-                umma_commit(&emptyB[sb]);
-                if (t == p.h_taps - 1) umma_commit(&emptyA[sa]);
-                if (kb - ci * p.chunk == p.chunk - 1 || kb == KB - 1) umma_commit(&tmem_full[buf]);
-            }
-        }
-    } else {
-        tc_epilogue<NG>(p, tmem_base, tmem_full, tmem_empty, NC, warp, lane, b, h0, w0, n0);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-    }
-}
-
-
-// ----------------------------------------------------------------------------------------------------------------
 // Epilogue with the 3x3 / stride-2 / pad-1 max-pool fused in (ResNet stem: conv7x7 s2 + BN + ReLU -> MaxPool2d(3, 2, 1), resnet.py:186-189).
-// The stem output (64 ch at 1/2 resolution: 503 MB at batch 16 x 384 x 1280) is by far the largest tensor of the backbone and its only consumer is
-// the pool: here it never leaves the SM.  Per 8 x 16 tile: promote the accumulator chunks as usual, apply scale / bias / ReLU, park the 128 x 64
-// values in a shared-memory tile, then produce the pooled pixels whose 3x3 window touches the tile: 5 x 9 positions.  Positions whose window lies
-// entirely inside the tile (3 of 4 pooled rows, 7 of 8 pooled columns) are written with plain stores; the others are shared with the neighbouring
-// tile(s) and combined with atomicMax on the integer bit pattern -- exact and order-independent because ReLU makes every value >= +0 (the target
-// rows / columns are zeroed by pool_border_zero_kernel before the launch).  max() is exact, so the result equals maxpool(stem) bit for bit.
+// The stem output (64 ch at 1/2 resolution) is by far the largest tensor of the backbone and its only consumer is the pool: here it never
+// leaves the SM.  Per 8 x 16 tile: apply scale / bias / ReLU to the staged 128 x 64 accumulator in place, then produce the pooled pixels whose
+// 3x3 window touches the tile: 5 x 9 positions.  Positions whose window lies entirely inside the tile (3 of 4 pooled rows, 7 of 8 pooled
+// columns) are written with plain stores; the others are shared with the neighbouring tile(s) and combined with atomicMax on the integer bit
+// pattern -- exact and order-independent because ReLU makes every value >= +0 (the target rows / columns are zeroed by pool_border_zero_kernel
+// before the launch).  max() is exact, so the result equals maxpool(stem) bit for bit.
 // ----------------------------------------------------------------------------------------------------------------
-constexpr int POOL_LD = 68;          // floats per staged pixel row (64 + 4: conflict-free float4 rows)
+constexpr int POOL_LD = 68;          // floats per staged pixel row of the 64-column tile (64 + 4: conflict-free float4 rows)
 
-__device__ __forceinline__ void tcp_epilogue_pool(const TcParams& p, uint8_t* smem_base, uint32_t tmem_base, uint64_t* tmem_full, uint64_t* tmem_empty,
-                                                  int warp, int lane, int NC, int u0, int ustep, int units, int mt_units) {
-    const int e = warp - 2, q = warp & 3, half = e >> 2;
-    const int cb = half * 32;                                        // BN = 64: each thread owns 32 accumulator columns of one pixel
-    float* tile = reinterpret_cast<float*>(smem_base + p.pool_smem_off);
-    const uint32_t te_local = smem_u32(&tmem_empty[0]);
+__device__ __forceinline__ void tcp_pool_tile(const TcParams& p, float* tile, int u, int mt_units, int warp, int lane) {
+    const int q = warp & 3, half = warp >> 2;
+    const int cb = half * 32;                                        // each thread owns 32 accumulator columns of one pixel
     const float osc = p.out_scale;
-    const int et = e * 32 + lane;                                    // 0..255 among the epilogue threads
-    int cc = 0;
-    for (int u = u0; u < units; u += ustep) {
-        float acc[2][16];
+    const int et = warp * 32 + lane;                                 // 0..255 among the consumer threads
+    int mu, nt;
+    unit_tile(p, u, mt_units, mu, nt);
+    int mt = mu;
+    const int tw = mt % p.tiles_w; mt /= p.tiles_w;
+    const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
+    const int r = q * 32 + lane;
+    // ---- scale / bias / ReLU, in place in the staged tile ----
+    {
+        float* tp = tile + r * POOL_LD + cb;
 #pragma unroll
-        for (int g = 0; g < 2; ++g)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[g][i] = 0.f;
-        for (int ci = 0; ci < NC; ++ci, ++cc) {
-            const int buf = cc % p.nbuf, use = cc / p.nbuf;
-            mbar_wait(&tmem_full[buf], use & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int g = 0; g < 2; ++g) {
-                uint32_t v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * p.BN + cb + g * 16), v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 16; ++i) acc[g][i] += __uint_as_float(v[i]);
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(te_local + (uint32_t)buf * 8u) : "memory");
+        for (int i = 0; i < 32; i += 4) {
+            const float4 bb = p.bias ? ldg4(p.bias + cb + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const float4 v = *reinterpret_cast<const float4*>(tp + i);
+            float4 a;
+            a.x = fmaxf(v.x * osc + bb.x, 0.f); a.y = fmaxf(v.y * osc + bb.y, 0.f);
+            a.z = fmaxf(v.z * osc + bb.z, 0.f); a.w = fmaxf(v.w * osc + bb.w, 0.f);
+            *reinterpret_cast<float4*>(tp + i) = a;
         }
-        int mu, nt;
-        unit_tile(p, u, mt_units, mu, nt);
-        int mt = mu;
-        const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-        const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
-        const int r = q * 32 + lane;
-        // ---- scale / bias / ReLU, parked in the shared-memory tile ----
-        asm volatile("bar.sync 2, 256;" ::: "memory");               // the previous tile has been pooled by everyone
-        {
-            float* tp = tile + r * POOL_LD + cb;
-#pragma unroll
-            for (int g = 0; g < 2; ++g)
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const int n = cb + g * 16 + i;
-                    const float4 bb = p.bias ? ldg4(p.bias + n) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    float4 a;
-                    a.x = fmaxf(acc[g][i] * osc + bb.x, 0.f); a.y = fmaxf(acc[g][i + 1] * osc + bb.y, 0.f);
-                    a.z = fmaxf(acc[g][i + 2] * osc + bb.z, 0.f); a.w = fmaxf(acc[g][i + 3] * osc + bb.w, 0.f);
-                    *reinterpret_cast<float4*>(tp + g * 16 + i) = a;
-                }
-        }
-        asm volatile("bar.sync 2, 256;" ::: "memory");
-        // ---- pooled positions touched by this tile: rows i0 .. i0 + 4, columns j0 .. j0 + 8 ----
-        const int h0 = th * TC_TH, w0 = tw * TC_TW, i0 = th * (TC_TH / 2), j0 = tw * (TC_TW / 2);
-        for (int item = et; item < 45 * 16; item += 256) {
-            const int cq = item & 15, pp = item >> 4;
-            const int pi = pp / 9, pj = pp - pi * 9;
-            const int i = i0 + pi, j = j0 + pj;
-            if (i >= p.pool_H || j >= p.pool_W) continue;
-            // window rows / columns in tile coordinates, clipped to the tile and to the conv output
-            int r_lo = 2 * pi - 1, r_hi = 2 * pi + 1, c_lo = 2 * pj - 1, c_hi = 2 * pj + 1;
-            const int r_max = min(TC_TH - 1, p.Ho - 1 - h0), c_max = min(TC_TW - 1, p.Wo - 1 - w0);
-            // complete: every window row / column that exists in the conv output lies inside this tile
-            const bool complete = (r_lo >= 0 || h0 + r_lo < 0) && (2 * pi <= r_max || h0 + 2 * pi > p.Ho - 1) && (r_hi <= r_max || h0 + r_hi > p.Ho - 1) &&
-                                  (c_lo >= 0 || w0 + c_lo < 0) && (2 * pj <= c_max || w0 + 2 * pj > p.Wo - 1) && (c_hi <= c_max || w0 + c_hi > p.Wo - 1);
-            r_lo = max(r_lo, 0); c_lo = max(c_lo, 0); r_hi = min(r_hi, r_max); c_hi = min(c_hi, c_max);
-            if (r_lo > r_hi || c_lo > c_hi) continue;
-            float4 m = make_float4(0.f, 0.f, 0.f, 0.f);             // values are >= 0 after the ReLU
-            for (int rr = r_lo; rr <= r_hi; ++rr)
-                for (int c2 = c_lo; c2 <= c_hi; ++c2) {
-                    const float4 v = *reinterpret_cast<const float4*>(tile + (rr * TC_TW + c2) * POOL_LD + cq * 4);
-                    m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
-                }
-            float* op = p.pool_out + (((long long)b * p.pool_H + i) * p.pool_W + j) * p.pool_cs + p.pool_co + cq * 4;
-            if (complete) *reinterpret_cast<float4*>(op) = m;
-            else {
-                int* ip = reinterpret_cast<int*>(op);
-                atomicMax(ip, __float_as_int(m.x)); atomicMax(ip + 1, __float_as_int(m.y));
-                atomicMax(ip + 2, __float_as_int(m.z)); atomicMax(ip + 3, __float_as_int(m.w));
+    }
+    consumers_sync();
+    // ---- pooled positions touched by this tile: rows i0 .. i0 + 4, columns j0 .. j0 + 8 ----
+    const int h0 = th * TC_TH, w0 = tw * TC_TW, i0 = th * (TC_TH / 2), j0 = tw * (TC_TW / 2);
+    for (int item = et; item < 45 * 16; item += TC_CONSUMERS) {
+        const int cq = item & 15, pp = item >> 4;
+        const int pi = pp / 9, pj = pp - pi * 9;
+        const int i = i0 + pi, j = j0 + pj;
+        if (i >= p.pool_H || j >= p.pool_W) continue;
+        // window rows / columns in tile coordinates, clipped to the tile and to the conv output
+        int r_lo = 2 * pi - 1, r_hi = 2 * pi + 1, c_lo = 2 * pj - 1, c_hi = 2 * pj + 1;
+        const int r_max = min(TC_TH - 1, p.Ho - 1 - h0), c_max = min(TC_TW - 1, p.Wo - 1 - w0);
+        // complete: every window row / column that exists in the conv output lies inside this tile
+        const bool complete = (r_lo >= 0 || h0 + r_lo < 0) && (2 * pi <= r_max || h0 + 2 * pi > p.Ho - 1) && (r_hi <= r_max || h0 + r_hi > p.Ho - 1) &&
+                              (c_lo >= 0 || w0 + c_lo < 0) && (2 * pj <= c_max || w0 + 2 * pj > p.Wo - 1) && (c_hi <= c_max || w0 + c_hi > p.Wo - 1);
+        r_lo = max(r_lo, 0); c_lo = max(c_lo, 0); r_hi = min(r_hi, r_max); c_hi = min(c_hi, c_max);
+        if (r_lo > r_hi || c_lo > c_hi) continue;
+        float4 m = make_float4(0.f, 0.f, 0.f, 0.f);             // values are >= 0 after the ReLU
+        for (int rr = r_lo; rr <= r_hi; ++rr)
+            for (int c2 = c_lo; c2 <= c_hi; ++c2) {
+                const float4 v = *reinterpret_cast<const float4*>(tile + (rr * TC_TW + c2) * POOL_LD + cq * 4);
+                m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
             }
+        float* op = p.pool_out + (((long long)b * p.pool_H + i) * p.pool_W + j) * p.pool_cs + p.pool_co + cq * 4;
+        if (complete) *reinterpret_cast<float4*>(op) = m;
+        else {
+            int* ip = reinterpret_cast<int*>(op);
+            atomicMax(ip, __float_as_int(m.x)); atomicMax(ip + 1, __float_as_int(m.y));
+            atomicMax(ip + 2, __float_as_int(m.z)); atomicMax(ip + 3, __float_as_int(m.w));
         }
     }
 }
@@ -484,475 +104,128 @@ __global__ void pool_border_zero_kernel(float* __restrict__ out, int B, int Hp, 
 }
 
 // ----------------------------------------------------------------------------------------------------------------
-// Persistent kernel (fp16 hi/lo operands; the default engine).
-//
-// One CTA per SM (CG = 1) or one CTA pair per TPC (CG = 2: cta_group::2, UMMA M = 256, every CTA stages its own 128
-// pixels of A and HALF of the weight tile, so the tensor core of each SM reads 6 KB instead of 8 KB of operands per
-// MMA and the TMA writes 48 KB instead of 64 KB per k-block: the kernel is shared-memory-bandwidth bound).
-// Tiles are taken round-robin (M fastest, so concurrently running CTAs share one weight tile in L2).  The TMA->MMA
-// ring and the chunked TMEM promotion run across tile boundaries: while the eight epilogue warps write tile i to
-// global memory the MMA warp is already accumulating the first two chunks of tile i+1.
-// Warp roles: 0 = TMA producer, 1 = MMA issuer (leader CTA only) + TMEM owner, 2..9 = epilogue; epilogue warp e works
-// on TMEM lane quadrant (warp % 4) and on column half e / 4 of the BN accumulator columns.
+// Persistent kernel.  Shared memory: [stages][A hi | A lo | W hi | W lo] operand ring, the [128][BN + 4] fp32 staged accumulator, barriers.
 // ----------------------------------------------------------------------------------------------------------------
-template <int NG16, int CG, int PL>   // NG16 = 16-column groups per epilogue thread (>= ceil(BN / 32)); CG = CTAs per MMA (1 or 2); PL: see tcp_epilogue
+constexpr int TCP_THREADS = TC_CONSUMERS + 32;      // warps 0..7 = consumers, warp 8 = TMA producer
+
+template <int BN, bool F16>
 __global__ void __launch_bounds__(TCP_THREADS, 1)
 conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t bnl = (uint32_t)p.BN / CG;                      // weight rows staged by this CTA
-    const uint32_t rowb = (uint32_t)p.rowb;                        // 128 (SWIZZLE_128B, 64 channels per k-block) or 64 (SWIZZLE_64B, 32)
+    constexpr int LD = BN + 4;
+    const uint32_t rowb = (uint32_t)p.rowb;                        // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
     const uint32_t a_bytes = 128u * rowb;                          // one A plane of a stage: 128 pixel rows
-    const uint32_t b_bytes = bnl * rowb;
+    const uint32_t b_bytes = (uint32_t)BN * rowb;
     const uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;      // [A hi | A lo | W hi | W lo]
-    const int kbc = (int)rowb / 2;                                 // channels per k-block
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* full = bars;                        // [stages]  TMA -> MMA (leader's copy is the live one when CG = 2)
-    uint64_t* empty = bars + p.stages;            // [stages]  MMA -> TMA (multicast to both CTAs)
-    uint64_t* tmem_full = bars + 2 * p.stages;    // [2]       MMA -> epilogue (multicast)
-    uint64_t* tmem_empty = tmem_full + 4;         // [nbuf <= 4] epilogue -> MMA (leader's copy, 8 * CG arrivals)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
+    const int kbc = (int)rowb / (F16 ? 2 : 4);                     // channels per k-block
+    float* tile = reinterpret_cast<float*>(smem + (size_t)p.stages * stage_bytes);
+    uint64_t* full = reinterpret_cast<uint64_t*>(tile + 128 * LD);  // [stages]  TMA -> consumers
+    uint64_t* empty = full + p.stages;                              // [stages]  consumers (8 warps) -> TMA
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;      // (warp-uniform for the compiler)
     const int cchunks = p.cin_pad / kbc;
     const int KB = p.KH * p.KW * cchunks;
-    const int NC = (KB + p.chunk - 1) / p.chunk;
-    const int mt_units = (p.m_tiles + CG - 1) / CG;            // scheduling units along M (tiles or tile pairs)
+    const int mt_units = p.m_tiles;
     const int units = mt_units * p.n_tiles;
-    const int u0 = (int)blockIdx.x / CG, ustep = (int)gridDim.x / CG;
+    const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
+    const int mode = tc_mma_mode(p);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int i = 0; i < 4; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 8 * CG); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], TC_CONSUMERS / 32); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {   // TMEM allocation (whole warp; with CG = 2 the same warp of both CTAs)
-        if (CG == 2) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CG == 2) cluster_sync_all();      // the peer's barriers are initialised before anything arrives on them
-    tc_fence_after();
-    // REDUX puts the (identical) value in a uniform register: the MMA issue loop then needs no per-instruction lane-broadcast of the
-    // accumulator address (measured: ~90 -> ~25 clk of issue time per tcgen05.mma)
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, *tmem_slot);
     pdl_launch_dependents();
     pdl_wait();                            // (PDL launches only) the producer of the activations / residual has completed
 
-    if (warp == 0) {
-        {
-            // ================= TMA producer (both CTAs of a pair): the whole warp walks the ring, one elected lane issues =================
+    if (warp == TC_CONSUMERS / 32) {
+        if (lane == 0) {
+            // ================= TMA producer =================
+            const bool lo_too = mode != 1 && !(p.dbg & 2);
+            const uint32_t tx = lo_too ? stage_bytes : a_bytes + b_bytes;
             int it = 0, s = 0, ph = 0;
             for (int u = u0; u < units; u += ustep) {
                 int mu, nt;
                 unit_tile(p, u, mt_units, mu, nt);
-                int mt = mu * CG + (int)rank;
-                const bool live = mt < p.m_tiles;
+                int mt = mu;
                 const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-                const int th = mt % p.tiles_h; const int b = live ? mt / p.tiles_h : p.B;      // dead half of an odd pair: out-of-range batch -> zero fill
+                const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
                 const int wi0 = tw * TC_TW * p.stride_w - p.pad_w, hi0 = th * TC_TH * p.stride - p.pad;
-                const int nvalid = min(p.BN, p.cout_pad - nt * p.BN);                  // ragged last N tile (multiple of 16)
-                const int n0 = nt * p.BN + (int)rank * (nvalid / CG);                  // this CTA's weight rows start here (the box holds BN / CG rows)
+                const int n0 = nt * BN;
                 int tap = 0, kh = 0, kw = 0, c0 = 0;
                 for (int kb = 0; kb < KB; ++kb, ++it) {
                     mbar_wait(&empty[s], ph ^ 1);
                     const bool tr = p.trace && blockIdx.x == 0 && it < p.trace_n;
-                    if (elect_one()) {
                     if (tr) p.trace[it] = clock64();                                          // [0] stage free, about to issue the loads
                     uint8_t* st = smem + (size_t)s * stage_bytes;
                     const int wi = wi0 + kw * p.dil, hi = hi0 + kh * p.dil;
                     const int kcol = tap * p.cin_pad + c0;
-                    const bool lo_too = !(p.dbg & 2);
-                    const uint32_t tx = lo_too ? stage_bytes : stage_bytes / 2;
-                    if (CG == 2) {
-                        const uint32_t lbar = mapa_shared(smem_u32(&full[s]), 0);
-                        if (rank == 0) mbar_expect_tx(&full[s], 2u * tx);
-                        tma_load_4d_2sm(st, &mapA, lbar, c0, wi, hi, b);
-                        if (lo_too) tma_load_4d_2sm(st + a_bytes, &mapAlo, lbar, c0, wi, hi, b);
-                        tma_load_2d_2sm(st + 2 * a_bytes, &mapWhi, lbar, kcol, n0);
-                        if (lo_too) tma_load_2d_2sm(st + 2 * a_bytes + b_bytes, &mapWlo, lbar, kcol, n0);
-                    } else {
-                        mbar_expect_tx(&full[s], tx);
-                        tma_load_4d(st, &mapA, &full[s], c0, wi, hi, b);
-                        if (lo_too) tma_load_4d(st + a_bytes, &mapAlo, &full[s], c0, wi, hi, b);
-                        tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[s], kcol, n0);
-                        if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[s], kcol, n0);
-                    }
+                    mbar_expect_tx(&full[s], tx);
+                    tma_load_4d(st, &mapA, &full[s], c0, wi, hi, b);
+                    if (lo_too) tma_load_4d(st + a_bytes, &mapAlo, &full[s], c0, wi, hi, b);
+                    tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[s], kcol, n0);
+                    if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[s], kcol, n0);
                     if (tr) p.trace[p.trace_n + it] = clock64();                              // [1] loads issued
-                    }
-                    __syncwarp();
                     if (++s == p.stages) { s = 0; ph ^= 1; }
-                    // k-block order: channel chunk outermost, taps inside (the same order as the halo kernel, so both accumulate
-                    // identically and a layer gives bit-identical results whichever of the two the tile policy picks)
-                    if (p.dbg & 8) {          // timing experiment: taps outermost (the results then differ from the halo kernel's in the last bit)
-                        c0 += kbc;
-                        if (c0 == p.cin_pad) { c0 = 0; ++tap; if (++kw == p.KW) { kw = 0; ++kh; } }
-                    } else {
-                        ++tap;
-                        if (++kw == p.KW) { kw = 0; ++kh; }
-                        if (tap == p.KH * p.KW) { tap = 0; kh = 0; kw = 0; c0 += kbc; }
-                    }
+                    // k-block order: channel chunk outermost, taps inside
+                    ++tap;
+                    if (++kw == p.KW) { kw = 0; ++kh; }
+                    if (tap == p.KH * p.KW) { tap = 0; kh = 0; kw = 0; c0 += kbc; }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (rank == 0 && elect_one()) {
-            // ================= MMA issuer (leader CTA, one elected lane) =================
-            // Software-pipelined over the flat sequence of k-blocks of all tiles of this CTA: the barrier wait, fence and descriptor
-            // set-up of k-block g+1 sit BETWEEN the two halves of the MMAs of k-block g, where the tensor core still has queued work
-            // (issue is blocking and the queue is shallow: anything between the last MMA of g and the first of g+1 is a bubble).
-            const int my_units = (units - u0 + ustep - 1) / ustep;           // tiles of this CTA (>= 1: the grid never exceeds the tile count)
-            const long long total = (long long)my_units * KB;
-            const int mma_mode = (p.dbg & 1) ? 1 : (p.two_pass ? 3 : 0);      // 0 = production
-            int s = 0, ph = 0, cc = 0;
-            auto stage_desc = [&](int st, uint64_t& dA, uint64_t& dAlo, uint64_t& dB, uint64_t& dBlo) {
-                const uint32_t sa = smem_u32(smem + (size_t)st * stage_bytes);
-                const uint32_t sbo = 8u * rowb, lay = rowb == 128u ? 2u : 4u;
-                dA = make_sdesc(sa, sbo, lay); dAlo = make_sdesc(sa + a_bytes, sbo, lay);
-                dB = make_sdesc(sa + 2 * a_bytes, sbo, lay); dBlo = make_sdesc(sa + 2 * a_bytes + b_bytes, sbo, lay);
-            };
-            auto tile_idesc = [&](int unit_local) {
-                const int u = u0 + unit_local * ustep;
-                const int nvalid = min(p.BN, p.cout_pad - unit_nt(p, u, mt_units) * p.BN);
-                return (p.idesc & ~(0x3Fu << 17)) | ((uint32_t)(nvalid >> 3) << 17);      // MMA N = valid columns of the tile
-            };
-            auto issue = [&](uint32_t d_tmem, uint32_t idesc, uint64_t dA, uint64_t dAlo, uint64_t dB, uint64_t dBlo, int k, uint32_t acc0) {
-                const uint64_t off = (uint64_t)((k * 32) >> 4);       // one MMA K-step = 16 fp16 = 32 bytes inside the swizzle row
-                if (mma_mode != 0) {          // experiments (results differ): 1 = one MMA per K step, 3 = two passes
-                    if (mma_mode == 1) {
-                        if (CG == 2) umma_f16_2sm(d_tmem, dA + off, dB + off, idesc, acc0); else umma_f16(d_tmem, dA + off, dB + off, idesc, acc0);
-                    } else if (CG == 2) { umma_f16_2sm(d_tmem, dA + off, dBlo + off, idesc, acc0); umma_f16_2sm(d_tmem, dA + off, dB + off, idesc, 1); }
-                    else { umma_f16(d_tmem, dA + off, dBlo + off, idesc, acc0); umma_f16(d_tmem, dA + off, dB + off, idesc, 1); }
-                } else if (CG == 2) {
-                    umma_f16_2sm(d_tmem, dAlo + off, dB + off, idesc, acc0);      // small terms first, then the main product
-                    umma_f16_2sm(d_tmem, dA + off, dBlo + off, idesc, 1);
-                    umma_f16_2sm(d_tmem, dA + off, dB + off, idesc, 1);
-                } else {
-                    umma_f16(d_tmem, dAlo + off, dB + off, idesc, acc0);
-                    umma_f16(d_tmem, dA + off, dBlo + off, idesc, 1);
-                    umma_f16(d_tmem, dA + off, dB + off, idesc, 1);
-                }
-            };
-            // prologue: first accumulator buffer and first stage
-            mbar_wait(&tmem_empty[0], 1);
-            mbar_wait(&full[0], 0);
-            tc_fence_after();
-            uint64_t dA, dAlo, dB, dBlo;
-            stage_desc(0, dA, dAlo, dB, dBlo);
-            uint32_t idesc = tile_idesc(0);
-            int kb = 0, unit_local = 0;
-            for (long long g = 0; g < total; ++g) {
-                const int buf = cc % p.nbuf;
-                const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.BN);
-                const bool first_in_chunk = (kb % p.chunk) == 0;
-                const bool last_in_chunk = (kb % p.chunk) == p.chunk - 1 || kb == KB - 1;
-                const bool tr = p.trace && blockIdx.x == 0 && g < p.trace_n;
-                if (tr) p.trace[3 * p.trace_n + g] = clock64();                               // [3] about to issue k-block g
-                issue(d_tmem, idesc, dA, dAlo, dB, dBlo, 0, first_in_chunk ? 0u : 1u);
-                if (rowb == 128u) issue(d_tmem, idesc, dA, dAlo, dB, dBlo, 1, 1u);
-                // ---- look-ahead for k-block g+1 while the MMAs above are queued ----
-                const int s_cur = s;
-                uint64_t nA = 0, nAlo = 0, nB = 0, nBlo = 0;
-                const bool has_next = g + 1 < total;
-                if (has_next) {
-                    if (++s == p.stages) { s = 0; ph ^= 1; }
-                    if (tr) p.trace[2 * p.trace_n + g] = clock64();                           // [2] look-ahead wait starts
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    stage_desc(s, nA, nAlo, nB, nBlo);
-                }
-                if (rowb == 128u) {
-                    issue(d_tmem, idesc, dA, dAlo, dB, dBlo, 2, 1u);
-                    issue(d_tmem, idesc, dA, dAlo, dB, dBlo, 3, 1u);
-                } else {
-                    issue(d_tmem, idesc, dA, dAlo, dB, dBlo, 1, 1u);      // 64-byte rows: two K steps per k-block
-                }
-                if (CG == 2) umma_commit_2sm(&empty[s_cur]); else umma_commit(&empty[s_cur]);       // frees the stage (in both CTAs)
-                if (tr) p.trace[4 * p.trace_n + g] = clock64();                               // [4] MMAs + commit issued
-                if (last_in_chunk) {
-                    if (CG == 2) umma_commit_2sm(&tmem_full[buf]); else umma_commit(&tmem_full[buf]);
-                    ++cc;
-                    if (has_next) {
-                        const int nbuf = cc % p.nbuf, use = cc / p.nbuf;
-                        mbar_wait(&tmem_empty[nbuf], (use & 1) ^ 1);     // every epilogue warp has promoted this buffer's previous chunk
-                        tc_fence_after();
-                    }
-                }
-                if (++kb == KB) { kb = 0; ++unit_local; if (has_next) idesc = tile_idesc(unit_local); }
-                dA = nA; dAlo = nAlo; dB = nB; dBlo = nBlo;
-            }
-        }
-        __syncwarp();
     } else {
-        if constexpr (NG16 == 2 && CG == 1 && PL == 0) {
-            if (p.pool_out) tcp_epilogue_pool(p, smem, tmem_base, tmem_full, tmem_empty, warp, lane, NC, u0, ustep, units, mt_units);
-            else tcp_epilogue<NG16, CG, PL>(p, tmem_base, tmem_full, tmem_empty, warp, lane, rank, NC, u0, ustep, units, mt_units);
-        } else {
-            tcp_epilogue<NG16, CG, PL>(p, tmem_base, tmem_full, tmem_empty, warp, lane, rank, NC, u0, ustep, units, mt_units);
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (CG == 2) cluster_sync_all();      // no remote arrive / multicast commit may land in a CTA that has already exited
-    if (warp == 1) {
-        tc_fence_after();
-        if (CG == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-    }
-}
-
-// ----------------------------------------------------------------------------------------------------------------
-// Persistent halo kernel: 3x3 / stride 1 / pad 1 / dilation 1 convolutions (most of the network) with the A operand
-// staged ONCE per 64-channel chunk and reused by the nine taps (layout and descriptor arithmetic of conv2d_tc_halo_kernel,
-// h_mode 2), inside the persistent / paired structure of conv2d_tcp_kernel.
-//   A item  = [hi plane | lo plane], plane = [10 halo rows][2 half rows][10 px][128 B]; (row r, half g) is one TMA box
-//             {64 c, 10 w, 1 h} at pixel (w0 - 1 + 8g, h0 - 1 + r).  Tap (ky, kx) reads it through a descriptor that starts
-//             at ky*2560 + kx*128 and steps 1280 B per 8-pixel group.  200 px per chunk instead of 9 x 128.
-//   B stage = [W hi | W lo] of one (chunk, tap): BN / CG rows x 128 B each, own ring (warp 10 is its producer).
-// Operand bytes per 128 x 128 x 64 x 9-tap unit of work: 51 KB (A) + 9 x 32 KB / (CG * BN / 128) (W), against 9 x 64 KB.
-// ----------------------------------------------------------------------------------------------------------------
-constexpr int TCPH_THREADS = 352;            // warps: 0 = A producer, 1 = MMA, 2..9 = epilogue, 10 = W producer
-constexpr int TCPH_PLANE = 25600;
-constexpr int TCPH_XPLANE = 18 * 10 * 128;   // x-major item: 18 columns x 10 rows x 128 B (fits in the same plane slot)
-constexpr int TCPH_ITEM = 2 * TCPH_PLANE;
-
-template <int NG16, int CG, int PL>
-__global__ void __launch_bounds__(TCPH_THREADS, 1)
-conv2d_tcph_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAlo,
-                   const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t bnl = (uint32_t)p.BN / CG;
-    const uint32_t b_bytes = bnl * 128u;
-    const uint32_t b_stage = 2u * b_bytes;
-    uint8_t* smemA = smem;
-    uint8_t* smemB = smem + (size_t)p.h_sa * TCPH_ITEM;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smemB + (size_t)p.h_sb * b_stage);
-    uint64_t* fullA = bars;
-    uint64_t* emptyA = fullA + p.h_sa;
-    uint64_t* fullB = emptyA + p.h_sa;
-    uint64_t* emptyB = fullB + p.h_sb;
-    uint64_t* tmem_full = emptyB + p.h_sb;
-    uint64_t* tmem_empty = tmem_full + 4;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;
-    const int cchunks = p.cin_pad / 64;
-    const int KB = 9 * cchunks;
-    const int NC = (KB + p.chunk - 1) / p.chunk;
-    const int mt_units = (p.m_tiles + CG - 1) / CG;
-    const int units = mt_units * p.n_tiles;
-    const int u0 = (int)blockIdx.x / CG, ustep = (int)gridDim.x / CG;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < p.h_sa; ++s) { mbar_init(&fullA[s], 1); mbar_init(&emptyA[s], 1); }
-        for (int s = 0; s < p.h_sb; ++s) { mbar_init(&fullB[s], 1); mbar_init(&emptyB[s], 1); }
-        for (int i = 0; i < 4; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 8 * CG); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        if (CG == 2) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (CG == 2) cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, *tmem_slot);      // uniform register (see conv2d_tcp_kernel)
-    pdl_launch_dependents();
-    pdl_wait();
-
-    if (warp == 0) {
-        if (elect_one()) {
-            // ================= A producer (one elected lane): one halo item per (tile, 64-channel chunk) =================
-            int it = 0;
-            for (int u = u0; u < units; u += ustep) {
-                int mu, nt_unused;
-                unit_tile(p, u, mt_units, mu, nt_unused);
-                int mt = mu * CG + (int)rank;
-                const bool live = mt < p.m_tiles;
-                const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-                const int th = mt % p.tiles_h; const int b = live ? mt / p.tiles_h : p.B;
-                const int w0 = tw * TC_TW, h0 = th * TC_TH;
-                for (int ch = 0; ch < cchunks; ++ch, ++it) {
-                    const int s = it % p.h_sa, ph = (it / p.h_sa) & 1;
-                    mbar_wait(&emptyA[s], ph ^ 1);
-                    uint8_t* st = smemA + (size_t)s * TCPH_ITEM;
-                    const int c0 = ch * 64;
-                    if (p.m_xmajor) {
-                        // x-major item: ONE box {64 c, 10 h, 18 w} per plane (the tensor map lists h before w), written as [18 x][10 rows][128 B]:
-                        // 2 TMA operations of 23 KB per (tile, chunk) instead of 40 of 1.25 KB
-                        const bool lo_too = !(p.dbg & 2);
-                        const uint32_t bytes = lo_too ? 2u * TCPH_XPLANE : (uint32_t)TCPH_XPLANE;
-                        if (CG == 2) {
-                            const uint32_t lbar = mapa_shared(smem_u32(&fullA[s]), 0);
-                            if (rank == 0) mbar_expect_tx(&fullA[s], 2u * bytes);
-                            tma_load_4d_2sm(st, &mapA, lbar, c0, h0 - 1, w0 - 1, b);
-                            if (lo_too) tma_load_4d_2sm(st + TCPH_PLANE, &mapAlo, lbar, c0, h0 - 1, w0 - 1, b);
-                        } else {
-                            mbar_expect_tx(&fullA[s], bytes);
-                            tma_load_4d(st, &mapA, &fullA[s], c0, h0 - 1, w0 - 1, b);
-                            if (lo_too) tma_load_4d(st + TCPH_PLANE, &mapAlo, &fullA[s], c0, h0 - 1, w0 - 1, b);
-                        }
-                    } else if (CG == 2) {
-                        const uint32_t lbar = mapa_shared(smem_u32(&fullA[s]), 0);
-                        const bool lo_too = !(p.dbg & 2);
-                        if (rank == 0) mbar_expect_tx(&fullA[s], lo_too ? 2u * TCPH_ITEM : (uint32_t)TCPH_ITEM);
-                        for (int r = 0; r < 10; ++r)
-                            for (int g = 0; g < 2; ++g) {
-                                const uint32_t off = (uint32_t)r * 2560u + (uint32_t)g * 1280u;
-                                tma_load_4d_2sm(st + off, &mapA, lbar, c0, w0 - 1 + 8 * g, h0 - 1 + r, b);
-                                if (lo_too) tma_load_4d_2sm(st + TCPH_PLANE + off, &mapAlo, lbar, c0, w0 - 1 + 8 * g, h0 - 1 + r, b);
-                            }
-                    } else {
-                        mbar_expect_tx(&fullA[s], TCPH_ITEM);
-                        for (int r = 0; r < 10; ++r)
-                            for (int g = 0; g < 2; ++g) {
-                                const uint32_t off = (uint32_t)r * 2560u + (uint32_t)g * 1280u;
-                                tma_load_4d(st + off, &mapA, &fullA[s], c0, w0 - 1 + 8 * g, h0 - 1 + r, b);
-                                tma_load_4d(st + TCPH_PLANE + off, &mapAlo, &fullA[s], c0, w0 - 1 + 8 * g, h0 - 1 + r, b);
-                            }
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 10) {
-        if (elect_one()) {
-            // ================= W producer (one elected lane): one (chunk, tap) weight block per k-block =================
-            int it = 0;
-            if (p.w_res) {
-                // weight-resident mode (one N tile, 9 * cchunks weight blocks fit next to the two A items): every block is loaded ONCE per CTA
-                const int n0 = (int)rank * (min(p.BN, p.cout_pad) / CG);
-                const uint32_t lbar = CG == 2 ? mapa_shared(smem_u32(&fullB[0]), 0) : 0u;
-                if (rank == 0) mbar_expect_tx(&fullB[0], (uint32_t)CG * (uint32_t)KB * b_stage);
-                for (int kb = 0; kb < KB; ++kb) {
-                    const int ch = kb / 9, tap = kb - ch * 9;
-                    const int kcol = tap * p.cin_pad + ch * 64;
-                    uint8_t* st = smemB + (size_t)kb * b_stage;
-                    if (CG == 2) { tma_load_2d_2sm(st, &mapWhi, lbar, kcol, n0); tma_load_2d_2sm(st + b_bytes, &mapWlo, lbar, kcol, n0); }
-                    else { tma_load_2d(st, &mapWhi, &fullB[0], kcol, n0); tma_load_2d(st + b_bytes, &mapWlo, &fullB[0], kcol, n0); }
-                }
-            } else
-            for (int u = u0; u < units; u += ustep) {
-                const int nt = unit_nt(p, u, mt_units);
-                const int nvalid = min(p.BN, p.cout_pad - nt * p.BN);
-                const int n0 = nt * p.BN + (int)rank * (nvalid / CG);
-                for (int kb = 0; kb < KB; ++kb, ++it) {
-                    const int s = it % p.h_sb, ph = (it / p.h_sb) & 1;
-                    mbar_wait(&emptyB[s], ph ^ 1);
-                    const int ch = kb / 9, tap = kb - ch * 9;
-                    const int kcol = tap * p.cin_pad + ch * 64;
-                    uint8_t* st = smemB + (size_t)s * b_stage;
-                    if (CG == 2) {
-                        const uint32_t lbar = mapa_shared(smem_u32(&fullB[s]), 0);
-                        const bool lo_too = !(p.dbg & 2);
-                        if (rank == 0) mbar_expect_tx(&fullB[s], lo_too ? 2u * b_stage : b_stage);
-                        tma_load_2d_2sm(st, &mapWhi, lbar, kcol, n0);
-                        if (lo_too) tma_load_2d_2sm(st + b_bytes, &mapWlo, lbar, kcol, n0);
-                    } else {
-                        mbar_expect_tx(&fullB[s], b_stage);
-                        tma_load_2d(st, &mapWhi, &fullB[s], kcol, n0);
-                        tma_load_2d(st + b_bytes, &mapWlo, &fullB[s], kcol, n0);
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (rank == 0 && elect_one()) {
-            // ================= MMA issuer (leader CTA, one elected lane) =================
-            int ita = 0, itb = 0, cc = 0;
-            const int mma_mode = (p.dbg & 1) ? 1 : ((p.dbg & 64) ? 2 : (p.two_pass ? 3 : 0));      // 0 = production (hoisted: the issue loop tests one register)
-            if (p.w_res) { mbar_wait(&fullB[0], 0); tc_fence_after(); }
-            for (int u = u0; u < units; u += ustep) {
-                const int nvalid = min(p.BN, p.cout_pad - unit_nt(p, u, mt_units) * p.BN);
-                const uint32_t idesc = (p.idesc & ~(0x3Fu << 17)) | ((uint32_t)(nvalid >> 3) << 17);
-                bool first = true;
-                for (int kb = 0; kb < KB; ++kb, ++itb) {
-                    const int ci = kb / p.chunk;
-                    const int buf = (cc + ci) % p.nbuf;
-                    if (kb - ci * p.chunk == 0) {
-                        mbar_wait(&tmem_empty[buf], (((cc + ci) / p.nbuf) & 1) ^ 1);
-                        tc_fence_after();
-                        first = true;
-                    }
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.BN);
-                    const int ch = kb / 9, t = kb - ch * 9;
-                    const int sa = (ita + ch) % p.h_sa, sb = p.w_res ? kb : itb % p.h_sb;
-                    if (t == 0) mbar_wait(&fullA[sa], ((ita + ch) / p.h_sa) & 1);
-                    if (!p.w_res) mbar_wait(&fullB[sb], (itb / p.h_sb) & 1);
-                    tc_fence_after();
-                    const int ky = t / 3, kx = t - ky * 3;
-                    const uint32_t a0 = smem_u32(smemA + (size_t)sa * TCPH_ITEM) +
-                                        (p.m_xmajor ? (uint32_t)kx * 1280u + (uint32_t)ky * 128u : (uint32_t)ky * 2560u + (uint32_t)kx * 128u);
-                    const uint32_t b0 = smem_u32(smemB + (size_t)sb * b_stage);
-                    const uint64_t dA = make_sdesc(a0, 1280), dAlo = make_sdesc(a0 + TCPH_PLANE, 1280);
-                    const uint64_t dB = make_sdesc(b0), dBlo = make_sdesc(b0 + b_bytes);
-                    if (mma_mode == 0) {
-                        // the production path: three back-to-back MMAs per K step, nothing else in the issue loop
+        // ================= consumer warpgroups: MMAs, chunk promotion, epilogue =================
+        const int wg = warp >> 2;
+        const uint32_t sbo = 8u * rowb, lay = rowb == 128u ? 2u : 4u;
+        const int ksteps = (int)rowb / 32;
+        const bool tr0 = p.trace && blockIdx.x == 0 && threadIdx.x == 0;
+        auto release = [&](int st) {
+            __syncwarp();
+            if (st >= 0 && lane == 0) mbar_arrive(&empty[st]);
+        };
+        float tot[BN / 2], c[BN / 2];
+        float amax = 0.f;
+        int s = 0, ph = 0, g = 0;
+        for (int u = u0; u < units; u += ustep) {
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t off = (uint64_t)((k * 32) >> 4);
-                            if (CG == 2) {
-                                umma_f16_2sm(d_tmem, dAlo + off, dB + off, idesc, first ? 0u : 1u);
-                                umma_f16_2sm(d_tmem, dA + off, dBlo + off, idesc, 1);
-                                umma_f16_2sm(d_tmem, dA + off, dB + off, idesc, 1);
-                            } else {
-                                umma_f16(d_tmem, dAlo + off, dB + off, idesc, first ? 0u : 1u);
-                                umma_f16(d_tmem, dA + off, dBlo + off, idesc, 1);
-                                umma_f16(d_tmem, dA + off, dB + off, idesc, 1);
-                            }
-                            first = false;
-                        }
-                    } else {
-                        // experiments (results differ): 1 = one MMA per K step, 2 = only the first K step, 3 = two passes (A_lo * W_hi dropped)
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t off = (uint64_t)((k * 32) >> 4);
-                            const uint32_t acc = first ? 0u : 1u;
-                            if (mma_mode == 2 && k != 0) continue;
-                            if (mma_mode == 3) {
-                                if (CG == 2) { umma_f16_2sm(d_tmem, dA + off, dBlo + off, idesc, acc); umma_f16_2sm(d_tmem, dA + off, dB + off, idesc, 1); }
-                                else { umma_f16(d_tmem, dA + off, dBlo + off, idesc, acc); umma_f16(d_tmem, dA + off, dB + off, idesc, 1); }
-                            } else {
-                                if (CG == 2) umma_f16_2sm(d_tmem, dA + off, dB + off, idesc, acc); else umma_f16(d_tmem, dA + off, dB + off, idesc, acc);
-                            }
-                            first = false;
-                        }
-                    }
-                    if (!p.w_res) { if (CG == 2) umma_commit_2sm(&emptyB[sb]); else umma_commit(&emptyB[sb]); }
-                    if (t == 8) { if (CG == 2) umma_commit_2sm(&emptyA[sa]); else umma_commit(&emptyA[sa]); }
-                    if (kb - ci * p.chunk == p.chunk - 1 || kb == KB - 1) { if (CG == 2) umma_commit_2sm(&tmem_full[buf]); else umma_commit(&tmem_full[buf]); }
+            for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+            int pend = -1;                                                                     // stage whose MMAs may still be running
+            for (int kb = 0; kb < KB; ++kb, ++g) {
+                const bool first = kb % p.chunk == 0, last = kb % p.chunk == p.chunk - 1 || kb == KB - 1;
+                const bool tr = tr0 && g < p.trace_n;
+                if (tr) p.trace[2 * p.trace_n + g] = clock64();                                // [2] waiting for the stage
+                mbar_wait(&full[s], ph);
+                if (tr) p.trace[3 * p.trace_n + g] = clock64();                                // [3] about to issue k-block g
+                const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+                const uint32_t aw = sa + (uint32_t)wg * 64u * rowb;
+                const uint64_t dA = make_sdesc(aw, sbo, lay), dAlo = make_sdesc(aw + a_bytes, sbo, lay);
+                const uint64_t dB = make_sdesc(sa + 2 * a_bytes, sbo, lay), dBlo = make_sdesc(sa + 2 * a_bytes + b_bytes, sbo, lay);
+                wg_fence();
+                wg_kblock<BN, F16>(c, dA, dAlo, dB, dBlo, ksteps, mode, first);
+                wg_commit();
+                if (last) {
+                    wg_wait<0>();
+                    release(pend); release(s); pend = -1;
+                    wg_promote(tot, c);
+                } else {
+                    wg_wait<1>();                                                              // the previous k-block's MMAs are done
+                    release(pend); pend = s;
                 }
-                ita += cchunks;
-                cc += NC;
+                if (tr) p.trace[4 * p.trace_n + g] = clock64();                                // [4] k-block g issued, previous one retired
+                if (++s == p.stages) { s = 0; ph ^= 1; }
             }
+            consumers_sync();                                   // everyone is done reading the previous tile's staged accumulator
+            wg_stage<BN>(tot, tile, LD, wg, warp, lane);
+            consumers_sync();
+            if constexpr (BN == 64 && F16) {
+                if (p.pool_out) { tcp_pool_tile(p, tile, u, mt_units, warp, lane); continue; }
+            }
+            amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane));
         }
-        __syncwarp();
-    } else {
-        tcp_epilogue<NG16, CG, PL>(p, tmem_base, tmem_full, tmem_empty, warp, lane, rank, NC, u0, ustep, units, mt_units);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (CG == 2) cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        if (CG == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
+        note_fp16_range(amax, p.range_flag);
     }
 }
 
@@ -994,22 +267,6 @@ __global__ void split_h16_kernel(const float* __restrict__ in, __half* __restric
 // ----------------------------------------------------------------------------------------------------------------
 // `stride` > 1: TMA traversal stride (elementStrides) on W and H, so the box holds every stride-th pixel: a strided conv
 // reads exactly the 16 x 8 input pixels its 128 outputs need for one tap, densely packed in shared memory.
-// activation map with the H dimension listed before W (box {64 c, box_h rows, box_w columns, 1}): the box lands in shared memory as
-// [column][row][64 c], which gives the halo kernel's x-major item one uniform 1280-byte stride between its 8-pixel groups
-static int make_map_act_hw(CUtensorMap* m, const void* base_v, int B, int H, int W, int C, int cs, int co, int box_h, int box_w) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) { set_error("conv2d_tc: cuTensorMapEncodeTiled unavailable"); return VD3D_ECUDA; }
-    const char* base = (const char*)base_v + (size_t)co * 2;
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)H, (cuuint64_t)W, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)W * cs * 2, (cuuint64_t)cs * 2, (cuuint64_t)H * W * cs * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)box_h, (cuuint32_t)box_w, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("conv2d_tc: cuTensorMapEncodeTiled(activation, h-major box) failed: %d", (int)r); return VD3D_ECUDA; }
-    return VD3D_OK;
-}
-
 static int make_map_act(CUtensorMap* m, const void* base_v, int B, int H, int W, int C, int cs, int co, int esize = 4,
                         int box_w = TC_TW, int box_h = TC_TH, int stride = 1) {
     EncodeTiledFn enc = get_encode();
@@ -1029,28 +286,23 @@ static int make_map_act(CUtensorMap* m, const void* base_v, int B, int H, int W,
 
 using namespace vd3d;
 
-// persistent fp16 engine: the widest tile (<= 256) that splits Cout evenly into ceil(Cout / 256) tiles of 16-column granules;
-// tiles wider than 128 columns run as CTA pairs (cta_group::2) so that three operand stages still fit in shared memory
+// persistent fp16 engine: the widest tile (<= TC_MAX_BN) that splits Cout evenly into ceil(Cout / TC_MAX_BN) tiles of 16-column granules
 extern "C" int vd3d_tc_pick_bn_persistent(int Cout) {
     const int cp = (Cout + 15) / 16 * 16;
-    const int nt = (cp + 255) / 256;
+    const int nt = (cp + TC_MAX_BN - 1) / TC_MAX_BN;
     return ((cp + nt - 1) / nt + 15) / 16 * 16;
 }
 
-// Tile width for a given problem: minimise  rounds x (BN + 64)  over 16-column granules, where rounds = ceil(tiles / SMs (pairs)) and the
-// constant stands for the per-k-block cost that does not scale with the tile width (barrier / commit / issue gaps); tiles wider than 128
-// columns run as CTA pairs.  E.g. Cout = 1152 at 120 M tiles: 5 x 240 needs 5 rounds (300 pair tiles on 74 pairs), 6 x 192 also 5 rounds
-// of narrower tiles: -16 %; Cout = 1408 keeps 6 x 240 (360 pair tiles, 4.86 rounds).
+// Tile width for a given problem: minimise  rounds x (BN + 64)  over 16-column granules, where rounds = ceil(tiles / SMs) and the
+// constant stands for the per-k-block cost that does not scale with the tile width (barrier / issue gaps and the epilogue).
 static int pick_bn_cost(int Cout, int m_tiles) {
     const int cp = (Cout + 15) / 16 * 16;
-    if (cp <= 128) return cp;
+    if (cp <= TC_MAX_BN) return cp;
     int best = vd3d_tc_pick_bn_persistent(Cout);
     long long best_cost = -1;
-    for (int bn = 96; bn <= 256; bn += 16) {
-        const int cg = bn > 128 ? 2 : 1;
-        const long long units = (long long)((m_tiles + cg - 1) / cg) * ((cp + bn - 1) / bn);
-        const long long slots = kNumSMs / cg;
-        const long long rounds = (units + slots - 1) / slots;
+    for (int bn = 64; bn <= TC_MAX_BN; bn += 16) {
+        const long long units = (long long)m_tiles * ((cp + bn - 1) / bn);
+        const long long rounds = (units + kNumSMs - 1) / kNumSMs;
         const long long cost = rounds * (bn + 64);
         if (best_cost < 0 || cost < best_cost || (cost == best_cost && bn > best)) { best_cost = cost; best = bn; }
     }
@@ -1060,13 +312,12 @@ static int pick_bn_cost(int Cout, int m_tiles) {
 extern "C" int vd3d_tc_pick_bn(int Cout) {
     // largest tile <= 128 that divides Cout evenly into 16-multiples; otherwise the single-tile / 64 fallbacks
     if (Cout % 128 == 0) return 128;
-    if (Cout <= 160 && Cout > 128) return (Cout + 15) / 16 * 16;
     if (Cout < 128 && Cout % 16) return (Cout + 15) / 16 * 16;        // single N tile, columns >= Cout masked (weight rows beyond Cout are TMA zero fill)
     if (Cout % 96 == 0) return 96;
     if (Cout % 64 == 0) return 64;
     if (Cout % 48 == 0) return 48;
     if (Cout % 32 == 0) return 32;
-    return 128;
+    return Cout <= 128 ? (Cout + 15) / 16 * 16 : 128;
 }
 
 // diagnostics: clock64 stamps of the TMA / MMA pipeline of CTA 0 ([5][n] int64 device buffer; NULL disables)
@@ -1074,131 +325,60 @@ static long long* g_trace = nullptr;
 static int g_trace_n = 0;
 extern "C" void vd3d_tc_set_trace(void* dev_i64, int n) { g_trace = (long long*)dev_i64; g_trace_n = n; }
 
-// launch of the persistent kernel: p.BN / p.idesc (for M = 128) / p.tmem_cols / p.chunk / tile counts are set by the caller,
-// the weight maps have BN / CG rows per box
-static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi, const CUtensorMap& mWlo, int CG, void* stream) {
+template <int BN, bool F16>
+static cudaError_t tcp_launch_kernel(const cudaLaunchConfig_t& cfg, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi,
+                                     const CUtensorMap& mWlo, const TcParams& p) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        const cudaError_t e = cudaFuncSetAttribute(conv2d_tcp_kernel<BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        if (e != cudaSuccess) return e;
+        attr_set = true;
+    }
+    return cudaLaunchKernelEx(&cfg, conv2d_tcp_kernel<BN, F16>, mA, mAlo, mWhi, mWlo, p);
+}
+
+// launch of the persistent kernel: p.BN (<= TC_MAX_BN) / p.chunk / tile counts are set by the caller, the weight maps have BN rows per box
+static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi, const CUtensorMap& mWlo, void* stream) {
     const int BN = p.BN;
     { const char* e = getenv("VD3D_TC_DEBUG"); p.dbg = e ? atoi(e) : 0; }
     p.trace = g_trace; p.trace_n = g_trace_n;
-    tcp_set_accumulators(p);
     if (p.rowb == 0) p.rowb = 128;
-    const size_t stage_bytes = 2 * (size_t)128 * p.rowb + 2 * (size_t)(BN / CG) * p.rowb;
-    const size_t pool_bytes = p.pool_out ? (size_t)128 * POOL_LD * sizeof(float) : 0;
-    VD3D_REQUIRE(!p.pool_out || (BN == 64 && CG == 1 && p.relu && !p.res && !p.res_h16_hi), "conv2d_tc: the fused max-pool needs a 64-column single-CTA tile with ReLU and no residual");
-    int stages = (int)((227 * 1024 - 1024 - 512 - pool_bytes) / stage_bytes);
+    VD3D_REQUIRE(BN % 16 == 0 && BN >= 16 && BN <= TC_MAX_BN, "conv2d_tc: BN must be a multiple of 16 in [16, %d]", TC_MAX_BN);
+    const size_t stage_bytes = 2 * (size_t)128 * p.rowb + 2 * (size_t)BN * p.rowb;
+    const size_t tile_bytes = (size_t)128 * (BN + 4) * sizeof(float);
+    VD3D_REQUIRE(!p.pool_out || (BN == 64 && p.f16 && p.relu && !p.res && !p.res_h16_hi), "conv2d_tc: the fused max-pool needs a 64-column fp16 tile with ReLU and no residual");
+    int stages = (int)((227 * 1024 - 1024 - 256 - tile_bytes) / stage_bytes);
     if (stages > 8) stages = 8;
     VD3D_REQUIRE(stages >= 2, "conv2d_tc: tile too large for shared memory");
     p.stages = stages;
-    if (CG == 2) p.idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-    const size_t bar_bytes = ((2 * stages + 10) * sizeof(uint64_t) + 15) / 16 * 16;
-    p.pool_smem_off = (uint32_t)(stages * stage_bytes + bar_bytes);
-    const size_t smem = stages * stage_bytes + bar_bytes + pool_bytes + 1024;
-    static bool pattr_set = false;
-    if (!pattr_set) {
-#define VD3D_TCP_ATTR(NG, C) VD3D_CUDA(cudaFuncSetAttribute(conv2d_tcp_kernel<NG, C, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-                             VD3D_CUDA(cudaFuncSetAttribute(conv2d_tcp_kernel<NG, C, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
-        VD3D_TCP_ATTR(2, 1); VD3D_TCP_ATTR(4, 1); VD3D_TCP_ATTR(5, 1); VD3D_TCP_ATTR(8, 1);
-        VD3D_TCP_ATTR(2, 2); VD3D_TCP_ATTR(4, 2); VD3D_TCP_ATTR(5, 2); VD3D_TCP_ATTR(8, 2);
-#undef VD3D_TCP_ATTR
-        pattr_set = true;
-    }
-    const int units = cdiv(p.m_tiles, CG) * p.n_tiles;
-    const int nsm = kNumSMs / CG;
+    const size_t smem = stages * stage_bytes + tile_bytes + ((2 * stages * sizeof(uint64_t) + 15) / 16 * 16) + 1024;
+    const int units = p.m_tiles * p.n_tiles;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(CG * (units < nsm ? units : nsm)));
+    cfg.gridDim = dim3((unsigned)(units < kNumSMs ? units : kNumSMs));
     cfg.blockDim = dim3(TCP_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)CG; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    const int ng = (BN + 31) / 32;
-    cudaError_t le;
-    const bool pl = (p.out == nullptr && p.pool_out == nullptr) || p.res_h16_hi != nullptr;      // (the fused-pool epilogue lives in the <2, 1, 0> instance)
-#define VD3D_TCP_LAUNCH(NG, C) le = pl ? cudaLaunchKernelEx(&cfg, conv2d_tcp_kernel<NG, C, 1>, mA, mAlo, mWhi, mWlo, p) \
-                                       : cudaLaunchKernelEx(&cfg, conv2d_tcp_kernel<NG, C, 0>, mA, mAlo, mWhi, mWlo, p)
-    if (CG == 2) {
-        if (ng <= 2) VD3D_TCP_LAUNCH(2, 2); else if (ng <= 4) VD3D_TCP_LAUNCH(4, 2); else if (ng == 5) VD3D_TCP_LAUNCH(5, 2); else VD3D_TCP_LAUNCH(8, 2);
-    } else {
-        if (ng <= 2) VD3D_TCP_LAUNCH(2, 1); else if (ng <= 4) VD3D_TCP_LAUNCH(4, 1); else if (ng == 5) VD3D_TCP_LAUNCH(5, 1); else VD3D_TCP_LAUNCH(8, 1);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cudaError_t le = cudaErrorInvalidValue;
+#define VD3D_TCP_CASE(N) case N: le = p.f16 ? tcp_launch_kernel<N, true>(cfg, mA, mAlo, mWhi, mWlo, p) : tcp_launch_kernel<N, false>(cfg, mA, mAlo, mWhi, mWlo, p); break
+    switch (BN) {
+        VD3D_TCP_CASE(16); VD3D_TCP_CASE(32); VD3D_TCP_CASE(48); VD3D_TCP_CASE(64);
+        VD3D_TCP_CASE(80); VD3D_TCP_CASE(96); VD3D_TCP_CASE(112); VD3D_TCP_CASE(128);
     }
-#undef VD3D_TCP_LAUNCH
+#undef VD3D_TCP_CASE
     if (le != cudaSuccess) { set_error("conv2d_tcp: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
     VD3D_CHECK_LAUNCH("conv2d_tcp");
     return VD3D_OK;
 }
 
-// launch of the persistent halo kernel (3x3, stride 1, pad 1, dilation 1); same contract as tcp_launch, activation maps have box {64 c, 10 w, 1 h}
-static int tcph_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi, const CUtensorMap& mWlo, int CG, void* stream) {
-    const int BN = p.BN;
-    { const char* e = getenv("VD3D_TC_DEBUG"); p.dbg = e ? atoi(e) : 0; }
-    tcp_set_accumulators(p);
-    const size_t b_stage = 2 * (size_t)(BN / CG) * 128;
-    const int KBtot = 9 * (p.cin_pad / 64);
-    p.h_sa = 2;
-    {
-        // input-halo stages: VD3D_TC_HSA=3 adds a third one when the resident weights leave room for it (64 -> 64 layers: 72 KB of weights + 3 x 50 KB)
-        const char* e = getenv("VD3D_TC_HSA");
-        const int want = e ? atoi(e) : 2;      // measured (same box, alternating): 3 stages 746 / 746 pairs/s against 748 / 758 with 2, layer 1 183 us against 169: no gain, kept as a switch
-        if (want >= 3 && p.n_tiles == 1 && (size_t)KBtot * b_stage + 3 * (size_t)TCPH_ITEM + (2 * 3 + 2 * KBtot + 10) * sizeof(uint64_t) + 1024 <= (size_t)227 * 1024) p.h_sa = 3;
-    }
-    const size_t budget = 227 * 1024 - 1024 - 512 - (size_t)p.h_sa * TCPH_ITEM;
-    p.w_res = (p.n_tiles == 1 && (size_t)KBtot * b_stage <= budget) ? 1 : 0;
-    if (!p.w_res && p.h_sa == 3) p.h_sa = 2;
-    p.h_sb = p.w_res ? KBtot : (int)(budget / b_stage);
-    if (!p.w_res && p.h_sb > 8) p.h_sb = 8;
-    VD3D_REQUIRE(p.h_sb >= 2, "conv2d_tc: halo tile too large for shared memory");
-    if (CG == 2) p.idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-    const size_t smem = (size_t)p.h_sa * TCPH_ITEM + (size_t)p.h_sb * b_stage + (2 * p.h_sa + 2 * p.h_sb + 10) * sizeof(uint64_t) + 1024;
-    static bool hattr_set = false;
-    if (!hattr_set) {
-#define VD3D_TCPH_ATTR(NG, C) VD3D_CUDA(cudaFuncSetAttribute(conv2d_tcph_kernel<NG, C, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-                              VD3D_CUDA(cudaFuncSetAttribute(conv2d_tcph_kernel<NG, C, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
-        VD3D_TCPH_ATTR(2, 1); VD3D_TCPH_ATTR(4, 1); VD3D_TCPH_ATTR(5, 1); VD3D_TCPH_ATTR(8, 1);
-        VD3D_TCPH_ATTR(2, 2); VD3D_TCPH_ATTR(4, 2); VD3D_TCPH_ATTR(5, 2); VD3D_TCPH_ATTR(8, 2);
-#undef VD3D_TCPH_ATTR
-        hattr_set = true;
-    }
-    const int units = cdiv(p.m_tiles, CG) * p.n_tiles;
-    const int nsm = kNumSMs / CG;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(CG * (units < nsm ? units : nsm)));
-    cfg.blockDim = dim3(TCPH_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = (unsigned)CG; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    const int ng = (BN + 31) / 32;
-    cudaError_t le;
-    const bool pl = p.out == nullptr || p.res_h16_hi != nullptr;
-#define VD3D_TCPH_LAUNCH(NG, C) le = pl ? cudaLaunchKernelEx(&cfg, conv2d_tcph_kernel<NG, C, 1>, mA, mAlo, mWhi, mWlo, p) \
-                                        : cudaLaunchKernelEx(&cfg, conv2d_tcph_kernel<NG, C, 0>, mA, mAlo, mWhi, mWlo, p)
-    if (CG == 2) {
-        if (ng <= 2) VD3D_TCPH_LAUNCH(2, 2); else if (ng <= 4) VD3D_TCPH_LAUNCH(4, 2); else if (ng == 5) VD3D_TCPH_LAUNCH(5, 2); else VD3D_TCPH_LAUNCH(8, 2);
-    } else {
-        if (ng <= 2) VD3D_TCPH_LAUNCH(2, 1); else if (ng <= 4) VD3D_TCPH_LAUNCH(4, 1); else if (ng == 5) VD3D_TCPH_LAUNCH(5, 1); else VD3D_TCPH_LAUNCH(8, 1);
-    }
-#undef VD3D_TCPH_LAUNCH
-    if (le != cudaSuccess) { set_error("conv2d_tcph: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
-    VD3D_CHECK_LAUNCH("conv2d_tcph");
-    return VD3D_OK;
-}
-
-static void tc_env(int& persist, int& cg) {
-    // engine switches (A/B timing in tools/prof_conv.py, test parametrisation): VD3D_TC_PERSIST (default 1), VD3D_TC_CG (1 | 2)
-    const char* e = getenv("VD3D_TC_PERSIST");
-    persist = e ? atoi(e) : 1;
-    e = getenv("VD3D_TC_CG");
-    cg = e ? atoi(e) : VD3D_TC_CG_DEFAULT;
+// a requested tile wider than TC_MAX_BN runs as equal halves (16-column granules): every width accumulates identically
+static int fit_bn(int bn) {
+    while (bn > TC_MAX_BN) bn = (bn / 2 + 15) / 16 * 16;
+    return bn;
 }
 
 static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
@@ -1219,17 +399,13 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     VD3D_REQUIRE(((uintptr_t)in & 15) == 0 && ((uintptr_t)w_hi & 15) == 0 && ((uintptr_t)out & 15) == 0, "conv2d_tc: pointers must be 16-byte aligned");
     VD3D_REQUIRE(!res_h16_hi || ((((uintptr_t)res_h16_hi | (uintptr_t)res_h16_lo) & 7) == 0), "conv2d_tc: residual planes must be 8-byte aligned");
     VD3D_REQUIRE(!out_h16_hi || (out_h16_lo && out_cs % 4 == 0), "conv2d_tc: fp16 output planes come in (hi, lo) pairs");
-    int persist, cg_env;
-    tc_env(persist, cg_env);
     int BN = bn;
     if (BN <= 0) {
-        if (f16 && passes == 3 && persist != 0) {
+        if (f16 && passes == 3) {
             const int Ho_ = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1, Wo_ = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
             BN = pick_bn_cost(Cout, cdiv(Wo_, TC_TW) * cdiv(Ho_, TC_TH) * B);
-            // short-K layers (the 1x1 expansion convs of the ResNet bottlenecks: 4 k-blocks, wide output, residual): a tile's MMAs are over before its
-            // epilogue has fetched the first residual columns, so the step is the epilogue's chain of global round trips.  64-column tiles take the
-            // prefetching epilogue variant (residual requested before the accumulation, tcp_epilogue PRE) and put twice as many CTAs on the output:
-            // measured on 256 -> 1024 at 11520 pixels: 93 us (256-column pairs) -> 78 (128) -> 76 (64) (profiles/r02_exp_bottleneck_r101.txt)
+            // short-K layers (the 1x1 expansion convs of the ResNet bottlenecks: 4 k-blocks, wide output, residual): a tile's MMAs are over
+            // before its epilogue has fetched the first residual columns; 64-column tiles put twice as many CTAs on the output
             const char* esk = getenv("VD3D_TC_SHORTK");
             const int shortk = esk ? atoi(esk) : 8;
             const int kb_total = KH * KW * ((Cin + 63) / 64);
@@ -1238,9 +414,8 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
             if (shortk > 0 && kb_total <= shortk && BN > 64 && Cout % 64 == 0 && (!need_res || res || res_h16_hi)) BN = 64;
         } else BN = vd3d_tc_pick_bn(Cout);
     }
-    const bool use_p = f16 && passes == 3 && persist != 0;
-    VD3D_REQUIRE(use_p || (out && !res_h16_hi), "conv2d_tc: planes-only output / plane residuals need the persistent fp16-split engine");
-    VD3D_REQUIRE(BN % 16 == 0 && BN >= 16 && BN <= (use_p ? 256 : 160), "conv2d_tc: BN must be a multiple of 16 in [16, %d]", use_p ? 256 : 160);
+    VD3D_REQUIRE(BN % 16 == 0 && BN >= 16 && BN <= 256, "conv2d_tc: BN must be a multiple of 16 in [16, 256]");
+    BN = fit_bn(BN);
     TcParams p;
     memset(&p, 0, sizeof(p));
     VD3D_REQUIRE(stride >= 1 && stride <= 4, "conv2d_tc: stride must be in [1, 4]");
@@ -1252,22 +427,21 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     p.stride_w = stride; p.pad_w = pad;
     p.cout_pad = (Cout + 15) / 16 * 16;
     p.m_tiles = p.tiles_w * p.tiles_h * B; p.n_tiles = cdiv(p.cout_pad, BN);
+    p.rowb = 128;
     {
-        // L2-aware tile order (unit_tile): M blocks whose activation slab (hi + lo planes of the block's input pixels, all channels) is about
-        // VD3D_TC_L2MB megabytes (default 44 = two blocks for the 1408-wide layers; measured with ncu: 550 -> 450 MB of DRAM reads per launch,
-        // same duration: the layers are not DRAM-bound); only when there is more than one N tile (otherwise A is read once anyway).  0 disables.
+        // L2-aware tile order (unit_tile): M blocks whose activation slab (the block's input pixels, all channels, both planes) is about
+        // VD3D_TC_L2MB megabytes (default 20: well inside the 50 MB L2), only when there is more than one N tile (otherwise A is read once
+        // anyway).  0 disables.
         const char* e = getenv("VD3D_TC_L2MB");
-        const double l2mb = e ? atof(e) : 44.0;
+        const double l2mb = e ? atof(e) : 20.0;
         p.mblock = 0;
-        if (f16 && p.n_tiles > 1 && l2mb > 0) {
-            const double a_bytes_per_tile = 128.0 * stride * stride * (double)p.cin_pad * 4.0;      // input pixels behind one 128-pixel output tile, 2 fp16 planes
-            const int cg_guess = BN > 128 ? 2 : 1;
-            int mb = (int)(l2mb * 1048576.0 / (a_bytes_per_tile * cg_guess));
-            const int mt_units = cdiv(p.m_tiles, cg_guess);
+        if (p.n_tiles > 1 && l2mb > 0) {
+            const double a_bytes_per_tile = 128.0 * stride * stride * (double)p.cin_pad * (f16 ? 4.0 : 8.0);
+            int mb = (int)(l2mb * 1048576.0 / a_bytes_per_tile);
             if (mb < 8) mb = 8;
-            if (mb < mt_units) {
-                const int nblk = cdiv(mt_units, mb);
-                p.mblock = cdiv(mt_units, nblk);       // equal blocks
+            if (mb < p.m_tiles) {
+                const int nblk = cdiv(p.m_tiles, mb);
+                p.mblock = cdiv(p.m_tiles, nblk);       // equal blocks
             }
         }
     }
@@ -1280,98 +454,11 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     p.res_h16_hi = res_h16_hi; p.res_h16_lo = res_h16_lo;
     p.two_pass = two_pass;
     p.range_flag = out_h16_hi ? fp16_range_flag() : nullptr;
-    // instruction descriptor (cute::UMMA::InstrDescriptor): D = f32 (1 @4), A/B format @7/@10 (tf32 = 2, f16 = 0), K-major, N>>3 @17, M>>4 @24
-    const uint32_t fmt = f16 ? 0u : 2u;
-    p.idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    uint32_t cols = 32; while (cols < (uint32_t)(2 * BN)) cols <<= 1;     // two accumulator buffers (chunked promotion)
-    p.tmem_cols = cols;
     {
         const char* e = getenv("VD3D_TC_CHUNK");
         p.chunk = e ? atoi(e) : 4;
         if (p.chunk < 1) p.chunk = 1;
     }
-    {
-        const char* e = getenv("VD3D_TC_HALO");
-        p.h_mode = e ? atoi(e) : 0;     // opt-in: measured no faster than the generic kernel (the bound is UMMA operand reads, not L2)
-        if (!(f16 && passes == 3 && KH == 3 && KW == 3 && pad == 1 && dil == 1 && stride == 1 && BN <= 128) || p.h_mode < 0 || p.h_mode > 2) p.h_mode = 0;
-    }
-    if (use_p && !p.h_mode) {
-        // ---- persistent kernel (default) ----
-        int CG = (cg_env == 2 || (cg_env == 0 && BN > 128)) ? 2 : 1;        // VD3D_TC_CG: 0 = auto (pairs for wide tiles), 1, 2
-        const bool s1_3x3 = KH == 3 && KW == 3 && pad == 1 && dil == 1 && stride == 1;
-        // one narrow N tile whose 9 * cchunks weight blocks fit beside the two input-halo items when split over a CTA pair (64 -> 64 layers):
-        // paired halo kernel with the weights resident in shared memory (only the input halo is streamed)
-        const char* ewr = getenv("VD3D_TC_WRES");
-        const bool wres_pair = (ewr ? atoi(ewr) : 1) != 0 && cg_env == 0 && s1_3x3 && p.n_tiles == 1 && BN % 16 == 0 &&
-                               (size_t)9 * (p.cin_pad / 64) * BN * 128 <= (size_t)(227 * 1024 - 1024 - 512) - 2 * (size_t)TCPH_ITEM;
-        if (wres_pair) CG = 2;
-        const int K = KH * KW * p.cin_pad;
-        CUtensorMap mA, mAlo, mWhi, mWlo;
-        int rc;
-        if ((rc = make_map_wgt(&mWhi, w_hi, Cout, K, BN / CG, 2))) return rc;
-        if ((rc = make_map_wgt(&mWlo, w_lo, Cout, K, BN / CG, 2))) return rc;
-        // Input-halo reuse for 3x3 stride-1 convs (A staged once per 64-channel chunk, nine taps read it): VD3D_TC_PHALO = 2 (default):
-        // for the wide, paired tiles only (measured: head conv -8 %, layer3 -2 %; the narrow-tile layers are 3..5 % slower with it), 1: always, 0: never
-        const char* eh = getenv("VD3D_TC_PHALO");
-        const int phalo = eh ? atoi(eh) : 2;
-        const bool halo_fits = 227 * 1024 - 1024 - 512 - 2 * (size_t)TCPH_ITEM >= 2 * (2 * (size_t)(BN / CG) * 128);
-        // VD3D_TC_PHALO_MAXC: widest input (channels) that still takes the halo kernel (experiments; default: no limit)
-        const char* ehc = getenv("VD3D_TC_PHALO_MAXC");
-        const bool halo_width_ok = !ehc || Cin <= atoi(ehc);
-        if ((phalo == 1 || (phalo == 2 && CG == 2)) && halo_fits && s1_3x3 && halo_width_ok) {
-            const char* exm = getenv("VD3D_TC_XMAJOR");
-            if (!(exm && atoi(exm) == 0) && make_map_act_hw(&mA, in, B, H, W, Cin, in_cs, in_co, 10, 18) == VD3D_OK &&
-                make_map_act_hw(&mAlo, in_lo, B, H, W, Cin, in_cs, in_co, 10, 18) == VD3D_OK) {
-                p.m_xmajor = 1;          // x-major halo item: 2 TMA operations per (tile, chunk)
-                return tcph_launch(p, mA, mAlo, mWhi, mWlo, CG, stream);
-            }
-            if ((rc = make_map_act(&mA, in, B, H, W, Cin, in_cs, in_co, 2, 10, 1))) return rc;
-            if ((rc = make_map_act(&mAlo, in_lo, B, H, W, Cin, in_cs, in_co, 2, 10, 1))) return rc;
-            return tcph_launch(p, mA, mAlo, mWhi, mWlo, CG, stream);
-        }
-        if ((rc = make_map_act(&mA, in, B, H, W, Cin, in_cs, in_co, 2, TC_TW, TC_TH, stride))) return rc;
-        if ((rc = make_map_act(&mAlo, in_lo, B, H, W, Cin, in_cs, in_co, 2, TC_TW, TC_TH, stride))) return rc;
-        return tcp_launch(p, mA, mAlo, mWhi, mWlo, CG, stream);
-    }
-    if (p.h_mode) {
-        // ---- halo kernel: A staged once per 64-channel chunk and reused by the taps ----
-        p.h_taps = p.h_mode == 2 ? 9 : 3;
-        p.h_rp = p.h_mode == 2 ? 2560u : 2048u;
-        p.h_sbo = p.h_mode == 2 ? 1280u : 1024u;
-        p.h_sa = 2;
-        const size_t a_item = 2 * (size_t)TCH_PLANE, b_stage = 2 * (size_t)BN * 128;
-        const size_t budget = 227 * 1024 - 1024 - 512 - p.h_sa * a_item;
-        p.h_sb = (int)(budget / b_stage);
-        if (p.h_sb > 8) p.h_sb = 8;
-        VD3D_REQUIRE(p.h_sb >= 2, "conv2d_tc: halo tile too large for shared memory");
-        const size_t smem = p.h_sa * a_item + p.h_sb * b_stage + (2 * p.h_sa + 2 * p.h_sb + 6) * sizeof(uint64_t) + 1024;
-        const int K = 9 * p.cin_pad;
-        CUtensorMap mA, mAlo, mWhi, mWlo;
-        int rc;
-        const int bw = p.h_mode == 2 ? 10 : 16, bh = p.h_mode == 2 ? 1 : 10;
-        if ((rc = make_map_act(&mA, in, B, H, W, Cin, in_cs, in_co, 2, bw, bh))) return rc;
-        if ((rc = make_map_act(&mAlo, in_lo, B, H, W, Cin, in_cs, in_co, 2, bw, bh))) return rc;
-        if ((rc = make_map_wgt(&mWhi, w_hi, Cout, K, BN, 2))) return rc;
-        if ((rc = make_map_wgt(&mWlo, w_lo, Cout, K, BN, 2))) return rc;
-        static bool hattr_set = false;
-        if (!hattr_set) {
-            VD3D_CUDA(cudaFuncSetAttribute(conv2d_tc_halo_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            VD3D_CUDA(cudaFuncSetAttribute(conv2d_tc_halo_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-            hattr_set = true;
-        }
-        dim3 grid(p.tiles_w * p.tiles_h * B, cdiv(Cout, BN));
-        cudaStream_t st = (cudaStream_t)stream;
-        if (BN <= 64) conv2d_tc_halo_kernel<2><<<grid, TCH_THREADS, smem, st>>>(mA, mAlo, mWhi, mWlo, p);
-        else conv2d_tc_halo_kernel<4><<<grid, TCH_THREADS, smem, st>>>(mA, mAlo, mWhi, mWlo, p);
-        VD3D_CHECK_LAUNCH("conv2d_tc_halo");
-        return VD3D_OK;
-    }
-    const size_t stage_bytes = 2 * (size_t)TC_A_BYTES + 2 * (size_t)BN * 128;
-    int stages = (int)((200 * 1024) / stage_bytes);
-    if (stages > 6) stages = 6;
-    VD3D_REQUIRE(stages >= 2, "conv2d_tc: tile too large for shared memory");
-    p.stages = stages;
-    const size_t smem = stages * stage_bytes + (2 * stages + 6) * sizeof(uint64_t) + 1024;
     const int K = KH * KW * p.cin_pad;
     CUtensorMap mA, mAlo, mWhi, mWlo;
     int rc;
@@ -1379,20 +466,7 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     if ((rc = make_map_act(&mAlo, in_lo ? in_lo : in, B, H, W, Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
     if ((rc = make_map_wgt(&mWhi, w_hi, Cout, K, BN, esize))) return rc;
     if ((rc = make_map_wgt(&mWlo, w_lo ? w_lo : w_hi, Cout, K, BN, esize))) return rc;
-    static bool attr_set = false;
-    if (!attr_set) {
-        VD3D_CUDA(cudaFuncSetAttribute(conv2d_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        VD3D_CUDA(cudaFuncSetAttribute(conv2d_tc_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        VD3D_CUDA(cudaFuncSetAttribute(conv2d_tc_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set = true;
-    }
-    dim3 grid(p.tiles_w * p.tiles_h * B, cdiv(Cout, BN));
-    cudaStream_t st = (cudaStream_t)stream;
-    if (BN <= 64) conv2d_tc_kernel<2><<<grid, TC_THREADS, smem, st>>>(mA, mAlo, mWhi, mWlo, p);
-    else if (BN <= 128) conv2d_tc_kernel<4><<<grid, TC_THREADS, smem, st>>>(mA, mAlo, mWhi, mWlo, p);
-    else conv2d_tc_kernel<5><<<grid, TC_THREADS, smem, st>>>(mA, mAlo, mWhi, mWlo, p);
-    VD3D_CHECK_LAUNCH("conv2d_tc");
-    return VD3D_OK;
+    return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
 }
 
 extern "C" int vd3d_conv2d_tc(const float* in, const float* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
@@ -1507,23 +581,17 @@ static int stem_launch(const void* in_hi, const void* in_lo, int B, int H, int W
     p.stride_w = 1; p.pad_w = 0;
     p.Ho = (H + 2 * pad - KH) / stride + 1; p.Wo = (W + 2 * pad - KW) / stride + 1;
     VD3D_REQUIRE(p.Ho > 0 && p.Wo > 0, "conv2d_tc16_stem: empty output");
-    const int BN = Cout;
+    const int BN = fit_bn(Cout);
     p.Cout = Cout; p.BN = BN; p.passes = 3; p.f16 = 1; p.bk = win; p.cin_pad = win; p.rowb = 2 * win; p.out_scale = out_scale;
     p.tiles_w = cdiv(p.Wo, TC_TW); p.tiles_h = cdiv(p.Ho, TC_TH);
     p.cout_pad = Cout;
-    p.m_tiles = p.tiles_w * p.tiles_h * B; p.n_tiles = 1;
+    p.m_tiles = p.tiles_w * p.tiles_h * B; p.n_tiles = cdiv(Cout, BN);
     p.v8 = (out_cs % 8 == 0 && out_co % 8 == 0 && ((uintptr_t)out & 31) == 0 && (!bias || ((uintptr_t)bias & 31) == 0) &&
             (!out_hi16 || ((((uintptr_t)out_hi16 | (uintptr_t)out_lo16) & 15) == 0))) ? 1 : 0;
     p.out_cs = out_cs; p.out_co = out_co; p.relu = relu;
     p.bias = bias; p.out = out; p.out_h16_hi = out_hi16; p.out_h16_lo = out_lo16;
     p.range_flag = out_hi16 ? fp16_range_flag() : nullptr;
-    p.idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    uint32_t cols = 32; while (cols < (uint32_t)(2 * BN)) cols <<= 1;
-    p.tmem_cols = cols;
     p.chunk = 4;
-    int persist, cg_env;
-    tc_env(persist, cg_env);
-    const int CG = pool_out ? 1 : ((cg_env == 2 || (cg_env == 0 && BN > 128)) ? 2 : 1);
     if (pool_out) {
         p.pool_out = pool_out; p.pool_cs = pool_cs; p.pool_co = pool_co;
         p.pool_H = (p.Ho + 2 - 3) / 2 + 1; p.pool_W = (p.Wo + 2 - 3) / 2 + 1;
@@ -1547,9 +615,9 @@ static int stem_launch(const void* in_hi, const void* in_lo, int B, int H, int W
         }
     }
     int rc;
-    if ((rc = make_map_wgt(&mWhi, w_hi, Cout, KH * win, BN / CG, 2, 2 * win))) return rc;
-    if ((rc = make_map_wgt(&mWlo, w_lo, Cout, KH * win, BN / CG, 2, 2 * win))) return rc;
-    return tcp_launch(p, mA, mAlo, mWhi, mWlo, CG, stream);
+    if ((rc = make_map_wgt(&mWhi, w_hi, Cout, KH * win, BN, 2, 2 * win))) return rc;
+    if ((rc = make_map_wgt(&mWlo, w_lo, Cout, KH * win, BN, 2, 2 * win))) return rc;
+    return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
 }
 
 extern "C" int vd3d_split_lo_nhwc(const float* in, float* lo, long long npix, int C, int cs, int co, void* stream) {

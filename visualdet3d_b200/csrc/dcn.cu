@@ -5,7 +5,7 @@
 // with the reference's sampling rule (deform_conv_cuda_kernel.cu:467-497,570-633): a tap contributes only if
 // h > -1 && w > -1 && h < H && w < W; the four neighbours are individually zero outside the image.  The K order
 // (tap-major, channel-minor) is the conv engines' weight order, so the GEMM that follows is a plain 1x1 convolution on the
-// tcgen05 engine (the `lo` companion of the columns is produced here for free).  Sampling coordinates and weights are
+// wgmma engine (the `lo` companion of the columns is produced here for free).  Sampling coordinates and weights are
 // computed once per (pixel, tap) and shared by all channels: one CTA = 32 pixels x all taps, threads sweep channel quads.
 // HBM-bound gather: reads x once (L2 serves the 9x tap reuse), writes KH*KW*C floats (+lo) per pixel.
 #include "common.cuh"

@@ -1,5 +1,5 @@
 // Fused (modulated) deformable convolution on the tensor cores: the bilinear gather of deformable im2col goes STRAIGHT into the swizzled
-// shared-memory A operand of the tcgen05 GEMM.  The reference writes `columns[C*9, H*W]` to HBM per image and reads it back with cuBLAS
+// shared-memory A operand of the wgmma GEMM.  The reference writes `columns[C*9, H*W]` to HBM per image and reads it back with cuBLAS
 // (R/lib/ops/dcn/src/cuda/deform_conv_cuda.cpp:539-556, kernel deform_conv_cuda_kernel.cu:570-633); round 1 of this repo still wrote the
 // fp16 (hi, lo) column planes (4 x 9C bytes per pixel) and re-read them in a 1x1 conv.  Here no column tensor exists:
 //
@@ -9,10 +9,10 @@
 //                           + offsets / mask + output, instead of + 2 x 36 C bytes per pixel of column planes.
 //
 // Structure = the persistent conv kernel (conv2d_tc.cu) with the activation TMA producer replaced by eight GATHER warps:
-//   warp 0      weight producer: TMA boxes [64 k][BN] of the (hi, lo) weight matrix, one per k-block (tap, 64-channel chunk)
-//   warp 1      MMA issuer + TMEM owner: 3 kind::f16 MMAs per K step on (A_lo W_hi + A_hi W_lo + A_hi W_hi), chunked promotion
-//   warps 2..9  epilogue (tcp_epilogue of tc_conv.cuh: scale / bias / residual / ReLU -> fp32 and / or fp16 planes)
-//   warps 10..17 gather: per tile the sampling position, validity and the 4 bilinear weights of every (pixel, tap) are computed once into
+//   warps 0..7  two consumer warpgroups: 3 kind::f16 MMAs per K step on (A_lo W_hi + A_hi W_lo + A_hi W_hi), chunked promotion, then the
+//               epilogue (tcp_store_tile of tc_conv.cuh: scale / bias / residual / ReLU -> fp32 and / or fp16 planes)
+//   warp 8      weight producer: TMA boxes [64 k][BN] of the (hi, lo) weight matrix, one per k-block (tap, 64-channel chunk)
+//   warps 9..16 gather: per tile the sampling position, validity and the 4 bilinear weights of every (pixel, tap) are computed once into
 //               shared memory (same rule as dcn.cu: a tap contributes iff h > -1, w > -1, h < H, w < W; corners are individually zero
 //               outside); per k-block each thread produces 8 channels of 4 pixels: 4 corner loads of 32 B, the weighted sum, x mask,
 //               the (hi, lo) fp16 split, and two 16-byte stores into the SWIZZLE_128B K-major operand layout
@@ -25,7 +25,8 @@
 
 namespace vd3d {
 
-constexpr int DF_THREADS = 576;
+constexpr int DF_THREADS = 256 + 32 + 256;      // consumers, weight producer, gather warps
+constexpr int DF_GATHER0 = 288;                  // first gather thread
 constexpr int DF_GATHER_WARPS = 8;
 constexpr int DF_MAXK = 9;
 
@@ -36,57 +37,47 @@ struct DfParams {
     int KW, stride, pad, dil;
     int K;                                          // taps
     int cchunks;                                    // C / 64
-    int stages;
+    int stages;                                     // operand ring (fused kernel) / weight ring (staged kernel)
     uint32_t stage_bytes;
     int dbg;                                        // timing knock-outs (VD3D_DF_DEBUG; results wrong): 1 no corner loads, 2 no offset / mask loads, 4 no operand stores, 8 one MMA per k-block
 };
 
 struct DfSample { int base_flags; float w1, w2, w3, w4, m; };      // base + W + 1 in bits 0..25, validity bits 26..30 (bit 30 = tap inside)
 
-template <int NG16>
+template <int BN>
 __global__ void __launch_bounds__(DF_THREADS, 1)
 deform_conv_fused_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p, const DfParams q) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    constexpr int LD = BN + 4;
     const uint32_t a_bytes = 128u * 128u;                        // one A plane of a stage: 128 pixels x 64 fp16
-    const uint32_t b_bytes = (uint32_t)p.BN * 128u;
+    const uint32_t b_bytes = (uint32_t)BN * 128u;
     const uint32_t stage_bytes = q.stage_bytes;                  // [A hi | A lo | W hi | W lo]
     DfSample* samp = reinterpret_cast<DfSample*>(smem + (size_t)q.stages * stage_bytes);          // [128][K]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(samp) + sizeof(DfSample) * 128 * DF_MAXK);
-    uint64_t* fullA = bars;                       // [stages]  gather warps -> MMA (8 arrivals)
-    uint64_t* fullB = fullA + q.stages;           // [stages]  TMA -> MMA
-    uint64_t* empty = fullB + q.stages;           // [stages]  MMA -> producers
-    uint64_t* tmem_full = empty + q.stages;       // [4]
-    uint64_t* tmem_empty = tmem_full + 4;         // [4]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
+    float* tile = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(samp) + sizeof(DfSample) * 128 * DF_MAXK);     // [128][LD] staged accumulator
+    uint64_t* bars = reinterpret_cast<uint64_t*>(tile + 128 * LD);
+    uint64_t* fullA = bars;                       // [stages]  gather warps -> consumers (8 arrivals)
+    uint64_t* fullB = fullA + q.stages;           // [stages]  TMA -> consumers
+    uint64_t* empty = fullB + q.stages;           // [stages]  consumers (8 warps) -> producers
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int KB = q.K * q.cchunks;
-    const int NC = (KB + p.chunk - 1) / p.chunk;
     const int mt_units = p.m_tiles;
     const int units = mt_units * p.n_tiles;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < q.stages; ++s) { mbar_init(&fullA[s], DF_GATHER_WARPS); mbar_init(&fullB[s], 1); mbar_init(&empty[s], 1); }
-        for (int i = 0; i < 4; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 8); }
+        for (int s = 0; s < q.stages; ++s) { mbar_init(&fullA[s], DF_GATHER_WARPS); mbar_init(&fullB[s], 1); mbar_init(&empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, *tmem_slot);
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= weight producer =================
         int it = 0;
         for (int u = u0; u < units; u += ustep) {
             const int nt = unit_nt(p, u, mt_units);
-            const int n0 = nt * p.BN;
+            const int n0 = nt * BN;
             for (int kb = 0; kb < KB; ++kb, ++it) {
                 const int s = it % q.stages, ph = (it / q.stages) & 1;
                 mbar_wait(&empty[s], ph ^ 1);
@@ -99,49 +90,45 @@ deform_conv_fused_kernel(const __grid_constant__ CUtensorMap mapWhi, const __gri
                 __syncwarp();
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (elect_one()) {
-            int it = 0, cc = 0;
-            for (int u = u0; u < units; u += ustep) {
-                const int nvalid = min(p.BN, p.cout_pad - unit_nt(p, u, mt_units) * p.BN);
-                const uint32_t idesc = (p.idesc & ~(0x3Fu << 17)) | ((uint32_t)(nvalid >> 3) << 17);
-                for (int kb = 0; kb < KB; ++kb, ++it) {
-                    const int ci = kb / p.chunk;
-                    const int buf = (cc + ci) % p.nbuf;
-                    const bool first_in_chunk = kb - ci * p.chunk == 0;
-                    if (first_in_chunk) {
-                        mbar_wait(&tmem_empty[buf], (((cc + ci) / p.nbuf) & 1) ^ 1);
-                        tc_fence_after();
-                    }
-                    const int s = it % q.stages, ph = (it / q.stages) & 1;
-                    mbar_wait(&fullB[s], ph);
-                    mbar_wait(&fullA[s], ph);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.BN);
-                    const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-                    const uint64_t dA = make_sdesc(sa), dAlo = make_sdesc(sa + a_bytes);
-                    const uint64_t dB = make_sdesc(sa + 2 * a_bytes), dBlo = make_sdesc(sa + 2 * a_bytes + b_bytes);
+    } else if (warp < 8) {
+        // ================= consumer warpgroups =================
+        const int wg = warp >> 2;
+        const int mode = (q.dbg & 8) ? 1 : 0;
+        auto release = [&](int st) {
+            __syncwarp();
+            if (st >= 0 && lane == 0) mbar_arrive(&empty[st]);
+        };
+        float tot[BN / 2], c[BN / 2];
+        float amax = 0.f;
+        int it = 0;
+        for (int u = u0; u < units; u += ustep) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t off = (uint64_t)((k * 32) >> 4);
-                        umma_f16(d_tmem, dAlo + off, dB + off, idesc, (first_in_chunk && k == 0) ? 0u : 1u);      // small terms first (same order as conv2d_tcp_kernel)
-                        umma_f16(d_tmem, dA + off, dBlo + off, idesc, 1);
-                        umma_f16(d_tmem, dA + off, dB + off, idesc, 1);
-                    }
-                    umma_commit(&empty[s]);
-                    if (kb - ci * p.chunk == p.chunk - 1 || kb == KB - 1) umma_commit(&tmem_full[buf]);
-                }
-                cc += NC;
+            for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+            int pend = -1;
+            for (int kb = 0; kb < KB; ++kb, ++it) {
+                const bool first = kb % p.chunk == 0, last = kb % p.chunk == p.chunk - 1 || kb == KB - 1;
+                const int s = it % q.stages, ph = (it / q.stages) & 1;
+                mbar_wait(&fullB[s], ph);
+                mbar_wait(&fullA[s], ph);
+                const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+                const uint32_t aw = sa + (uint32_t)wg * 64u * 128u;
+                const uint64_t dA = make_sdesc(aw), dAlo = make_sdesc(aw + a_bytes);
+                const uint64_t dB = make_sdesc(sa + 2 * a_bytes), dBlo = make_sdesc(sa + 2 * a_bytes + b_bytes);
+                wg_fence();
+                wg_kblock<BN, true>(c, dA, dAlo, dB, dBlo, 4, mode, first);      // small terms first (same order as conv2d_tcp_kernel)
+                wg_commit();
+                if (last) { wg_wait<0>(); release(pend); release(s); pend = -1; wg_promote(tot, c); }
+                else { wg_wait<1>(); release(pend); pend = s; }
             }
+            consumers_sync();
+            wg_stage<BN>(tot, tile, LD, wg, warp, lane);
+            consumers_sync();
+            amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane));
         }
-        __syncwarp();
-    } else if (warp < 10) {
-        tcp_epilogue<NG16, 1, 0>(p, tmem_base, tmem_full, tmem_empty, warp, lane, 0u, NC, u0, ustep, units, mt_units);
-        tc_fence_before();
+        note_fp16_range(amax, p.range_flag);
     } else {
         // ================= gather warps (256 threads) =================
-        const int gt = (int)threadIdx.x - 320;            // 0..255
+        const int gt = (int)threadIdx.x - DF_GATHER0;     // 0..255
         const int j = gt & 7;                             // 8-channel group inside the 64-channel chunk
         const int m0 = gt >> 3;                           // pixels m0, m0 + 32, m0 + 64, m0 + 96 of the tile
         int it = 0;
@@ -226,11 +213,6 @@ deform_conv_fused_kernel(const __grid_constant__ CUtensorMap mapWhi, const __gri
             }
         }
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-    }
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -243,70 +225,61 @@ deform_conv_fused_kernel(const __grid_constant__ CUtensorMap mapWhi, const __gri
 //   the nine taps of the chunk then gather from shared memory (a corner that falls outside the staged region -- an offset beyond
 //   +-1 pixel around the regular tap position -- is read from global memory instead: correct for any offset, fast for small ones).
 // The sampling table (position, validity, 4 weights, mask of every (pixel, tap)) is computed once per tile for all nine taps.
-// Weights run through their own 4-deep TMA ring (16 KB blocks), the gathered operand through a 2-deep ring: measured with the shared
-// 2-deep ring of the first version, every k-block paid the full latency of its weight load (1.9k clk of a 3.0k clk k-block period).
+// Weights run through their own TMA ring (up to 4 deep, as many 16 KB blocks as shared memory leaves), the gathered operand through a
+// 2-deep ring: with one shared 2-deep ring every k-block pays the full latency of its weight load.
 // Each gather thread owns channels [4j, 4j + 4) and [32 + 4j, 32 + 4j + 4) of four pixels: its two 16-byte shared-memory reads per corner
 // are conflict-free (8 lanes = 128 contiguous bytes).
 // K order: 64-channel chunk outermost, taps inside (k = (chunk * 9 + tap) * 64 + c): the weight matrix and the unfused A/B path
 // (vd3d_deform_im2col_h16 with k_order = 1) use the same order, so both still produce identical bits.
-// Shared memory: A ring 2 x 32 KB + W ring 4 x 16 KB + region 60 KB + sample table 31.5 KB = 221 KB.
+// Shared memory: A ring 2 x 32 KB + W ring + region 60 KB + sample table 31.5 KB + staged accumulator 34 KB (BN = 64: 2 W stages, 222 KB).
 // ----------------------------------------------------------------------------------------------------------------
 constexpr int DFS_HALO = 2;
 constexpr int DFS_RH = TC_TH + 2 * DFS_HALO, DFS_RW = TC_TW + 2 * DFS_HALO;       // 12 x 20 pixels
 constexpr uint32_t DFS_REGION_BYTES = DFS_RH * DFS_RW * 64 * 4;                   // 61,440
-constexpr int DFS_A_STAGES = 2, DFS_W_STAGES = 4;
+constexpr int DFS_A_STAGES = 2, DFS_W_STAGES = 4;      // (W: at most)
 constexpr uint32_t DFS_A_STAGE = 2u * 128u * 128u;                                 // A hi | A lo
 
 struct DfSample2 { int hl, wl_flags; float w1, w2, w3, w4, m; };                  // wl in the low 16 bits (biased by 16384), validity bits 16..20
 
-template <int NG16>
+template <int BN>
 __global__ void __launch_bounds__(DF_THREADS, 1)
 deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const __grid_constant__ CUtensorMap mapWhi,
                                 const __grid_constant__ CUtensorMap mapWlo, const TcParams p, const DfParams q) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    constexpr int LD = BN + 4;
     const uint32_t a_bytes = 128u * 128u;
-    const uint32_t b_bytes = (uint32_t)p.BN * 128u;
+    const uint32_t b_bytes = (uint32_t)BN * 128u;
     const uint32_t w_stage = 2u * b_bytes;
+    const int WS = q.stages;                       // weight ring depth
     uint8_t* smemA = smem;
     uint8_t* smemW = smemA + (size_t)DFS_A_STAGES * DFS_A_STAGE;
-    uint8_t* region = smemW + (size_t)DFS_W_STAGES * w_stage;
+    uint8_t* region = smemW + (size_t)WS * w_stage;
     DfSample2* samp = reinterpret_cast<DfSample2*>(region + DFS_REGION_BYTES);               // [K taps][128 pixels]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(samp) + (size_t)DF_MAXK * 128 * sizeof(DfSample2));
-    uint64_t* fullA = bars;                        // [2]  gather warps -> MMA (8 arrivals)
-    uint64_t* emptyA = fullA + DFS_A_STAGES;       // [2]  MMA -> gather warps
-    uint64_t* fullW = emptyA + DFS_A_STAGES;       // [4]  weight TMA -> MMA
-    uint64_t* emptyW = fullW + DFS_W_STAGES;       // [4]  MMA -> weight producer
-    uint64_t* fullR = emptyW + DFS_W_STAGES;       // [1]  region TMA -> gather warps
+    float* tile = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(samp) + (size_t)DF_MAXK * 128 * sizeof(DfSample2));     // [128][LD]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(tile + 128 * LD);
+    uint64_t* fullA = bars;                        // [2]  gather warps -> consumers (8 arrivals)
+    uint64_t* emptyA = fullA + DFS_A_STAGES;       // [2]  consumers (8 warps) -> gather warps
+    uint64_t* fullW = emptyA + DFS_A_STAGES;       // [WS] weight TMA -> consumers
+    uint64_t* emptyW = fullW + WS;                 // [WS] consumers (8 warps) -> weight producer
+    uint64_t* fullR = emptyW + WS;                 // [1]  region TMA -> gather warps
     uint64_t* emptyR = fullR + 1;                  // [1]  gather warps -> region producer (8 arrivals)
-    uint64_t* tmem_full = emptyR + 1;              // [4]
-    uint64_t* tmem_empty = tmem_full + 4;          // [4]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int KB = q.K * q.cchunks;
-    const int NC = (KB + p.chunk - 1) / p.chunk;
     const int mt_units = p.m_tiles;
     const int units = mt_units * p.n_tiles;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < DFS_A_STAGES; ++s) { mbar_init(&fullA[s], DF_GATHER_WARPS); mbar_init(&emptyA[s], 1); }
-        for (int s = 0; s < DFS_W_STAGES; ++s) { mbar_init(&fullW[s], 1); mbar_init(&emptyW[s], 1); }
+        for (int s = 0; s < DFS_A_STAGES; ++s) { mbar_init(&fullA[s], DF_GATHER_WARPS); mbar_init(&emptyA[s], 8); }
+        for (int s = 0; s < WS; ++s) { mbar_init(&fullW[s], 1); mbar_init(&emptyW[s], 8); }
         mbar_init(fullR, 1); mbar_init(emptyR, DF_GATHER_WARPS);
-        for (int i = 0; i < 4; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, *tmem_slot);
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= TMA producer: the input region of every (tile, chunk), then its nine weight blocks =================
         int itw = 0, ir = 0;
         for (int u = u0; u < units; u += ustep) {
@@ -315,7 +288,7 @@ deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const 
             int mt = mu;
             const int tw = mt % p.tiles_w; mt /= p.tiles_w;
             const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
-            const int n0 = nt * p.BN;
+            const int n0 = nt * BN;
             for (int ch = 0; ch < q.cchunks; ++ch, ++ir) {
                 mbar_wait(emptyR, (ir & 1) ^ 1);                     // the gather warps are done with the previous region
                 if (elect_one()) {
@@ -324,7 +297,7 @@ deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const 
                 }
                 __syncwarp();
                 for (int t = 0; t < q.K; ++t, ++itw) {
-                    const int s = itw % DFS_W_STAGES, ph = (itw / DFS_W_STAGES) & 1;
+                    const int s = itw % WS, ph = (itw / WS) & 1;
                     mbar_wait(&emptyW[s], ph ^ 1);
                     if (elect_one()) {
                         uint8_t* st = smemW + (size_t)s * w_stage;
@@ -337,53 +310,45 @@ deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const 
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        if (elect_one()) {
-            int it = 0, cc = 0;
-            for (int u = u0; u < units; u += ustep) {
-                const int nvalid = min(p.BN, p.cout_pad - unit_nt(p, u, mt_units) * p.BN);
-                const uint32_t idesc = (p.idesc & ~(0x3Fu << 17)) | ((uint32_t)(nvalid >> 3) << 17);
-                for (int kb = 0; kb < KB; ++kb, ++it) {
-                    const int ci = kb / p.chunk;
-                    const int buf = (cc + ci) % p.nbuf;
-                    const bool first_in_chunk = kb - ci * p.chunk == 0;
-                    if (first_in_chunk) {
-                        mbar_wait(&tmem_empty[buf], (((cc + ci) / p.nbuf) & 1) ^ 1);
-                        tc_fence_after();
-                    }
-                    const int sa = it % DFS_A_STAGES, pa = (it / DFS_A_STAGES) & 1;
-                    const int sw = it % DFS_W_STAGES, pw = (it / DFS_W_STAGES) & 1;
-                    mbar_wait(&fullW[sw], pw);
-                    mbar_wait(&fullA[sa], pa);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * p.BN);
-                    const uint32_t aa = smem_u32(smemA + (size_t)sa * DFS_A_STAGE), ww = smem_u32(smemW + (size_t)sw * w_stage);
-                    const uint64_t dA = make_sdesc(aa), dAlo = make_sdesc(aa + a_bytes);
-                    const uint64_t dB = make_sdesc(ww), dBlo = make_sdesc(ww + b_bytes);
-                    if (q.dbg & 8) umma_f16(d_tmem, dA, dB, idesc, first_in_chunk ? 0u : 1u);
-                    else
+    } else if (warp < 8) {
+        // ================= consumer warpgroups =================
+        const int wg = warp >> 2;
+        const int mode = (q.dbg & 8) ? 1 : 0;
+        auto release = [&](int i) {
+            __syncwarp();
+            if (i >= 0 && lane == 0) { mbar_arrive(&emptyA[i % DFS_A_STAGES]); mbar_arrive(&emptyW[i % WS]); }
+        };
+        float tot[BN / 2], c[BN / 2];
+        float amax = 0.f;
+        int it = 0;
+        for (int u = u0; u < units; u += ustep) {
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t off = (uint64_t)((k * 32) >> 4);
-                        umma_f16(d_tmem, dAlo + off, dB + off, idesc, (first_in_chunk && k == 0) ? 0u : 1u);
-                        umma_f16(d_tmem, dA + off, dBlo + off, idesc, 1);
-                        umma_f16(d_tmem, dA + off, dB + off, idesc, 1);
-                    }
-                    umma_commit(&emptyA[sa]);
-                    umma_commit(&emptyW[sw]);
-                    if (kb - ci * p.chunk == p.chunk - 1 || kb == KB - 1) umma_commit(&tmem_full[buf]);
-                }
-                cc += NC;
+            for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+            int pend = -1;
+            for (int kb = 0; kb < KB; ++kb, ++it) {
+                const bool first = kb % p.chunk == 0, last = kb % p.chunk == p.chunk - 1 || kb == KB - 1;
+                const int sa = it % DFS_A_STAGES, pa = (it / DFS_A_STAGES) & 1;
+                const int sw = it % WS, pw = (it / WS) & 1;
+                mbar_wait(&fullW[sw], pw);
+                mbar_wait(&fullA[sa], pa);
+                const uint32_t aa = smem_u32(smemA + (size_t)sa * DFS_A_STAGE) + (uint32_t)wg * 64u * 128u, ww = smem_u32(smemW + (size_t)sw * w_stage);
+                const uint64_t dA = make_sdesc(aa), dAlo = make_sdesc(aa + a_bytes);
+                const uint64_t dB = make_sdesc(ww), dBlo = make_sdesc(ww + b_bytes);
+                wg_fence();
+                wg_kblock<BN, true>(c, dA, dAlo, dB, dBlo, 4, mode, first);
+                wg_commit();
+                if (last) { wg_wait<0>(); release(pend); release(it); pend = -1; wg_promote(tot, c); }
+                else { wg_wait<1>(); release(pend); pend = it; }
             }
+            consumers_sync();
+            wg_stage<BN>(tot, tile, LD, wg, warp, lane);
+            consumers_sync();
+            amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane));
         }
-        __syncwarp();
-    } else if (warp < 10) {
-        tcp_epilogue<NG16, 1, 0>(p, tmem_base, tmem_full, tmem_empty, warp, lane, 0u, NC, u0, ustep, units, mt_units);
-        tc_fence_before();
+        note_fp16_range(amax, p.range_flag);
     } else {
         // ================= gather warps (256 threads) =================
-        const int gt = (int)threadIdx.x - 320;
+        const int gt = (int)threadIdx.x - DF_GATHER0;
         const int j = gt & 7;                             // channel groups [4j, 4j + 4) and [32 + 4j, 32 + 4j + 4) of the chunk
         const int m0 = gt >> 3;                           // pixels m0, m0 + 32, m0 + 64, m0 + 96 of the tile
         int it = 0, ir = 0;
@@ -492,16 +457,24 @@ deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const 
             }
         }
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
-    }
 }
 
 }  // namespace vd3d
 
 using namespace vd3d;
+
+// sets the shared-memory limit of a kernel instance once, then launches it
+template <typename K, typename... Args>
+static cudaError_t df_launch(K kernel, int grid, size_t smem, void* stream, Args... args) {
+    static bool attr_set = false;      // one flag per kernel instance (K differs per instance)
+    if (!attr_set) {
+        const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        if (e != cudaSuccess) return e;
+        attr_set = true;
+    }
+    kernel<<<grid, DF_THREADS, smem, (cudaStream_t)stream>>>(args...);
+    return cudaGetLastError();
+}
 
 extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C, int x_cs, int x_co,
                                       const float* om, int om_cs, int off_co, int msk_co, int has_mask, int mask_sigmoid,
@@ -522,7 +495,7 @@ extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C
     const int Ho = (H + 2 * pad - (dil * (KH - 1) + 1)) / stride + 1, Wo = (W + 2 * pad - (dil * (KW - 1) + 1)) / stride + 1;
     VD3D_REQUIRE(Ho > 0 && Wo > 0, "deform_conv_fused: empty output");
     const int cp = (Cout + 15) / 16 * 16;
-    const int BN = cp <= 64 ? cp : 64;                 // 576 threads leave ~110 registers per thread: 64-column tiles keep the epilogue spill-free
+    const int BN = cp <= 64 ? cp : 64;                 // 544 threads leave ~120 registers per thread: 64-column tiles keep the consumers spill-free
     p.B = B; p.H = Ho; p.W = Wo; p.Ho = Ho; p.Wo = Wo; p.Cin = KH * KW * C; p.KH = 1; p.KW = 1; p.stride = 1; p.dil = 1;
     p.Cout = Cout; p.BN = BN; p.passes = 3; p.f16 = 1; p.bk = 64; p.cin_pad = KH * KW * C; p.out_scale = out_scale;
     p.tiles_w = cdiv(Wo, TC_TW); p.tiles_h = cdiv(Ho, TC_TH);
@@ -533,11 +506,9 @@ extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C
     p.out_cs = out_cs; p.out_co = out_co; p.res_cs = res_cs; p.res_co = res_co; p.relu = relu;
     p.bias = bias; p.res = res; p.out = out; p.out_h16_hi = out_hi16; p.out_h16_lo = out_lo16;
     p.range_flag = out_hi16 ? fp16_range_flag() : nullptr;
-    p.idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
     { const char* e = getenv("VD3D_TC_CHUNK"); p.chunk = e ? atoi(e) : 4; if (p.chunk < 1) p.chunk = 1; }
     { const char* e = getenv("VD3D_TC_DEBUG"); p.dbg = e ? atoi(e) : 0; }
     { const char* e = getenv("VD3D_DF_DEBUG"); q.dbg = e ? atoi(e) : 0; }
-    tcp_set_accumulators(p);
     q.x = x; q.H = H; q.W = W; q.C = C; q.x_cs = x_cs; q.x_co = x_co;
     q.om = om; q.om_cs = om_cs; q.off_co = off_co; q.msk_co = msk_co; q.has_mask = has_mask; q.mask_sigmoid = mask_sigmoid;
     q.KW = KW; q.stride = stride; q.pad = pad; q.dil = dil; q.K = KH * KW; q.cchunks = C / 64;
@@ -548,12 +519,7 @@ extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C
     if ((rc = make_map_wgt(&mWlo, w_lo, Cout, KH * KW * C, BN, 2))) return rc;
     const int units = p.m_tiles * p.n_tiles;
     const int grid = units < kNumSMs ? units : kNumSMs;
-    static bool attr_set = false;
-    if (!attr_set) {
-        VD3D_CUDA(cudaFuncSetAttribute(deform_conv_fused_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        VD3D_CUDA(cudaFuncSetAttribute(deform_conv_fused_staged_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr_set = true;
-    }
+    const size_t tile_bytes = (size_t)128 * (BN + 4) * sizeof(float);
     const char* es = getenv("VD3D_DCN_STAGED");
     const bool staged = k_order == 1 && stride == 1 && dil == 1 && pad == 1 && KH == 3 && KW == 3 && !(es && atoi(es) == 0);
     if (staged) {
@@ -568,22 +534,33 @@ extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C
         CUresult cr = enc(&mX, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)(x + x_co), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         VD3D_REQUIRE(cr == CUDA_SUCCESS, "deform_conv_fused: cuTensorMapEncodeTiled(input regions) failed: %d", (int)cr);
-        q.stages = DFS_A_STAGES;
-        const size_t smem = (size_t)DFS_A_STAGES * DFS_A_STAGE + (size_t)DFS_W_STAGES * 2 * BN * 128 + (size_t)DFS_REGION_BYTES +
-                            (size_t)DF_MAXK * 128 * sizeof(DfSample2) + 32 * sizeof(uint64_t) + 1024;
-        VD3D_REQUIRE(smem <= 227 * 1024, "deform_conv_fused: shared-memory budget exceeded");
-        deform_conv_fused_staged_kernel<2><<<grid, DF_THREADS, smem, (cudaStream_t)stream>>>(mX, mWhi, mWlo, p, q);
+        const size_t fixed = (size_t)DFS_A_STAGES * DFS_A_STAGE + (size_t)DFS_REGION_BYTES + (size_t)DF_MAXK * 128 * sizeof(DfSample2) + tile_bytes +
+                             32 * sizeof(uint64_t) + 1024;
+        int ws = (int)((227 * 1024 - fixed) / (2 * (size_t)BN * 128));
+        if (ws > DFS_W_STAGES) ws = DFS_W_STAGES;
+        VD3D_REQUIRE(ws >= 2, "deform_conv_fused: shared-memory budget exceeded");
+        q.stages = ws;
+        const size_t smem = fixed + (size_t)ws * 2 * BN * 128;
+        cudaError_t le = cudaErrorInvalidValue;
+#define VD3D_DFS_CASE(N) case N: le = df_launch(deform_conv_fused_staged_kernel<N>, grid, smem, stream, mX, mWhi, mWlo, p, q); break
+        switch (BN) { VD3D_DFS_CASE(16); VD3D_DFS_CASE(32); VD3D_DFS_CASE(48); VD3D_DFS_CASE(64); }
+#undef VD3D_DFS_CASE
+        if (le != cudaSuccess) { set_error("deform_conv_fused_staged: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
         VD3D_CHECK_LAUNCH("deform_conv_fused_staged");
         return VD3D_OK;
     }
     VD3D_REQUIRE(k_order == 0 || C == 64, "deform_conv_fused: the chunk-major K order needs the staged kernel (3x3, stride 1, pad 1, dilation 1)");
-    const size_t fixed = sizeof(DfSample) * 128 * DF_MAXK + 32 * sizeof(uint64_t) + 1024;
+    const size_t fixed = sizeof(DfSample) * 128 * DF_MAXK + tile_bytes + 32 * sizeof(uint64_t) + 1024;
     int stages = (int)((227 * 1024 - fixed) / q.stage_bytes);
     if (stages > 6) stages = 6;
     VD3D_REQUIRE(stages >= 2, "deform_conv_fused: tile too large for shared memory");
     q.stages = stages;
     const size_t smem = (size_t)stages * q.stage_bytes + fixed;
-    deform_conv_fused_kernel<2><<<grid, DF_THREADS, smem, (cudaStream_t)stream>>>(mWhi, mWlo, p, q);
+    cudaError_t le = cudaErrorInvalidValue;
+#define VD3D_DF_CASE(N) case N: le = df_launch(deform_conv_fused_kernel<N>, grid, smem, stream, mWhi, mWlo, p, q); break
+    switch (BN) { VD3D_DF_CASE(16); VD3D_DF_CASE(32); VD3D_DF_CASE(48); VD3D_DF_CASE(64); }
+#undef VD3D_DF_CASE
+    if (le != cudaSuccess) { set_error("deform_conv_fused: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
     VD3D_CHECK_LAUNCH("deform_conv_fused");
     return VD3D_OK;
 }

@@ -1,20 +1,20 @@
-// PSMCosine cost volume (R/lib/PSM_cost_volume.py:76-91) on the tcgen05 tensor cores.
+// PSMCosine cost volume (R/lib/PSM_cost_volume.py:76-91) on the Hopper tensor cores (wgmma).
 //
 //   cost[q, d] = (x(q) >= d) ? 1/C * sum_c L[q, c] * R[q - d, c] : 0        q = flat pixel index (b, y, x), x(q) = q mod W
 //
-// The SIMT kernels of cost_volume.cu are bound by shared-memory reads and instruction issue (ncu: both ~65 %, DRAM 53 %);
-// the correlation is a banded matrix product, so here it is computed as the FULL product of a 128-pixel L tile with the
-// 160-pixel R window [q0 - 32, q0 + 128) on the tensor core and only the band is kept:
+// The SIMT kernels of cost_volume.cu are bound by shared-memory reads and instruction issue; the correlation is a banded matrix product,
+// so here it is computed as the FULL product of a 128-pixel L tile with the 160-pixel R window [q0 - 32, q0 + 128) on the tensor core and
+// only the band is kept:
 //
 //   * pixels are addressed flat across rows and images: R[q - d] leaves the row exactly when x(q) < d, where the reference
 //     writes 0, so the tile grid needs no row alignment (B*H*W / 128 tiles, no ragged tiles at W = 320).
 //   * operands are the fp16 (hi, lo) planes the tensor-core convs already produce for the features; three kind::f16 MMAs per
-//     k-step (Llo*Rhi + Lhi*Rlo + Lhi*Rhi) into one fp32 TMEM accumulator [128 x 160]: 22 significant operand bits, and only
+//     k-step (Llo*Rhi + Lhi*Rlo + Lhi*Rhi) into one fp32 accumulator [128 x 160]: 22 significant operand bits, and only
 //     4 * C/64 * 3 accumulations, so no promotion is needed (error ~1e-6 of the 1e-3 parity budget).
-//   * warp 0 = TMA producer (4 boxes per 64-channel k-block: Lhi, Llo [128 x 64], Rhi, Rlo [160 x 64], 128-byte swizzle),
-//     warp 1 = MMA issuer + TMEM owner (two accumulators: the epilogue of tile i overlaps the MMAs of tile i+1),
-//     warps 2..5 = epilogue: lane = pixel p reads accumulator columns [32 (p/32), +64), parks them in a private
-//     conflict-free shared-memory column and picks its band  column(p, d) = p - d + 32; scale, mask, 16-byte stores.
+//   * warp 8 = TMA producer (4 boxes per 64-channel k-block: Lhi, Llo [128 x 64], Rhi, Rlo [160 x 64], 128-byte swizzle),
+//     warps 0..7 = two consumer warpgroups (64 L pixels x 160 window pixels each): after the last k-block every thread parks the
+//     accumulator entries of the band (window pixel - L pixel in [0, 32]) in a [128][36] shared-memory tile, then thread t writes the
+//     disparities d = 4 (t / 128) + 8 i of pixel t % 128: scale, mask, 16-byte stores.
 //   * persistent: one CTA per SM strides over the tiles; HBM traffic = the algorithmic bytes (each L / R element once from
 //     DRAM, the 32-pixel window overlap comes from L2).
 #include "tc_common.cuh"
@@ -22,14 +22,14 @@
 
 namespace vd3d {
 
-constexpr int PT_M = 128;                 // L pixels per tile (UMMA M)
+constexpr int PT_M = 128;                 // L pixels per tile
 constexpr int PT_PAD = 32;                // R window starts PT_PAD pixels before the tile: disparities < 32
-constexpr int PT_N = PT_M + PT_PAD;       // 160 R pixels (UMMA N)
-constexpr int PT_THREADS = 192;
+constexpr int PT_N = PT_M + PT_PAD;       // 160 R pixels (wgmma N)
+constexpr int PT_THREADS = 256 + 32;      // warps 0..7 = consumers, warp 8 = TMA producer
 constexpr int PT_STAGES = 2;
 constexpr int PT_L_BYTES = PT_M * 128, PT_R_BYTES = PT_N * 128;
 constexpr int PT_STAGE_BYTES = 2 * PT_L_BYTES + 2 * PT_R_BYTES;       // 73728
-constexpr int PT_SCRATCH_FLOATS = 64 * 32;                              // per epilogue warp: [64 columns][32 lanes]
+constexpr int PT_BAND_LD = 36;                                          // band tile row: entries 0..32 used
 
 struct PsmTcParams {
     long long npix;
@@ -37,7 +37,6 @@ struct PsmTcParams {
     int out_cs, out_co;
     float inv_c;
     float* out;
-    uint32_t idesc;
 };
 
 __global__ void __launch_bounds__(PT_THREADS, 1)
@@ -45,30 +44,18 @@ psm_cosine_tc_kernel(const __grid_constant__ CUtensorMap mapLhi, const __grid_co
                      const __grid_constant__ CUtensorMap mapRhi, const __grid_constant__ CUtensorMap mapRlo, const PsmTcParams p) {
     extern __shared__ __align__(1024) uint8_t psm_tc_smem[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(psm_tc_smem) + 1023) & ~(uintptr_t)1023);
-    float* scratch = reinterpret_cast<float*>(smem + (size_t)PT_STAGES * PT_STAGE_BYTES);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(scratch + 4 * PT_SCRATCH_FLOATS);
-    uint64_t* full = bars;                      // [stages]  TMA -> MMA
-    uint64_t* empty = bars + PT_STAGES;         // [stages]  MMA -> TMA
-    uint64_t* tfull = bars + 2 * PT_STAGES;     // [2]       MMA -> epilogue
-    uint64_t* tempty = tfull + 2;               // [2]       epilogue -> MMA
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+    float* band = reinterpret_cast<float*>(smem + (size_t)PT_STAGES * PT_STAGE_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(band + PT_M * PT_BAND_LD);     // [stages]  TMA -> consumers
+    uint64_t* empty = full + PT_STAGES;                                          // [stages]  consumers (8 warps) -> TMA
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < PT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+        for (int s = 0; s < PT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             // ================= TMA producer =================
             int it = 0;
@@ -86,78 +73,66 @@ psm_cosine_tc_kernel(const __grid_constant__ CUtensorMap mapLhi, const __grid_co
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ================= MMA issuer =================
-            int it = 0, tc = 0;
-            for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x, ++tc) {
-                const int buf = tc & 1, use = tc >> 1;
-                mbar_wait(&tempty[buf], (use & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(buf * PT_N);
-                for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
-                    const int s = it % PT_STAGES, ph = (it / PT_STAGES) & 1;
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + (size_t)s * PT_STAGE_BYTES);
-                    const uint64_t dLh = make_sdesc(sa), dLl = make_sdesc(sa + PT_L_BYTES);
-                    const uint64_t dRh = make_sdesc(sa + 2 * PT_L_BYTES), dRl = make_sdesc(sa + 2 * PT_L_BYTES + PT_R_BYTES);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t off = (uint64_t)((k * 32) >> 4);
-                        umma_f16(d_tmem, dLl + off, dRh + off, p.idesc, (kb == 0 && k == 0) ? 0u : 1u);
-                        umma_f16(d_tmem, dLh + off, dRl + off, p.idesc, 1);
-                        umma_f16(d_tmem, dLh + off, dRh + off, p.idesc, 1);
-                    }
-                    umma_commit(&empty[s]);
-                }
-                umma_commit(&tfull[buf]);
-            }
-        }
     } else {
-        // ================= epilogue: warps 2..5 <-> TMEM lane quadrants (warp % 4) =================
-        const int q = warp & 3;
-        float* col = scratch + q * PT_SCRATCH_FLOATS + lane;        // this lane's private column: col[k * 32] <-> accumulator column 32 q + k
-        int tc = 0;
-        for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x, ++tc) {
-            const int buf = tc & 1, use = tc >> 1;
-            mbar_wait(&tfull[buf], use & 1);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * PT_N + q * 32);
-            {
-                uint32_t v[32];
-                tmem_ld32(taddr, v);
-#pragma unroll
-                for (int k = 0; k < 32; ++k) col[k * 32] = __uint_as_float(v[k]);
-                tmem_ld32(taddr + 32, v);
-#pragma unroll
-                for (int k = 0; k < 32; ++k) col[(k + 32) * 32] = __uint_as_float(v[k]);
-            }
-            tc_fence_before();
+        // ================= consumer warpgroups =================
+        const int wg = warp >> 2;
+        auto release = [&](int st) {
             __syncwarp();
-            if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tempty[buf])) : "memory");
-            const long long pix = (long long)tile * PT_M + q * 32 + lane;
+            if (st >= 0 && lane == 0) mbar_arrive(&empty[st]);
+        };
+        float acc[PT_N / 2];
+        int it = 0;
+        const int t = warp * 32 + lane, row = t & (PT_M - 1), dh = t >> 7;
+        for (int tile = blockIdx.x; tile < p.ntiles; tile += gridDim.x) {
+            int pend = -1;
+            for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
+                const int s = it % PT_STAGES, ph = (it / PT_STAGES) & 1;
+                mbar_wait(&full[s], ph);
+                const uint32_t sa = smem_u32(smem + (size_t)s * PT_STAGE_BYTES);
+                const uint32_t la = sa + (uint32_t)wg * 64u * 128u;
+                const uint64_t dLh = make_sdesc(la), dLl = make_sdesc(la + PT_L_BYTES);
+                const uint64_t dRh = make_sdesc(sa + 2 * PT_L_BYTES), dRl = make_sdesc(sa + 2 * PT_L_BYTES + PT_R_BYTES);
+                wg_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint64_t off = (uint64_t)((k * 32) >> 4);
+                    wgmma_f16<PT_N>(acc, dLl + off, dRh + off, (kb == 0 && k == 0) ? 0u : 1u);
+                    wgmma_f16<PT_N>(acc, dLh + off, dRl + off, 1u);
+                    wgmma_f16<PT_N>(acc, dLh + off, dRh + off, 1u);
+                }
+                wg_commit();
+                if (kb == p.kblocks - 1) { wg_wait<0>(); release(pend); release(s); }
+                else { wg_wait<1>(); release(pend); pend = s; }
+            }
+            wg_fence_regs(acc);
+            consumers_sync();                                  // the previous tile's band has been read
+            {
+                const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < PT_N / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int r = r0 + 8 * (e >> 1), k = 8 * j + c0 + (e & 1) - r;      // window pixel - L pixel
+                        if (k >= 0 && k <= PT_PAD) band[r * PT_BAND_LD + k] = acc[4 * j + e];
+                    }
+            }
+            consumers_sync();
+            const long long pix = (long long)tile * PT_M + row;
             if (pix < p.npix) {
                 const int x = (int)(pix % p.W);
                 float* op = p.out + pix * p.out_cs + p.out_co;
-                // disparity d <-> window pixel (32 q + lane) - d + 32 <-> private column entry k = lane + 32 - d
-                for (int d = 0; d < p.D; d += 4) {
+                const float* bp = band + row * PT_BAND_LD;
+                // disparity d <-> window pixel row - d + 32 <-> band entry 32 - d
+                for (int d = 4 * dh; d < p.D; d += 8) {
                     float4 o;
-                    o.x = (x >= d + 0) ? col[(lane + 32 - d) * 32] * p.inv_c : 0.f;
-                    o.y = (x >= d + 1) ? col[(lane + 31 - d) * 32] * p.inv_c : 0.f;
-                    o.z = (x >= d + 2) ? col[(lane + 30 - d) * 32] * p.inv_c : 0.f;
-                    o.w = (x >= d + 3) ? col[(lane + 29 - d) * 32] * p.inv_c : 0.f;
+                    o.x = (x >= d + 0) ? bp[32 - d] * p.inv_c : 0.f;
+                    o.y = (x >= d + 1) ? bp[31 - d] * p.inv_c : 0.f;
+                    o.z = (x >= d + 2) ? bp[30 - d] * p.inv_c : 0.f;
+                    o.w = (x >= d + 3) ? bp[29 - d] * p.inv_c : 0.f;
                     *reinterpret_cast<float4*>(op + d) = o;
                 }
             }
-            __syncwarp();
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
     }
 }
 
@@ -178,8 +153,6 @@ extern "C" int vd3d_psm_cosine_h16(const void* l_hi, const void* l_lo, const voi
     memset(&p, 0, sizeof(p));
     p.npix = npix; p.W = W; p.D = D; p.kblocks = C / 64; p.ntiles = (int)((npix + PT_M - 1) / PT_M);
     p.out_cs = out_cs; p.out_co = out_co; p.inv_c = 1.0f / (float)C; p.out = out;
-    // instruction descriptor: D = f32, A = B = f16, K-major, N = 160, M = 128
-    p.idesc = (1u << 4) | ((uint32_t)(PT_N >> 3) << 17) | ((uint32_t)(PT_M >> 4) << 24);
     CUtensorMap mLh, mLl, mRh, mRl;
     int rc;
     const __half* lh = (const __half*)l_hi + co; const __half* ll = (const __half*)l_lo + co;
@@ -188,7 +161,7 @@ extern "C" int vd3d_psm_cosine_h16(const void* l_hi, const void* l_lo, const voi
     if ((rc = make_map_2d_h16(&mLl, ll, npix, C, cs, PT_M, "psm_cosine_h16"))) return rc;
     if ((rc = make_map_2d_h16(&mRh, rh, npix, C, cs, PT_N, "psm_cosine_h16"))) return rc;
     if ((rc = make_map_2d_h16(&mRl, rl, npix, C, cs, PT_N, "psm_cosine_h16"))) return rc;
-    const size_t smem = (size_t)PT_STAGES * PT_STAGE_BYTES + 4 * PT_SCRATCH_FLOATS * sizeof(float) + (2 * PT_STAGES + 5) * sizeof(uint64_t) + 1024;
+    const size_t smem = (size_t)PT_STAGES * PT_STAGE_BYTES + PT_M * PT_BAND_LD * sizeof(float) + 2 * PT_STAGES * sizeof(uint64_t) + 1024;
     static bool attr_set = false;
     if (!attr_set) {
         VD3D_CUDA(cudaFuncSetAttribute(psm_cosine_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));

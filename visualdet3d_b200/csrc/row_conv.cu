@@ -1,20 +1,22 @@
 // Few-channel KHxKW convolutions (the DLA-34 front end: base_layer 7x7 3 -> 16, level0 3x3 16 -> 16, level1 3x3 / 2 16 -> 32 at full image
-// resolution, R/networks/backbones/dla.py:246-262) on the tensor cores as ROW-STRIP kernels: the generalisation of stem_pool.cu without the pool.
+// resolution, R/networks/backbones/dla.py:246-262) on the Hopper tensor cores (wgmma) as ROW-STRIP kernels: the generalisation of stem_pool.cu
+// without the pool.
 //
 // The input is kept as fp16 (hi, lo) ROW PLANES [B][H][Wp][PC] (PC = 4, 8 or 16 channels = 8, 16 or 32 bytes per pixel, `xoff` >= pad zero pixels
 // in front of every row, zeros behind).  For filter row ky the KW * PC operand values of output column m are CONTIGUOUS in the staged image row and
-// start S * PC * 2 bytes after those of column m - 1.  A K-major no-swizzle UMMA operand has its core-matrix rows 16 bytes apart, so the
+// start S * PC * 2 bytes after those of column m - 1.  A K-major no-swizzle wgmma operand has its core-matrix rows 16 bytes apart, so the
 // descriptor (leading byte offset 16, stride byte offset 128) reads operand row r at byte 16 r of the staged row: output column m is operand row
 // RS * m with RS = S * PC * 2 / 16 (1, 2 or 4); the rows in between are windows that start inside a pixel: computed and ignored.  A tile is one
 // conv row x 128 / RS output columns; nothing is gathered or re-laid-out, and an image row is loaded once per strip (ring of 16 rows, 1-D bulk
 // copies, rows outside the image zero-filled by the producer warp).  Weights: KH blocks [N][KS * 16] fp16 hi | lo (k = kx * PC + c, zero beyond
 // KW * PC), resident in shared memory.  Three MMAs per K step (A_lo W_hi, A_hi W_lo, A_hi W_hi), promotion chunks of <= 4 filter rows.
-// The exact-fp32 SIMT kernel these layers ran on needs 1.4 + 1.0 + 0.36 ms per batch-8 MonoFlex step at 384x1280 (15 .. 18 % of the step).
+// Warps 0..7 = two consumer warpgroups (operand rows 64 w .. 64 w + 63: MMAs, promotion, then the epilogue of the conv row through a staged
+// [128][N + 4] shared-memory tile), warp 8 = row producer.
 #include "tc_conv.cuh"
 
 namespace vd3d {
 
-constexpr int RC_THREADS = 192;                  // warps: 0 = row producer, 1 = MMA issuer + TMEM owner, 2..5 = epilogue (one per TMEM lane quadrant)
+constexpr int RC_THREADS = 256 + 32;             // warps: 0..7 = consumers, 8 = row producer
 constexpr int RC_RING = 16;                      // staged image rows
 
 struct RcParams {
@@ -26,23 +28,14 @@ struct RcParams {
     int nstrips, nseg, seg_rows, pxs;            // pxs = output columns per strip = 128 / RS
     int rowb;                                    // staged bytes per image row and plane
     int N, w_block;                              // output channels; bytes of one filter-row weight block per plane (N * KS * 32)
-    uint32_t w_layout, w_sbo;                    // UMMA layout type / stride byte offset of the weight blocks (SWIZZLE_64B: 4 / 512, SWIZZLE_128B: 2 / 1024)
+    uint32_t w_layout, w_sbo;                    // descriptor layout type / stride byte offset of the weight blocks (SWIZZLE_64B: 4 / 512, SWIZZLE_128B: 2 / 1024)
     float out_scale; const float* bias; int relu;
     float* out; __half* out_hi; __half* out_lo;  // NHWC [B][Ho][out_W][out_cs], image column x at out_xoff + x
     int out_W, out_xoff, out_cs, out_co;
     int* range_flag;
-    uint32_t idesc, tmem_cols;
     int dbg;
 };
 
-__device__ __forceinline__ uint64_t rc_sdesc_ns(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
 __device__ __forceinline__ void rc_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes),
                  "r"(smem_u32(bar)) : "memory");
@@ -59,40 +52,31 @@ __global__ void __launch_bounds__(RC_THREADS, 1)
 row_conv_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const RcParams q) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    constexpr int LD = N + 4;
     uint8_t* wsm = smem;                                                       // [KH][hi | lo] weight blocks
     uint8_t* ring = wsm + (((size_t)q.KH * 2 * q.w_block + 1023) & ~(size_t)1023);      // [RC_RING][hi | lo] image rows
     const uint32_t slotb = 2u * (uint32_t)q.rowb;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)RC_RING * slotb);
+    float* tile = reinterpret_cast<float*>(ring + (size_t)RC_RING * slotb);   // [128][LD] staged accumulator of one conv row
+    uint64_t* bars = reinterpret_cast<uint64_t*>(tile + 128 * LD);
     uint64_t* full = bars;                       // [RC_RING]
-    uint64_t* empty = full + RC_RING;            // [RC_RING]
+    uint64_t* empty = full + RC_RING;            // [RC_RING]  consumers (8 warps) -> producer
     uint64_t* fullW = empty + RC_RING;           // [1]
-    uint64_t* tmem_full = fullW + 1;             // [4]
-    uint64_t* tmem_empty = tmem_full + 4;        // [4]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int units = q.B * q.nstrips * q.nseg;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
     const int NCH = q.KH > 4 ? 2 : 1;            // promotion chunks per conv row
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < RC_RING; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        for (int s = 0; s < RC_RING; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         mbar_init(fullW, 1);
-        for (int i = 0; i < 4; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(q.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, *tmem_slot);
     pdl_launch_dependents();
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= producer: the weights once, then S image rows per conv row =================
         if (elect_one()) {
             mbar_expect_tx(fullW, (uint32_t)q.KH * 2u * (uint32_t)q.w_block);
@@ -132,96 +116,71 @@ row_conv_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_constan
                 __syncwarp();
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer (one elected lane) =================
-        if (elect_one()) {
-            mbar_wait(fullW, 0);
-            tc_fence_after();
-            const uint32_t wbase = smem_u32(wsm), rbase = smem_u32(ring);
-            int gl = 0, cc = 0;
-            for (int u = u0; u < units; u += ustep) {
-                int b, strip, y0, T;
-                rc_unit(q, u, b, strip, y0, T);
-                for (int t = 0; t < T; ++t) {
-                    // conv row t reads local image rows S t .. S t + KH - 1; rows up to S t + KH - S - 1 were waited for by earlier conv rows
-                    for (int l = (t == 0 ? 0 : q.S * t + q.KH - q.S); l < q.S * t + q.KH; ++l) mbar_wait(&full[(gl + l) % RC_RING], ((gl + l) / RC_RING) & 1);
-                    tc_fence_after();
-                    for (int chunk = 0; chunk < NCH; ++chunk, ++cc) {
-                        const int buf = cc & 3;
-                        mbar_wait(&tmem_empty[buf], ((cc >> 2) & 1) ^ 1);
-                        tc_fence_after();
-                        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * N);
-                        const int ky0 = chunk * 4, ky1 = (chunk == NCH - 1) ? q.KH : 4;
-                        for (int ky = ky0; ky < ky1; ++ky) {
-                            const uint32_t ra = rbase + (uint32_t)((gl + q.S * t + ky) % RC_RING) * slotb;
-                            const uint32_t wa = wbase + (uint32_t)(ky * 2 * q.w_block);
-                            for (int s = 0; s < q.KS; ++s) {
-                                const uint64_t dA = rc_sdesc_ns(ra + 32u * s, 16u, 128u), dAlo = rc_sdesc_ns(ra + q.rowb + 32u * s, 16u, 128u);
-                                const uint64_t dB = make_sdesc(wa, q.w_sbo, q.w_layout) + (uint64_t)(2 * s);
-                                const uint64_t dBlo = make_sdesc(wa + q.w_block, q.w_sbo, q.w_layout) + (uint64_t)(2 * s);
-                                const uint32_t first = (ky == ky0 && s == 0) ? 0u : 1u;
-                                if (q.dbg & 1) { umma_f16(d_tmem, dA, dB, q.idesc, first); continue; }
-                                umma_f16(d_tmem, dAlo, dB, q.idesc, first);
-                                umma_f16(d_tmem, dA, dBlo, q.idesc, 1u);
-                                umma_f16(d_tmem, dA, dB, q.idesc, 1u);
-                            }
-                        }
-                        umma_commit(&tmem_full[buf]);
-                    }
-                    for (int l = q.S * t; l < q.S * (t + 1); ++l) umma_commit(&empty[(gl + l) % RC_RING]);      // not read by the next conv row
-                }
-                const int L = q.S * (T - 1) + q.KH;
-                for (int l = q.S * T; l < L; ++l) umma_commit(&empty[(gl + l) % RC_RING]);
-                gl += L;
-            }
-        }
-        __syncwarp();
     } else {
-        // ================= epilogue: one warp per TMEM lane quadrant, thread = operand row =================
-        const int qd = warp & 3;
-        const int r = qd * 32 + lane;
-        const uint32_t te = smem_u32(&tmem_empty[0]);
+        // ================= consumer warpgroups: MMAs of operand rows 64 wg .. 64 wg + 63, promotion, epilogue =================
+        const int wg = warp >> 2;
+        const int qd = warp & 3, half = warp >> 2;
+        const int r = qd * 32 + lane;                                  // epilogue: operand row of this thread, columns [half N / 2, +N / 2)
         const float osc = q.out_scale;
         const bool lane_px = (r % q.RS) == 0;
         const int xl = r / q.RS;                                       // output column inside the strip
+        auto release = [&](int slot) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[slot]);
+        };
+        mbar_wait(fullW, 0);
+        const uint32_t wbase = smem_u32(wsm), rbase = smem_u32(ring);
         float amax = 0.f;
-        int cc = 0;
+        float tot[N / 2], c[N / 2];
+        int gl = 0;
         for (int u = u0; u < units; u += ustep) {
             int b, strip, y0, T;
             rc_unit(q, u, b, strip, y0, T);
             const int x = strip * q.pxs + xl;
             const bool ok = lane_px && x < q.Wo && !(q.dbg & 16);
             for (int t = 0; t < T; ++t) {
-                float acc[N];
+                // conv row t reads local image rows S t .. S t + KH - 1; rows up to S t + KH - S - 1 were waited for by earlier conv rows
+                for (int l = (t == 0 ? 0 : q.S * t + q.KH - q.S); l < q.S * t + q.KH; ++l) mbar_wait(&full[(gl + l) % RC_RING], ((gl + l) / RC_RING) & 1);
 #pragma unroll
-                for (int k = 0; k < N; ++k) acc[k] = 0.f;
-                for (int chunk = 0; chunk < NCH; ++chunk, ++cc) {
-                    const int buf = cc & 3;
-                    mbar_wait(&tmem_full[buf], (cc >> 2) & 1);
-                    tc_fence_after();
-#pragma unroll
-                    for (int g = 0; g < N / 16; ++g) {
-                        uint32_t v[16];
-                        tmem_ld16(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(buf * N + g * 16), v);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) acc[g * 16 + i] += __uint_as_float(v[i]);
+                for (int k = 0; k < N / 2; ++k) tot[k] = 0.f;
+                for (int chunk = 0; chunk < NCH; ++chunk) {
+                    const int ky0 = chunk * 4, ky1 = (chunk == NCH - 1) ? q.KH : 4;
+                    wg_fence();
+                    for (int ky = ky0; ky < ky1; ++ky) {
+                        const uint32_t ra = rbase + (uint32_t)((gl + q.S * t + ky) % RC_RING) * slotb + (uint32_t)wg * 64u * 16u;
+                        const uint32_t wa = wbase + (uint32_t)(ky * 2 * q.w_block);
+                        for (int s = 0; s < q.KS; ++s) {
+                            const uint64_t dA = make_sdesc_ns(ra + 32u * s, 16u, 128u), dAlo = make_sdesc_ns(ra + q.rowb + 32u * s, 16u, 128u);
+                            const uint64_t dB = make_sdesc(wa, q.w_sbo, q.w_layout) + (uint64_t)(2 * s);
+                            const uint64_t dBlo = make_sdesc(wa + q.w_block, q.w_sbo, q.w_layout) + (uint64_t)(2 * s);
+                            const uint32_t first = (ky == ky0 && s == 0) ? 0u : 1u;
+                            if (q.dbg & 1) { wgmma_f16<N>(c, dA, dB, first); continue; }
+                            wgmma_f16<N>(c, dAlo, dB, first);
+                            wgmma_f16<N>(c, dA, dBlo, 1u);
+                            wgmma_f16<N>(c, dA, dB, 1u);
+                        }
                     }
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(te + (uint32_t)buf * 8u) : "memory");
+                    wg_commit();
+                    wg_wait<0>();
+                    wg_promote(tot, c);
                 }
+                for (int l = q.S * t; l < q.S * (t + 1); ++l) release((gl + l) % RC_RING);      // not read by the next conv row
+                consumers_sync();                                      // the previous conv row's staged accumulator has been read
+                wg_stage<N>(tot, tile, LD, wg, warp, lane);
+                consumers_sync();
                 if (ok) {
+                    const float* acc = tile + r * LD;
                     const long long pix = ((long long)b * q.Ho + (y0 + t)) * q.out_W + q.out_xoff + x;
                     const long long o = pix * q.out_cs + q.out_co;
 #pragma unroll
-                    for (int k = 0; k < N; k += 8) {
+                    for (int k = half * (N / 2); k < (half + 1) * (N / 2); k += 8) {
                         float a[8];
 #pragma unroll
                         for (int m = 0; m < 8; m += 4) {
                             const float4 bb = q.bias ? ldg4(q.bias + k + m) : make_float4(0.f, 0.f, 0.f, 0.f);
-                            a[m] = acc[k + m] * osc + bb.x; a[m + 1] = acc[k + m + 1] * osc + bb.y;
-                            a[m + 2] = acc[k + m + 2] * osc + bb.z; a[m + 3] = acc[k + m + 3] * osc + bb.w;
+                            const float4 av = *reinterpret_cast<const float4*>(acc + k + m);
+                            a[m] = av.x * osc + bb.x; a[m + 1] = av.y * osc + bb.y;
+                            a[m + 2] = av.z * osc + bb.z; a[m + 3] = av.w * osc + bb.w;
                         }
                         if (q.relu) {
 #pragma unroll
@@ -243,14 +202,11 @@ row_conv_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_constan
                     }
                 }
             }
+            const int L = q.S * (T - 1) + q.KH;
+            for (int l = q.S * T; l < L; ++l) release((gl + l) % RC_RING);
+            gl += L;
         }
         if (q.out_hi) note_fp16_range(amax, q.range_flag);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(q.tmem_cols) : "memory");
     }
 }
 
@@ -349,22 +305,20 @@ extern "C" int vd3d_row_conv(const void* in_hi, const void* in_lo, int B, int H,
     q.out_scale = out_scale; q.bias = bias; q.relu = relu;
     q.out = out; q.out_hi = (__half*)out_hi16; q.out_lo = (__half*)out_lo16; q.out_W = out_W; q.out_xoff = out_xoff; q.out_cs = out_cs; q.out_co = out_co;
     q.range_flag = out_hi16 ? fp16_range_flag() : nullptr;
-    q.idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    q.tmem_cols = 4 * N < 32 ? 32 : 4 * N;
     { const char* e = getenv("VD3D_TC_DEBUG"); q.dbg = e ? atoi(e) : 0; }
     CUtensorMap mWhi, mWlo;
     int rc;
     if ((rc = make_map_wgt(&mWhi, w_hi, N, KH * q.KS * 16, N, 2, q.KS * 32))) return rc;
     if ((rc = make_map_wgt(&mWlo, w_lo, N, KH * q.KS * 16, N, 2, q.KS * 32))) return rc;
     const size_t wbytes = ((size_t)KH * 2 * q.w_block + 1023) & ~(size_t)1023;
-    const size_t smem = wbytes + (size_t)RC_RING * 2 * q.rowb + (2 * RC_RING + 1 + 8 + 2) * sizeof(uint64_t) + 1024;
+    const size_t smem = wbytes + (size_t)RC_RING * 2 * q.rowb + (size_t)128 * (N + 4) * sizeof(float) + (2 * RC_RING + 1) * sizeof(uint64_t) + 1024;
     static bool attr_set = false;
     if (!attr_set) {
-        VD3D_CUDA(cudaFuncSetAttribute(row_conv_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-        VD3D_CUDA(cudaFuncSetAttribute(row_conv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+        VD3D_CUDA(cudaFuncSetAttribute(row_conv_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        VD3D_CUDA(cudaFuncSetAttribute(row_conv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         attr_set = true;
     }
-    VD3D_REQUIRE(smem <= 160 * 1024, "row_conv: shared-memory budget exceeded");
+    VD3D_REQUIRE(smem <= 227 * 1024, "row_conv: shared-memory budget exceeded");
     const int units = B * q.nstrips * q.nseg;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));

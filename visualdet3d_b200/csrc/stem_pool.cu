@@ -1,9 +1,9 @@
-// ResNet stem as ONE persistent tcgen05 kernel: conv 7x7 / stride 2 / pad 3 (<= 4 -> 64 channels) + folded BN + ReLU + MaxPool2d(3, 2, 1)
+// ResNet stem as ONE persistent wgmma kernel: conv 7x7 / stride 2 / pad 3 (<= 4 -> 64 channels) + folded BN + ReLU + MaxPool2d(3, 2, 1)
 // (R/networks/backbones/resnet.py:120-122,186-189), with NO im2col and no window re-reads from L2.
 //
 // conv2d_tcp_kernel's stem path presents the image to TMA as a virtual [B][H][Wo][32] tensor with overlapping windows: every tile loads its
-// 7 x 128 windows again, 3.1 GB of L2 -> SM traffic per batch-16 launch (ncu, profiles/r02_ncu_conv2d_all.txt row 0), which is what bounds it
-// (527 us at 16 % tensor-pipe utilisation).  Here the overlap is expressed in the UMMA shared-memory descriptor instead:
+// 7 x 128 windows again (3.1 GB of L2 -> SM traffic per batch-16 launch at 384 x 1280), which is what bounds it.
+// Here the overlap is expressed in the wgmma shared-memory descriptor instead:
 //   * a tile is ONE conv output row x 128 output columns.  For filter row ky the 32 operand values of output column m (8 pixels x 4 channels
 //     of the fp16 row planes, pixel 2m .. 2m + 7 of the padded row) start 16 bytes after those of column m - 1.  A K-major, NO-swizzle operand
 //     has its 8-row core matrices at a 16-byte row pitch, so with leading byte offset 16 (next 16-byte K chunk) and stride byte offset 128
@@ -12,6 +12,8 @@
 //   * a CTA walks DOWN a strip of 128 conv columns: consecutive conv rows share 5 of their 7 image rows, so the producer streams two new
 //     image rows per conv row (1-D bulk copies into a ring of 8 row pairs; out-of-image rows are zero-filled by the producer warp).
 //     The weights (7 filter rows x [64][32] fp16 hi | lo, 56 KB) are loaded once per CTA.
+//   * warps 0..7 = two consumer warpgroups (strip columns 64 w .. 64 w + 63): the MMAs of a conv row, the promotion of its two chunks, and
+//     the epilogue on the accumulator staged in shared memory ([128][68] fp32); warp 8 = producer.
 //   * the max-pool happens in registers: thread (column x) keeps the running maximum of its column over the conv rows of the open pooled row;
 //     after every second conv row the horizontal 3-max of these column maxima (neighbour columns by warp shuffle, the one column across a warp
 //     boundary through 2 KB of shared memory) is the pooled row, and it is written.  Strips overlap by 2 conv columns (63 pooled columns per 128-column strip) and row segments by one conv row, so every
@@ -24,7 +26,7 @@
 
 namespace vd3d {
 
-constexpr int SP_THREADS = 320;                  // warps: 0 = image-row producer, 1 = MMA issuer + TMEM owner, 2..9 = epilogue
+constexpr int SP_THREADS = 256 + 32;             // warps: 0..7 = consumers (MMAs, promotion, epilogue), 8 = image-row producer
 constexpr int SP_KH = 7, SP_STRIDE = 2, SP_PAD = 3;
 constexpr int SP_XOFF = 5;                       // zero pixels in front of every row of the planes (pad 3 + 2: column -1 of strip 0 stays in the row)
 constexpr int SP_ROWB = 2112;                    // staged bytes per image row and plane: 264 pixels x 4 channels x fp16
@@ -33,6 +35,7 @@ constexpr int SP_PAIRS = 8;                      // ring of row pairs
 constexpr int SP_PAIR = 2 * SP_ROW;              // 8448 B
 constexpr int SP_CENTERS = 63;                   // pooled columns per strip (conv columns 126 t - 1 .. 126 t + 126)
 constexpr int SP_WROW = 2 * 64 * 64;             // weights of one filter row: [hi | lo][64 cout][32 k] fp16, SWIZZLE_64B
+constexpr int SP_LD = 68;                        // floats per staged accumulator row (64 + 4: conflict-free float4 rows)
 
 struct SpParams {
     const __half* in_hi; const __half* in_lo;    // [B][H][Wp][4]
@@ -43,20 +46,8 @@ struct SpParams {
     float* out; __half* out_hi; __half* out_lo;   // pooled NHWC tensor: fp32 (optional) and / or fp16 (hi, lo) planes (optional)
     int out_cs, out_co;
     int* range_flag;
-    uint32_t idesc;
     int dbg;
 };
-
-// K-major, no-swizzle shared-memory matrix descriptor (cute::UMMA::LayoutType::SWIZZLE_NONE): 8-row x 16-byte core matrices,
-// `lbo` bytes between core matrices adjacent in K, `sbo` bytes between core matrices adjacent in M
-__device__ __forceinline__ uint64_t make_sdesc_ns(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
 
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes),
@@ -77,36 +68,26 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_consta
     uint8_t* wsm = smem;                                          // [7][hi | lo] weights, 1024-byte aligned blocks
     uint8_t* ring = wsm + (size_t)SP_KH * SP_WROW;                // [SP_PAIRS][2 rows][hi | lo]
     float* edge = reinterpret_cast<float*>(ring + (size_t)SP_PAIRS * SP_PAIR);     // [2 parities][2 halves][4 quadrants][32]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(edge + 2 * 2 * 4 * 32);
-    uint64_t* full = bars;                       // [SP_PAIRS] producer -> MMA
-    uint64_t* empty = full + SP_PAIRS;           // [SP_PAIRS] MMA -> producer
+    float* stage = edge + 2 * 2 * 4 * 32;                         // [128][SP_LD] staged accumulator of one conv row
+    uint64_t* bars = reinterpret_cast<uint64_t*>(stage + 128 * SP_LD);
+    uint64_t* full = bars;                       // [SP_PAIRS] producer -> consumers
+    uint64_t* empty = full + SP_PAIRS;           // [SP_PAIRS] consumers (8 warps) -> producer
     uint64_t* fullW = empty + SP_PAIRS;          // [1]
-    uint64_t* tmem_full = fullW + 1;             // [4]
-    uint64_t* tmem_empty = tmem_full + 4;        // [4]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 4);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
     const int units = q.B * q.nstrips * q.nseg;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < SP_PAIRS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        for (int s = 0; s < SP_PAIRS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         mbar_init(fullW, 1);
-        for (int i = 0; i < 4; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __reduce_or_sync(0xffffffffu, *tmem_slot);
     pdl_launch_dependents();
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 8) {
         // ================= producer: the weights once, then two image rows per conv row =================
         if (elect_one()) {
             mbar_expect_tx(fullW, (uint32_t)SP_KH * SP_WROW);
@@ -154,66 +135,28 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_consta
                 __syncwarp();
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer (one elected lane) =================
-        if (elect_one()) {
-            mbar_wait(fullW, 0);
-            tc_fence_after();
-            const uint32_t wbase = smem_u32(wsm), rbase = smem_u32(ring);
-            int gq = 0, cc = 0;
-            for (int u = u0; u < units; u += ustep) {
-                int b, strip, i0, nrows;
-                sp_unit(q, u, b, strip, i0, nrows);
-                const int T = 2 * nrows + 1;
-                for (int t = 0; t < T; ++t) {
-                    // image rows of conv row t: local rows 2t .. 2t + 6 = pairs t .. t + 3
-                    for (int pq = (t == 0 ? 0 : t + 3); pq <= t + 3; ++pq) mbar_wait(&full[(gq + pq) % SP_PAIRS], ((gq + pq) / SP_PAIRS) & 1);
-                    tc_fence_after();
-#pragma unroll 1
-                    for (int chunk = 0; chunk < 2; ++chunk, ++cc) {
-                        const int buf = cc & 3;
-                        mbar_wait(&tmem_empty[buf], ((cc >> 2) & 1) ^ 1);
-                        tc_fence_after();
-                        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * 64);
-                        const int ky0 = chunk * 4, ky1 = chunk ? SP_KH : 4;
-                        for (int ky = ky0; ky < ky1; ++ky) {
-                            const int l = 2 * t + ky;                                        // local image row
-                            const uint32_t ra = rbase + (uint32_t)(((gq + (l >> 1)) % SP_PAIRS) * SP_PAIR + (l & 1) * SP_ROW);
-                            const uint32_t wa = wbase + (uint32_t)(ky * SP_WROW);
-#pragma unroll
-                            for (int s = 0; s < 2; ++s) {
-                                const uint64_t dA = make_sdesc_ns(ra + 32u * s, 16u, 128u), dAlo = make_sdesc_ns(ra + SP_ROWB + 32u * s, 16u, 128u);
-                                const uint64_t dB = make_sdesc(wa, 512u, 4u) + (uint64_t)(2 * s), dBlo = make_sdesc(wa + SP_WROW / 2, 512u, 4u) + (uint64_t)(2 * s);
-                                if (q.dbg & 1) { umma_f16(d_tmem, dA, dB, q.idesc, (ky == ky0 && s == 0) ? 0u : 1u); continue; }
-                                umma_f16(d_tmem, dAlo, dB, q.idesc, (ky == ky0 && s == 0) ? 0u : 1u);
-                                umma_f16(d_tmem, dA, dBlo, q.idesc, 1u);
-                                umma_f16(d_tmem, dA, dB, q.idesc, 1u);
-                            }
-                        }
-                        umma_commit(&tmem_full[buf]);
-                    }
-                    umma_commit(&empty[(gq + t) % SP_PAIRS]);                              // rows 2t, 2t + 1 are not read again
-                }
-                for (int pq = T; pq < T + 3; ++pq) umma_commit(&empty[(gq + pq) % SP_PAIRS]);
-                gq += T + 3;
-            }
-        }
-        __syncwarp();
     } else {
-        // ================= epilogue warps: promotion, bias / ReLU, 3 x 3 / stride-2 max in registers =================
-        const int e = warp - 2, qd = warp & 3, half = e >> 2;
-        const int x = qd * 32 + lane;                                  // conv column inside the strip
-        const uint32_t te = smem_u32(&tmem_empty[0]);
+        // ================= consumer warpgroups: MMAs of strip columns 64 wg .. 64 wg + 63, promotion, bias / ReLU, 3 x 3 / stride-2 max in registers =================
+        const int wg = warp >> 2;
+        const int e = warp, qd = warp & 3, half = e >> 2;
+        const int x = qd * 32 + lane;                                  // epilogue: conv column inside the strip
         const float osc = q.out_scale;
         const int cb = half * 32;
+        auto release = [&](int slot) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[slot]);
+        };
+        mbar_wait(fullW, 0);
+        const uint32_t wbase = smem_u32(wsm), rbase = smem_u32(ring);
         float amax = 0.f;
-        int cc = 0, tile = 0;
+        float tot[32], c[32];
+        int gq = 0, tile = 0;
         for (int u = u0; u < units; u += ustep) {
             int b, strip, i0, nrows;
             sp_unit(q, u, b, strip, i0, nrows);
             const int T = 2 * nrows + 1;
-            const int c = 126 * strip - 1 + x;                         // conv column
-            const bool col_ok = c >= 0 && c < q.Wo;
+            const int cc0 = 126 * strip - 1 + x;                       // conv column
+            const bool col_ok = cc0 >= 0 && cc0 < q.Wo;
             const int jl = (x - 1) >> 1;                               // pooled column inside the strip (x odd)
             const int j = SP_CENTERS * strip + jl;
             const bool centre = (x & 1) && jl < SP_CENTERS && j < q.Wq;
@@ -223,21 +166,45 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_consta
 #pragma unroll
             for (int k = 0; k < 32; ++k) run[k] = 0.f;
             for (int t = 0; t < T; ++t) {
-                float acc[32];
+                // image rows of conv row t: local rows 2t .. 2t + 6 = pairs t .. t + 3
+                for (int pq = (t == 0 ? 0 : t + 3); pq <= t + 3; ++pq) mbar_wait(&full[(gq + pq) % SP_PAIRS], ((gq + pq) / SP_PAIRS) & 1);
 #pragma unroll
-                for (int k = 0; k < 32; ++k) acc[k] = 0.f;
+                for (int k = 0; k < 32; ++k) tot[k] = 0.f;
 #pragma unroll 1
-                for (int chunk = 0; chunk < 2; ++chunk, ++cc) {
-                    const int buf = cc & 3;
-                    mbar_wait(&tmem_full[buf], (cc >> 2) & 1);
-                    tc_fence_after();
-                    uint32_t v[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(buf * 64 + cb), v);
+                for (int chunk = 0; chunk < 2; ++chunk) {
+                    const int ky0 = chunk * 4, ky1 = chunk ? SP_KH : 4;
+                    wg_fence();
+                    for (int ky = ky0; ky < ky1; ++ky) {
+                        const int l = 2 * t + ky;                                        // local image row
+                        const uint32_t ra = rbase + (uint32_t)(((gq + (l >> 1)) % SP_PAIRS) * SP_PAIR + (l & 1) * SP_ROW) + (uint32_t)wg * 64u * 16u;
+                        const uint32_t wa = wbase + (uint32_t)(ky * SP_WROW);
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) acc[i] += __uint_as_float(v[i]);
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(te + (uint32_t)buf * 8u) : "memory");
+                        for (int s = 0; s < 2; ++s) {
+                            const uint64_t dA = make_sdesc_ns(ra + 32u * s, 16u, 128u), dAlo = make_sdesc_ns(ra + SP_ROWB + 32u * s, 16u, 128u);
+                            const uint64_t dB = make_sdesc(wa, 512u, 4u) + (uint64_t)(2 * s), dBlo = make_sdesc(wa + SP_WROW / 2, 512u, 4u) + (uint64_t)(2 * s);
+                            const uint32_t first = (ky == ky0 && s == 0) ? 0u : 1u;
+                            if (q.dbg & 1) { wgmma_f16<64>(c, dA, dB, first); continue; }
+                            wgmma_f16<64>(c, dAlo, dB, first);
+                            wgmma_f16<64>(c, dA, dBlo, 1u);
+                            wgmma_f16<64>(c, dA, dB, 1u);
+                        }
+                    }
+                    wg_commit();
+                    wg_wait<0>();
+                    wg_promote(tot, c);
+                }
+                release((gq + t) % SP_PAIRS);                                    // rows 2t, 2t + 1 are not read again
+                consumers_sync();                                                // the previous conv row's staged accumulator has been read
+                wg_stage<64>(tot, stage, SP_LD, wg, warp, lane);
+                consumers_sync();
+                float acc[32];
+                {
+                    const float* sp = stage + x * SP_LD + cb;
+#pragma unroll
+                    for (int k = 0; k < 32; k += 4) {
+                        const float4 v = *reinterpret_cast<const float4*>(sp + k);
+                        acc[k] = v.x; acc[k + 1] = v.y; acc[k + 2] = v.z; acc[k + 3] = v.w;
+                    }
                 }
                 const int y = 2 * i0 - 1 + t;                          // conv row
                 const bool ok = col_ok && y >= 0 && y < q.Ho;
@@ -303,14 +270,10 @@ stem_pool_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_consta
                     for (int k = 0; k < 32; ++k) run[k] = acc[k];          // conv row 2i + 1 is also the first row of pooled row i + 1
                 }
             }
+            for (int pq = T; pq < T + 3; ++pq) release((gq + pq) % SP_PAIRS);
+            gq += T + 3;
         }
         if (q.out_hi) note_fp16_range(amax, q.range_flag);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
     }
 }
 
@@ -364,13 +327,12 @@ extern "C" int vd3d_stem_pool_fused(const void* in_hi, const void* in_lo, int B,
     }
     q.out_scale = out_scale; q.bias = bias; q.out = out; q.out_hi = (__half*)out_hi16; q.out_lo = (__half*)out_lo16; q.out_cs = out_cs; q.out_co = out_co;
     q.range_flag = out_hi16 ? fp16_range_flag() : nullptr;
-    q.idesc = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
     { const char* e = getenv("VD3D_TC_DEBUG"); q.dbg = e ? atoi(e) : 0; }
     CUtensorMap mWhi, mWlo;
     int rc;
     if ((rc = make_map_wgt(&mWhi, w_hi, 64, SP_KH * 32, 64, 2, 64))) return rc;
     if ((rc = make_map_wgt(&mWlo, w_lo, 64, SP_KH * 32, 64, 2, 64))) return rc;
-    const size_t smem = (size_t)SP_KH * SP_WROW + (size_t)SP_PAIRS * SP_PAIR + 2 * 2 * 4 * 32 * sizeof(float) + (2 * SP_PAIRS + 1 + 8 + 2) * sizeof(uint64_t) + 1024;
+    const size_t smem = (size_t)SP_KH * SP_WROW + (size_t)SP_PAIRS * SP_PAIR + (2 * 2 * 4 * 32 + 128 * SP_LD) * sizeof(float) + (2 * SP_PAIRS + 1) * sizeof(uint64_t) + 1024;
     static bool attr_set = false;
     if (!attr_set) {
         VD3D_CUDA(cudaFuncSetAttribute(stem_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

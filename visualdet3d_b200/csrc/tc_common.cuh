@@ -1,6 +1,7 @@
-// tcgen05 / TMA / mbarrier PTX wrappers and the tensor-map encoder shared by the tensor-core kernels (conv2d_tc.cu, psm_tc.cu).
+// wgmma / TMA / mbarrier PTX wrappers and the tensor-map encoder shared by the tensor-core kernels (conv2d_tc.cu, psm_tc.cu, ...).
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <mutex>
@@ -18,7 +19,8 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// Bounded wait: a protocol bug traps (cudaErrorLaunchFailure on the host) after ~2 s instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (cudaErrorLaunchFailure on the host) after ~2 s instead of hanging the GPU.  (No printf here: a call
+// inside the consumers' wait would make the compiler serialise every in-flight wgmma.)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
     uint32_t done = 0, spins = 0;
@@ -34,7 +36,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         if ((++spins & 0xFFFu) == 0) {
             const long long t = clock64();
             if (t0 == 0) t0 = t;
-            else if (t - t0 > 4000000000LL) { printf("vd3d: mbarrier wait timed out (block %d, thread %d)\n", (int)blockIdx.x, (int)threadIdx.x); __trap(); }
+            else if (t - t0 > 4000000000LL) __trap();
         }
     }
 }
@@ -50,32 +52,7 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-// ---- 2-CTA (cta_group::2) variants: both CTAs of the pair issue their own loads, completion is signalled on the LEADER's barrier ----
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-    uint32_t r; asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank)); return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-        "l"(map), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* map, uint32_t leader_bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-        "l"(map), "r"(leader_bar), "r"(c0), "r"(c1)
-        : "memory");
-}
-// arrive (count 1) on a barrier of any CTA of the cluster, given its shared::cluster address
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// one elected lane of a fully converged warp (the compiler knows exactly one thread runs the guarded code: no per-lane loops
-// around the single-thread tcgen05 / TMA instructions)
+// one elected lane of a fully converged warp (the compiler knows exactly one thread runs the guarded code)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -86,80 +63,56 @@ __device__ __forceinline__ bool elect_one() {
         "}\n" : "=r"(pred));
     return pred != 0;
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 // Programmatic dependent launch (VD3D_PDL=1): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may become resident while its
-// predecessor is still draining; everything it does before pdl_wait() (barrier init, TMEM allocation) overlaps the predecessor's tail, and
+// predecessor is still draining; everything it does before pdl_wait() (barrier init) overlaps the predecessor's tail, and
 // pdl_wait() returns when the predecessor has completed and its writes are visible.  Both are no-ops in an ordinary launch.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor layout)
-// `layout`: cute::UMMA::LayoutType, 2 = SWIZZLE_128B (128-byte rows, 8-row groups 1024 B apart), 4 = SWIZZLE_64B (64-byte rows, 512 B)
+// shared-memory matrix descriptor of wgmma (sm_90): start address, leading / stride byte offsets (16-byte units), layout type in bits 62..63
+// `layout`: the swizzle written by TMA, encoded as the 3-bit field at bit 61: 2 = SWIZZLE_128B (128-byte rows, 8-row groups 1024 B apart),
+// 4 = SWIZZLE_64B (64-byte rows, 512 B), 0 = none -- i.e. the 2-bit wgmma layout type (1, 2, 0) shifted to bit 62
 __device__ __forceinline__ uint64_t make_sdesc(uint32_t saddr, uint32_t sbo = 1024, uint32_t layout = 2) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);        // start address
     d |= (uint64_t)0 << 16;                          // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(sbo >> 4) << 32;                 // stride byte offset between 8-row groups (dense: 8 rows * row bytes)
-    d |= (uint64_t)1 << 46;                          // descriptor version (Blackwell)
     d |= (uint64_t)layout << 61;
     return d;
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// K-major, no-swizzle descriptor: 8-row x 16-byte core matrices, `lbo` bytes between core matrices adjacent in K, `sbo` between those adjacent in M / N
+__device__ __forceinline__ uint64_t make_sdesc_ns(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+    uint64_t d = 0;
+    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
+    return d;
 }
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+
+// ---- warpgroup MMA (wgmma): four consecutive warps issue together; the accumulator lives in their registers ----
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins the accumulator registers at this point of the instruction stream (reads after a wg_wait must not be hoisted above it)
+template <int R> __device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// Writes the fp32 fragment of a 64 x N accumulator (warpgroup `wg` = rows 64 wg .. 64 wg + 63 of the tile) into a row-major [128][ld] shared-memory
+// tile: the per-pixel epilogues read their rows back from there.
+template <int N> __device__ __forceinline__ void wg_stage(const float (&d)[N / 2], float* tile, int ld, int wg, int warp, int lane) {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+        *reinterpret_cast<float2*>(tile + r0 * ld + 8 * j + c0) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(tile + (r0 + 8) * ld + 8 * j + c0) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
 }
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// commit of a cta_group::2 MMA group: arrives on the barrier at the same shared-memory offset in both CTAs of the pair
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// named barrier of the 256 consumer threads (warps 0..7) of the tensor-core kernels
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------------------------
 // host: tensor maps (driver entry point fetched at run time: the library does not link libcuda)

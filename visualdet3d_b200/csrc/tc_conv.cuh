@@ -1,16 +1,17 @@
-// Pieces of the tcgen05 conv engine shared by conv2d_tc.cu (dense convolutions) and dcn_fused.cu (deformable convolutions whose
-// A operand is gathered into shared memory by the kernel itself): kernel parameters, the persistent kernels' epilogue (TMEM chunk
-// promotion -> scale / bias / residual / ReLU -> fp32 value and / or fp16 (hi, lo) planes), the tile order, and host helpers.
+// Pieces of the wgmma conv engine shared by conv2d_tc.cu (dense convolutions) and dcn_fused.cu (deformable convolutions whose
+// A operand is gathered into shared memory by the kernel itself): kernel parameters, the k-block MMA sequence, the persistent kernels'
+// epilogue (staged accumulator -> scale / bias / residual / ReLU -> fp32 value and / or fp16 (hi, lo) planes), the tile order, and host helpers.
 #pragma once
 #include "tc_common.cuh"
 #include <cstdlib>
 
 namespace vd3d {
 
-constexpr int TC_TW = 16, TC_TH = 8;          // output tile = 8 rows x 16 columns = 128 pixels (UMMA M = 128)
-constexpr int TC_BK = 32;                     // channels per k-block (32 floats = one 128-byte swizzle row)
-constexpr int TC_THREADS = 192;
-constexpr int TC_A_BYTES = 128 * 128;         // one A (or Alo) stage: 128 rows x 128 B
+constexpr int TC_TW = 16, TC_TH = 8;          // output tile = 8 rows x 16 columns = 128 pixels (two 64-row warpgroup MMAs)
+constexpr int TC_MAX_BN = 128;                // widest tile: the chunk accumulator and its promoted sum take BN registers per consumer thread
+// Warp roles of the tensor-core kernels: warps 0..7 = two consumer warpgroups (warpgroup w issues the MMAs of tile rows 64 w .. 64 w + 63,
+// promotes the chunks and runs the epilogue), the warps after them produce the operands.
+constexpr int TC_CONSUMERS = 256;
 
 struct TcParams {
     int B, H, W, Cin, KH, KW, pad, dil, stride;
@@ -24,40 +25,25 @@ struct TcParams {
     int tiles_w, tiles_h;
     int stride_w, pad_w;     // W-direction stride / padding (the H direction uses stride / pad); equal to them for ordinary convs
     int m_tiles, n_tiles;    // persistent kernel: tile counts along M (B * tiles_h * tiles_w) and N
-    // fused 3x3 / stride-2 / pad-1 max-pool of the (ReLU) output (the ResNet stem, resnet.py:186-189): when pool_out != nullptr the epilogue of
-    // conv2d_tcp_kernel<2, 1, 0> does not write the conv output at all; it pools every tile in shared memory and writes the pooled tensor
+    // fused 3x3 / stride-2 / pad-1 max-pool of the (ReLU) output (the ResNet stem, resnet.py:186-189): when pool_out != nullptr the epilogue
+    // does not write the conv output at all; it pools every tile in shared memory and writes the pooled tensor
     float* pool_out; int pool_cs, pool_co, pool_H, pool_W;
-    uint32_t pool_smem_off;  // byte offset of the [128][68] fp32 staging tile in dynamic shared memory
-    int m_xmajor;            // pixel order inside the 8 x 16 output tile: 0: m = row * 16 + x (TMA tap boxes), 1: m = x * 8 + row (x-major halo item, see conv2d_tcph_kernel)
     int two_pass;            // error-budget experiments (vd3d_conv2d_tc16 passes = 2): drop the A_lo * W_hi product (activations then carry 11 significant bits)
-    int mblock;              // persistent kernels: scheduling units (tiles / tile pairs) per M block of the L2-aware tile order (0: one block)
-    int rowb;                // bytes per operand row in shared memory = K bytes per k-block: 128 (64 channels, SWIZZLE_128B) or 64 (32, SWIZZLE_64B)
+    int mblock;              // persistent kernels: scheduling units (tiles) per M block of the L2-aware tile order (0: one block)
+    int rowb;                // bytes per operand row in shared memory = K bytes per k-block: 128 (SWIZZLE_128B) or 64 (32 fp16, SWIZZLE_64B)
     int cout_pad;            // Cout rounded up to 16 (ragged last N tile = cout_pad - (n_tiles - 1) * BN columns)
-    int v8;                  // output / residual / bias slices are 32-byte aligned: 256-bit global accesses
+    int v8;                  // output / residual / bias slices are 32-byte aligned (fp16 plane slices then take 16-byte accesses)
     long long* trace; int trace_n;   // VD3D diagnostics (vd3d_tc_set_trace): per-k-block clock64 stamps of CTA 0, [5][trace_n]
-    int dbg;                 // timing experiments only (VD3D_TC_DEBUG; results are wrong): bit 0 = one MMA per k-step, bit 1 = skip the lo-plane loads, bit 3 = tap-major k-block order, bit 4 = no epilogue output, bit 5 = no residual loads
+    int dbg;                 // timing experiments only (VD3D_TC_DEBUG; results are wrong): bit 0 = one MMA per k-step, bit 1 = skip the lo-plane loads, bit 4 = no epilogue output, bit 5 = no residual loads
     int out_cs, out_co, res_cs, res_co, relu;
     const float* bias; const float* res; float* out; float* out_lo;
     const void* res_h16_hi; const void* res_h16_lo;   // residual given as fp16 (hi, lo) planes (value = hi + lo) instead of an fp32 tensor (`res`)
-    uint32_t idesc;
-    uint32_t tmem_cols;
-    // halo kernel (3x3, pad 1, dil 1, fp16 operands): one A item in shared memory serves `h_taps` taps
-    int h_mode;              // 2: full halo (10 rows x 2 half-rows of 10 px, 9 taps / item), 1: vertical halo (16 px x 10 rows per kx, 3 taps / item)
-    int h_taps, h_sa, h_sb;  // taps per A item, A stages, B stages
-    int nbuf;                // persistent kernels: TMEM accumulator (chunk) buffers, 2..4 = min(4, 512 / BN): how many chunks the MMA warp may run ahead of the epilogue
-    int w_res;               // persistent halo kernel: all weight blocks of the (single) N tile stay resident in shared memory
-    uint32_t h_rp, h_sbo;    // bytes per halo row, bytes between 8-pixel groups (UMMA stride byte offset)
 };
 
-// 8 consecutive channels: 256-bit global accesses when the slice is 32-byte aligned (`v8`), else two 128-bit ones
-__device__ __forceinline__ void ld8(const float* ptr, bool v8, float (&v)[8]) {
-    if (v8) {
-        asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(ptr));
-    } else {
-        const float4 a = ldg4(ptr), b = ldg4(ptr + 4);
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-    }
+// 8 consecutive channels (16-byte aligned)
+__device__ __forceinline__ void ld8(const float* ptr, float (&v)[8]) {
+    const float4 a = ldg4(ptr), b = ldg4(ptr + 4);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 // 8 consecutive channels of a tensor kept as fp16 (hi, lo) planes: value = hi + lo (exact in fp32: |lo| <= ulp16(hi) / 2)
 __device__ __forceinline__ void ld8_planes(const __half* hp, const __half* lp, bool v8, float (&v)[8]) {
@@ -85,14 +71,9 @@ __device__ __forceinline__ void ld4_planes(const __half* hp, const __half* lp, f
         v[2 * i] = fh.x + fl.x; v[2 * i + 1] = fh.y + fl.y;
     }
 }
-__device__ __forceinline__ void st8(float* ptr, bool v8, const float (&v)[8]) {
-    if (v8) {
-        asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(ptr), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]),
-                     "f"(v[6]), "f"(v[7]) : "memory");
-    } else {
-        *reinterpret_cast<float4*>(ptr) = make_float4(v[0], v[1], v[2], v[3]);
-        *reinterpret_cast<float4*>(ptr + 4) = make_float4(v[4], v[5], v[6], v[7]);
-    }
+__device__ __forceinline__ void st8(float* ptr, const float (&v)[8]) {
+    *reinterpret_cast<float4*>(ptr) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(ptr + 4) = make_float4(v[4], v[5], v[6], v[7]);
 }
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) { __half2 h = __halves2half2(a, b); return *reinterpret_cast<uint32_t*>(&h); }
 // fp16 (hi, lo) planes of 4 values: hi = rn16(v), lo = rn16(v - hi)
@@ -104,9 +85,8 @@ __device__ __forceinline__ void split4(const float* v, uint2& hv, uint2& lv) {
 }
 
 // Tile order of the persistent kernels.  Unit u -> (mu, nt): M fastest inside an M BLOCK of `mblock` units, then the N tiles, then the
-// next M block.  With one block (mblock == 0) every N tile streams the whole activation tensor again (1408-wide layers: 86 MB of
-// A per pass against ~63 MB of L2 that one SM's traffic can keep: 6 passes = 0.5 GB of DRAM reads); with blocks sized to stay L2-resident
-// the activations are read from DRAM once and the weights once per block.  Pure scheduling: every tile computes the same bits.
+// next M block.  With one block (mblock == 0) every N tile streams the whole activation tensor again; with blocks sized to stay
+// L2-resident the activations are read from DRAM once and the weights once per block.  Pure scheduling: every tile computes the same bits.
 __device__ __forceinline__ void unit_tile(const TcParams& p, int u, int mt_units, int& mu, int& nt) {
     if (p.mblock <= 0 || p.mblock >= mt_units) { mu = u % mt_units; nt = u / mt_units; return; }
     const int per = p.mblock * p.n_tiles;
@@ -117,165 +97,141 @@ __device__ __forceinline__ void unit_tile(const TcParams& p, int u, int mt_units
 }
 __device__ __forceinline__ int unit_nt(const TcParams& p, int u, int mt_units) { int mu, nt; unit_tile(p, u, mt_units, mu, nt); return nt; }
 
-constexpr int TCP_THREADS = 320;
-#ifndef VD3D_TC_CG_DEFAULT
-#define VD3D_TC_CG_DEFAULT 0
-#endif
-
-// epilogue warps of the persistent kernels (warps 2..9): epilogue warp e owns TMEM lane quadrant (warp % 4) and column half e / 4.
-// Per tile: promote every accumulated chunk into registers (tcgen05.ld + round-to-nearest add), then scale / bias / residual /
-// ReLU and write the fp32 value plus the fp16 (hi, lo) planes the next tensor-core conv reads.
-template <int NG16, int CG, int PL>   // PL = 1: "planes" mode (fp32 output optional, residual as fp32 tensor or as fp16 planes); PL = 0: fp32 output + fp32 residual only
-__device__ __forceinline__ void tcp_epilogue(const TcParams& p, uint32_t tmem_base, uint64_t* tmem_full, uint64_t* tmem_empty, int warp, int lane,
-                                             uint32_t rank, int NC, int u0, int ustep, int units, int mt_units) {
-    // ================= epilogue warps =================
-    const int e = warp - 2, q = warp & 3, half = e >> 2;
-    const int half_cols = ((p.BN + 31) / 32) * 16;
-    const int cb = half * half_cols;                                 // first accumulator column of this thread
-    const uint32_t te_local = smem_u32(&tmem_empty[0]);
-    const uint32_t te_leader = CG == 2 ? mapa_shared(te_local, 0) : te_local;
-    const float osc = p.out_scale;
-    float amax = 0.f;                                               // fp16-range guard: largest magnitude written to the fp16 planes
-    int cc = 0;
-    for (int u = u0; u < units; u += ustep) {
-        const int ncols = min(half_cols, min(p.BN, p.cout_pad - unit_nt(p, u, mt_units) * p.BN) - cb);      // valid columns of this thread in this tile (<= 0: none)
-        float acc[NG16][16];
+// One k-block of MMAs of a consumer warpgroup: `ksteps` K steps of 32 bytes (16 fp16 / 8 tf32) inside the operand rows, three products per
+// step (A_lo W_hi, A_hi W_lo, A_hi W_hi: small terms first, then the main product), one (A W) or two (A W_lo, A W) in the experiment modes.
+// `first`: the first k-block of a promotion chunk (the accumulator restarts from zero).
+template <int N, bool F16>
+__device__ __forceinline__ void wg_mma(float (&c)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
+    if constexpr (F16) wgmma_f16<N>(c, da, db, acc); else wgmma_tf32<N>(c, da, db, acc);
+}
+template <int N, bool F16>
+__device__ __forceinline__ void wg_kblock(float (&c)[N / 2], uint64_t dA, uint64_t dAlo, uint64_t dB, uint64_t dBlo, int ksteps, int mode, bool first) {
 #pragma unroll
-        for (int g = 0; g < NG16; ++g)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) acc[g][i] = 0.f;
-        // ---- tile coordinates and pointers (independent of the accumulation) ----
-        int mu, nt;
-        unit_tile(p, u, mt_units, mu, nt);
-        int mt = mu * CG + (int)rank;
-        const bool live = mt < p.m_tiles;
-        const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-        const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
-        const int r = q * 32 + lane;
-        const int ho = th * TC_TH + (p.m_xmajor ? (r & (TC_TH - 1)) : r / TC_TW), wo = tw * TC_TW + (p.m_xmajor ? r / TC_TH : r % TC_TW);
-        const bool ok = live && ho < p.Ho && wo < p.Wo;
-        const long long pix = ok ? ((long long)b * p.Ho + ho) * p.Wo + wo : 0;
-        const float* rp = (ok && p.res && !(p.dbg & 32)) ? p.res + pix * p.res_cs + p.res_co : nullptr;
-        const __half* rph = (PL == 1 && ok && p.res_h16_hi && !(p.dbg & 32)) ? reinterpret_cast<const __half*>(p.res_h16_hi) + pix * p.res_cs + p.res_co : nullptr;
-        const __half* rpl = (PL == 1 && rph) ? reinterpret_cast<const __half*>(p.res_h16_lo) + pix * p.res_cs + p.res_co : nullptr;
-        const bool has_res = rp || (PL == 1 && rph);
-        const int nbase = nt * p.BN + cb;
-        const bool v8 = p.v8 != 0;
-        constexpr int GB = NG16 >= 8 ? 1 : 2;         // 16-column groups per output batch (register budget of the widest variant)
-        // residual values of columns [bt * 16, (bt + GB) * 16): all loads of a batch are issued together
-        auto load_res = [&](int bt, float (&rr)[2 * GB][8]) {
-#pragma unroll
-            for (int j = 0; j < 2 * GB; ++j) {
-                const int col = bt * 16 + j * 8, n = nbase + col;
-                if (bt + j / 2 < NG16 && has_res && col < ncols && n + 8 <= p.Cout) {
-                    if (PL == 0 || rp) ld8(rp + n, v8, rr[j]); else ld8_planes(rph + n, rpl + n, v8, rr[j]);
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) rr[j][k] = 0.f;
-                    if (bt + j / 2 < NG16 && has_res && col < ncols && n + 4 <= p.Cout) {      // Cout % 8 == 4 tail
-                        if (PL == 0 || rp) {
-                            const float4 t4 = ldg4(rp + n);
-                            rr[j][0] = t4.x; rr[j][1] = t4.y; rr[j][2] = t4.z; rr[j][3] = t4.w;
-                        } else ld4_planes(rph + n, rpl + n, rr[j]);
-                    }
-                }
-            }
-        };
-        // narrow tiles (<= 64 columns: one batch, 32 registers): the residual is fetched NOW, so that its global-memory round trip runs under
-        // the accumulation of the tile instead of after it (measured on the 64-channel layers: 36 us of 177 were this exposed latency)
-        constexpr bool PRE = NG16 <= 2;
-        float rr_pre[2 * GB][8];
-        if (PRE) load_res(0, rr_pre);
-        for (int ci = 0; ci < NC; ++ci, ++cc) {
-            const int buf = cc % p.nbuf, use = cc / p.nbuf;
-            mbar_wait(&tmem_full[buf], use & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int g = 0; g < NG16; ++g) {
-                if (g * 16 < ncols) {
-                    uint32_t v[16];
-                    tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * p.BN + cb + g * 16), v);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) acc[g][i] += __uint_as_float(v[i]);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if (CG == 2) mbar_arrive_cluster(te_leader + (uint32_t)buf * 8u);
-                else asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(te_local + (uint32_t)buf * 8u) : "memory");
-            }
+    for (int k = 0; k < 4; ++k) {
+        if (k == ksteps) break;
+        const uint64_t off = (uint64_t)((k * 32) >> 4);
+        const uint32_t acc0 = (first && k == 0) ? 0u : 1u;
+        if (mode == 0) {
+            wg_mma<N, F16>(c, dAlo + off, dB + off, acc0);
+            wg_mma<N, F16>(c, dA + off, dBlo + off, 1u);
+            wg_mma<N, F16>(c, dA + off, dB + off, 1u);
+        } else if (mode == 2) {
+            wg_mma<N, F16>(c, dA + off, dBlo + off, acc0);
+            wg_mma<N, F16>(c, dA + off, dB + off, 1u);
+        } else {
+            wg_mma<N, F16>(c, dA + off, dB + off, acc0);
         }
-        // ---- tile output: scale / bias / residual / ReLU, fp32 value + the fp16 (hi, lo) planes ----
-        if (ok && !(p.dbg & 16)) {
-            float* op = (PL == 0 || p.out) ? p.out + pix * p.out_cs + p.out_co : nullptr;           // nullptr (PL = 1 only): planes-only output, no fp32 copy is written
-            __half* oh = p.out_h16_hi ? reinterpret_cast<__half*>(p.out_h16_hi) + pix * p.out_cs + p.out_co : nullptr;
-            __half* ol16 = p.out_h16_lo ? reinterpret_cast<__half*>(p.out_h16_lo) + pix * p.out_cs + p.out_co : nullptr;
+    }
+}
+// MMA mode of a TcParams launch: 0 = three products (production), 1 = one (passes == 1 or the VD3D_TC_DEBUG bit 0 experiment), 2 = two
+__host__ __device__ __forceinline__ int tc_mma_mode(const TcParams& p) { return (p.passes == 1 || (p.dbg & 1)) ? 1 : (p.two_pass ? 2 : 0); }
+
+// Chunked promotion: the tensor core adds every product into the fp32 accumulator with truncation, so the K loop is cut into chunks of
+// `chunk` k-blocks, each accumulated from zero in `c` and then added with round-to-nearest into the per-thread sum `tot`.
+template <int R> __device__ __forceinline__ void wg_promote(float (&tot)[R], float (&c)[R]) {
+    wg_fence_regs(c);
 #pragma unroll
-            for (int bt = 0; bt < NG16; bt += GB) {
-                float rr[2 * GB][8];
-                if (PRE) {
+    for (int i = 0; i < R; ++i) tot[i] += c[i];
+}
+
+// Epilogue of one tile, run by the 256 consumer threads after the tile's accumulator has been staged in shared memory ([128][ld] fp32, row = tile
+// pixel): thread (warp, lane) owns pixel row 32 (warp % 4) + lane and column half warp / 4.  Scale / bias / residual / ReLU, then the fp32 value
+// (and its tf32 `lo` companion when asked) and / or the fp16 (hi, lo) planes the next tensor-core conv reads.  Returns the largest magnitude
+// written to fp16 planes (fp16-range guard).
+template <int N>
+__device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int warp, int lane) {
+    constexpr int HALF = ((N + 31) / 32) * 16;                     // accumulator columns per thread
+    const int q = warp & 3, half = warp >> 2;
+    const int cb = half * HALF;
+    int mu, nt;
+    unit_tile(p, u, mt_units, mu, nt);
+    const int ncols = min(HALF, min(p.BN, p.cout_pad - nt * p.BN) - cb);      // valid columns of this thread in this tile (<= 0: none)
+    int mt = mu;
+    const int tw = mt % p.tiles_w; mt /= p.tiles_w;
+    const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
+    const int r = q * 32 + lane;
+    const int ho = th * TC_TH + r / TC_TW, wo = tw * TC_TW + r % TC_TW;
+    float amax = 0.f;
+    if (!(ho < p.Ho && wo < p.Wo) || ncols <= 0 || (p.dbg & 16)) return amax;
+    const long long pix = ((long long)b * p.Ho + ho) * p.Wo + wo;
+    const float* acc = tile + r * ld + cb;
+    const float* rp = (p.res && !(p.dbg & 32)) ? p.res + pix * p.res_cs + p.res_co : nullptr;
+    const __half* rph = (p.res_h16_hi && !(p.dbg & 32)) ? reinterpret_cast<const __half*>(p.res_h16_hi) + pix * p.res_cs + p.res_co : nullptr;
+    const __half* rpl = rph ? reinterpret_cast<const __half*>(p.res_h16_lo) + pix * p.res_cs + p.res_co : nullptr;
+    float* op = p.out ? p.out + pix * p.out_cs + p.out_co : nullptr;            // nullptr: planes-only output, no fp32 copy is written
+    float* olo = p.out_lo ? p.out_lo + pix * p.out_cs + p.out_co : nullptr;
+    __half* oh = p.out_h16_hi ? reinterpret_cast<__half*>(p.out_h16_hi) + pix * p.out_cs + p.out_co : nullptr;
+    __half* ol16 = p.out_h16_lo ? reinterpret_cast<__half*>(p.out_h16_lo) + pix * p.out_cs + p.out_co : nullptr;
+    const int nbase = nt * p.BN + cb;
+    const bool v8 = p.v8 != 0;
+    const float osc = p.out_scale;
 #pragma unroll
-                    for (int j = 0; j < 2 * GB; ++j)
+    for (int col = 0; col < HALF; col += 8) {
+        const int n = nbase + col;
+        if (col < ncols && n + 4 <= p.Cout) {
+            const bool full8 = n + 8 <= p.Cout;                  // else the Cout % 8 == 4 tail
+            float rr[8];
 #pragma unroll
-                        for (int k = 0; k < 8; ++k) rr[j][k] = rr_pre[j][k];
-                } else load_res(bt, rr);
+            for (int k = 0; k < 8; ++k) rr[k] = 0.f;
+            if (rp) {
+                if (full8) ld8(rp + n, rr);
+                else { const float4 t4 = ldg4(rp + n); rr[0] = t4.x; rr[1] = t4.y; rr[2] = t4.z; rr[3] = t4.w; }
+            } else if (rph) {
+                if (full8) ld8_planes(rph + n, rpl + n, v8, rr); else ld4_planes(rph + n, rpl + n, rr);
+            }
+            const float4 a0 = *reinterpret_cast<const float4*>(acc + col), a1 = *reinterpret_cast<const float4*>(acc + col + 4);
+            const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+            float a[8];
 #pragma unroll
-                for (int j = 0; j < 2 * GB; ++j) {
-                    if (bt + j / 2 < NG16) {
-                        const int g = bt + j / 2, i0 = (j & 1) * 8;
-                        const int col = bt * 16 + j * 8, n = nbase + col;
-                        if (col < ncols && n + 4 <= p.Cout) {
-                            const bool full8 = n + 8 <= p.Cout;
-                            float a[8];
+            for (int k = 0; k < 8; ++k) a[k] = av[k] * osc + rr[k];
+            if (p.bias) {
+                if (full8) {
+                    float bb[8];
+                    ld8(p.bias + n, bb);
 #pragma unroll
-                            for (int k = 0; k < 8; ++k) a[k] = acc[g][i0 + k] * osc + rr[j][k];
-                            if (p.bias) {
-                                if (full8) {
-                                    float bb[8];
-                                    ld8(p.bias + n, v8, bb);
+                    for (int k = 0; k < 8; ++k) a[k] += bb[k];
+                } else {
+                    const float4 b4 = ldg4(p.bias + n);
+                    a[0] += b4.x; a[1] += b4.y; a[2] += b4.z; a[3] += b4.w;
+                }
+            }
+            if (p.relu) {
 #pragma unroll
-                                    for (int k = 0; k < 8; ++k) a[k] += bb[k];
-                                } else {
-                                    const float4 b4 = ldg4(p.bias + n);
-                                    a[0] += b4.x; a[1] += b4.y; a[2] += b4.z; a[3] += b4.w;
-                                }
-                            }
-                            if (p.relu) {
+                for (int k = 0; k < 8; ++k) a[k] = fmaxf(a[k], 0.f);
+            }
+            if (op) {
+                if (full8) st8(op + n, a);
+                else *reinterpret_cast<float4*>(op + n) = make_float4(a[0], a[1], a[2], a[3]);
+            }
+            if (olo) {      // tf32 companion for the next 3xTF32 conv: the part of the value the MMA does not see
+                float l[8];
 #pragma unroll
-                                for (int k = 0; k < 8; ++k) a[k] = fmaxf(a[k], 0.f);
-                            }
-                            if (PL == 0 || op) {
-                                if (full8) st8(op + n, v8, a);
-                                else *reinterpret_cast<float4*>(op + n) = make_float4(a[0], a[1], a[2], a[3]);
-                            }
-                            if (oh) {      // fp16 hi/lo planes for the next fp16-split conv
-                                uint2 h0, l0, h1, l1;
+                for (int k = 0; k < 8; ++k) l[k] = a[k] - __uint_as_float(__float_as_uint(a[k]) & 0xFFFFE000u);
+                if (full8) st8(olo + n, l);
+                else *reinterpret_cast<float4*>(olo + n) = make_float4(l[0], l[1], l[2], l[3]);
+            }
+            if (oh) {      // fp16 hi/lo planes for the next fp16-split conv
+                uint2 h0, l0, h1, l1;
 #pragma unroll
-                                for (int k = 0; k < 8; ++k) amax = fmaxf(amax, fabsf(a[k]));     // (in the Cout % 8 == 4 tail a[4..7] belong to zero-weight padding columns)
-                                split4(a, h0, l0);
-                                if (full8) {
-                                    split4(a + 4, h1, l1);
-                                    if (v8) {
-                                        *reinterpret_cast<uint4*>(oh + n) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-                                        *reinterpret_cast<uint4*>(ol16 + n) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-                                    } else {
-                                        *reinterpret_cast<uint2*>(oh + n) = h0; *reinterpret_cast<uint2*>(oh + n + 4) = h1;
-                                        *reinterpret_cast<uint2*>(ol16 + n) = l0; *reinterpret_cast<uint2*>(ol16 + n + 4) = l1;
-                                    }
-                                } else {
-                                    *reinterpret_cast<uint2*>(oh + n) = h0;
-                                    *reinterpret_cast<uint2*>(ol16 + n) = l0;
-                                }
-                            }
-                        }
+                for (int k = 0; k < 8; ++k) amax = fmaxf(amax, fabsf(a[k]));     // (in the Cout % 8 == 4 tail a[4..7] belong to zero-weight padding columns)
+                split4(a, h0, l0);
+                if (full8) {
+                    split4(a + 4, h1, l1);
+                    if (v8) {
+                        *reinterpret_cast<uint4*>(oh + n) = make_uint4(h0.x, h0.y, h1.x, h1.y);
+                        *reinterpret_cast<uint4*>(ol16 + n) = make_uint4(l0.x, l0.y, l1.x, l1.y);
+                    } else {
+                        *reinterpret_cast<uint2*>(oh + n) = h0; *reinterpret_cast<uint2*>(oh + n + 4) = h1;
+                        *reinterpret_cast<uint2*>(ol16 + n) = l0; *reinterpret_cast<uint2*>(ol16 + n + 4) = l1;
                     }
+                } else {
+                    *reinterpret_cast<uint2*>(oh + n) = h0;
+                    *reinterpret_cast<uint2*>(ol16 + n) = l0;
                 }
             }
         }
     }
-    note_fp16_range(amax, p.range_flag);
+    return amax;
 }
 
 // VD3D_PDL=1: the persistent tensor-core kernels are launched as programmatic dependents of their predecessor in the stream (pdl_wait() in the kernels)
@@ -296,22 +252,6 @@ inline int make_map_wgt(CUtensorMap* m, const void* base, int Cout, int K, int B
                      rowb == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("conv2d_tc: cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return VD3D_ECUDA; }
     return VD3D_OK;
-}
-
-
-// TMEM accumulator buffers of the persistent kernels: as many BN-column chunk buffers as fit in the 512 columns, at most 4
-// (VD3D_TC_NBUF overrides).  With 2 buffers the MMA warp can run 2 chunks (8 k-blocks) ahead of the epilogue; 4 buffers let it
-// finish most of the next tile of a short-K layer while the epilogue warps are still writing the previous tile to global memory.
-inline void tcp_set_accumulators(TcParams& p) {
-    int nb = 512 / p.BN;
-    if (nb > 4) nb = 4;
-    if (nb < 2) nb = 2;
-    const char* e = getenv("VD3D_TC_NBUF");
-    if (e && atoi(e) >= 2 && atoi(e) <= nb) nb = atoi(e);
-    p.nbuf = nb;
-    uint32_t cols = 32;
-    while (cols < (uint32_t)(nb * p.BN)) cols <<= 1;
-    p.tmem_cols = cols;
 }
 
 

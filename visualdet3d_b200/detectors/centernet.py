@@ -1,10 +1,10 @@
-"""`MonoFlex` / `KM3D` — DLA-34 + DCNv2 up-sampling + CenterNet-style heads on B200
+"""`MonoFlex` / `KM3D` — DLA-34 + DCNv2 up-sampling + CenterNet-style heads on the GPU
 (drop-ins for R/detectors/KM3D.py:16-96, core R/detectors/KM3D_core.py:10-58, heads R/heads/km3d_head.py, monoflex_head.py).
 
 Protocol: ``module([image[1,3,H,W], P2[1,3,4]])`` -> ``(scores[K], bboxes[K,11], cls[K])``; a 3-element list is the training
 protocol (raises).  ``forward_batch(images, P2)`` runs B images at once.
 
-Head execution: the nine `conv3x3(64->256)+ReLU` stems are ONE tcgen05 conv (64 -> 9*256, weights concatenated), the nine 1x1
+Head execution: the nine `conv3x3(64->256)+ReLU` stems are ONE wgmma conv (64 -> 9*256, weights concatenated), the nine 1x1
 output convs write their channel slices of one [B,H/4,W/4,56] tensor that the decode kernels gather from.
 """
 from __future__ import annotations

@@ -3,7 +3,7 @@
 Parameter holders reproduce the reference `state_dict` keys (R/backbones/dla.py:40-326, R/backbones/dla_utils.py:42-155);
 `DLARunner` / `DLAUpRunner` execute them: every Root concat is a set of channel-slice writes, every `up(proj(x)) + prev` add
 is fused into the depthwise transposed-conv kernel, every DeformConv (DCNv2 + BN + ReLU) is one deformable im2col launch +
-one tcgen05 GEMM for the whole batch.
+one wgmma GEMM for the whole batch.
 """
 from __future__ import annotations
 

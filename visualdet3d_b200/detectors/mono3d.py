@@ -1,4 +1,4 @@
-"""`Yolo3D` and `GroundAwareYolo3D` — monocular anchor-based 3-D detectors on B200
+"""`Yolo3D` and `GroundAwareYolo3D` — monocular anchor-based 3-D detectors on the GPU
 (drop-ins for R/detectors/yolomono3d_detector.py:55-138; cores R/detectors/yolomono3d_core.py:9-18).
 
 Protocol (R/pipelines/testers.py:24-25): ``module([image[1,3,H,W], P2[1,3,4]])`` -> ``(scores[K], bboxes[K,11], cls[K])``;

@@ -1,4 +1,4 @@
-"""`Stereo3D` — YOLOStereo3D inference forward on B200 (drop-in for R/detectors/yolostereo3d_detector.py:16-103).
+"""`Stereo3D` — YOLOStereo3D inference forward on the GPU (drop-in for R/detectors/yolostereo3d_detector.py:16-103).
 
 Same construction (`DETECTOR_DICT['Stereo3D'](cfg.detector)`), same checkpoint keys, same list protocol:
 ``module([left[1,3,H,W], right, P2[1,3,4], P3])`` -> ``(scores[K], bboxes[K,11], cls_indexes[K] int64)``.

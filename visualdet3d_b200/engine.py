@@ -30,7 +30,7 @@ class Act:
     `lo` (optional) is the tensor-core companion of `t`, in one of two forms:
       * float32, same shape as `t`:  t - (t & 0xFFFFE000), the part of every value the tf32 MMA does not see ("tc" engine);
       * float16, shape [2, B, H, W, cs]: planes hi = rn16(t) and lo = rn16(t - hi) ("tc16" engine, the default).
-    The tcgen05 conv engine consumes and produces these; other producers leave them stale and the plan calls `split_lo`
+    The wgmma conv engine consumes and produces these; other producers leave them stale and the plan calls `split_lo`
     before a tensor-core consumer."""
     __slots__ = ("t", "co", "C", "lo", "f32", "lo_fresh")
 
@@ -156,7 +156,7 @@ def bn_dict(mod) -> Dict[str, torch.Tensor]:
 
 
 def conv_engine_default() -> str:
-    """'tc16' = tcgen05 fp16-split engine (3 kind::f16 MMAs, default), 'tc' = tcgen05 3xTF32 engine, 'simt' = exact-fp32 SIMT
+    """'tc16' = wgmma fp16-split engine (3 kind::f16 MMAs, default), 'tc' = wgmma 3xTF32 engine, 'simt' = exact-fp32 SIMT
     engine everywhere, 'tc1' = single-pass TF32 (NOT parity-grade; diagnostics only)."""
     import os
     return os.environ.get("VD3D_CONV_ENGINE", "tc16")
@@ -459,7 +459,7 @@ def image_to_row_planes(img: torch.Tensor, planes: torch.Tensor, xoff: int):
 
 class DeformConvLayer:
     """ModulatedDeformConvPack (R/lib/ops/dcn/deform_conv.py:408-466) [+ folded BN] [+ ReLU] on NHWC activations:
-    3x3 offset/mask conv (conv engine) -> deformable im2col with the mask sigmoid fused -> ONE tcgen05 1x1 GEMM over
+    3x3 offset/mask conv (conv engine) -> deformable im2col with the mask sigmoid fused -> ONE wgmma 1x1 GEMM over
     K = KH*KW*C for the whole batch (the reference loops over images and calls cuBLAS per image)."""
 
     def __init__(self, weight, bias, off_weight, off_bias, bn=None, stride=1, pad=1, dil=1, deform_groups=1, relu=False, device="cuda"):
@@ -499,7 +499,7 @@ class DeformConvLayer:
         om = self.off_conv(x, arena.act(name + ".om", (B, Ho, Wo, self.n_off_pad), dev))
         need_f32(x, "deformable gather")
         if self.fused_ok():
-            # gather -> shared-memory operand -> tcgen05 GEMM in ONE kernel: the column tensor never exists (csrc/dcn_fused.cu)
+            # gather -> shared-memory operand -> wgmma GEMM in ONE kernel: the column tensor never exists (csrc/dcn_fused.cu)
             m = self.main
             oh, ol = out.h16_ptrs
             out.f32 = True

@@ -4,9 +4,7 @@
 eagerly (it sizes the arena and builds the anchor tables), the second call captures the same launches into a `torch.cuda.CUDAGraph`, later
 calls replay it.  Every launch of the path goes through the C ABI on the current stream and nothing in it synchronises with the host, so
 the capture sees exactly the kernels of the eager step and the replay writes the same bits (tests/test_zz_next_rows_gpu.py).
-
-Measured on B200 (tools/exp_graph.py, batch 8 unless noted): YOLOStereo3D 384x1280 is not launch-bound (no change), GroundAwareYolo3D
-+3 %, MonoFlex +3 %, Yolo3D at batch 1 (the reference's own test-time batch) +34 %.
+tools/exp_graph.py measures the gain per config (graph replay against eager launches of the same step).
 """
 from __future__ import annotations
 

@@ -10,7 +10,7 @@ where they are re-bound locally (deform_conv_cuda.cpp:198-205,524-535) — are i
                       stride_w, pad_h, pad_w, dilation_h, dilation_w, group, deformable_group, with_bias) -> None
 
 Tensors are the reference's NCHW fp32 CUDA tensors.  Internally: NCHW -> NHWC, deformable im2col (one launch for the whole
-batch, not one per image), ONE tcgen05 1x1 GEMM over K = KH*KW*C with 3xTF32 accuracy, NHWC -> NCHW.
+batch, not one per image), ONE wgmma 1x1 GEMM over K = KH*KW*C with 3xTF32 accuracy, NHWC -> NCHW.
 Errors mirror the reference: CPU tensors -> RuntimeError("... not implemented on CPU"), non-contiguous input/weight and
 shape mismatches -> RuntimeError.  `group > 1` is not supported (no in-scope caller uses it).  The three backward entries
 (deform_conv_ext.cpp:69-104,126-147) are implemented too (SURVEY.md 8(f) rank 4): the reference's unmodified autograd Functions
