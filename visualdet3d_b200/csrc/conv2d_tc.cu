@@ -182,40 +182,38 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         const uint32_t sbo = 8u * rowb, lay = rowb == 128u ? 2u : 4u;
         const int ksteps = (int)rowb / 32;
         const bool tr0 = p.trace && blockIdx.x == 0 && threadIdx.x == 0;
+        int s = 0, ph = 0, g = 0;
+        auto acquire = [&]() {
+            const bool tr = tr0 && g < p.trace_n;
+            if (tr) p.trace[2 * p.trace_n + g] = clock64();                                    // [2] waiting for the stage
+            mbar_wait(&full[s], ph);
+            if (tr) p.trace[3 * p.trace_n + g] = clock64();                                    // [3] about to issue k-block g
+            const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+            const uint32_t aw = sa + (uint32_t)wg * 64u * rowb;
+            const KbOperands o = {make_sdesc(aw, sbo, lay), make_sdesc(aw + a_bytes, sbo, lay),
+                                  make_sdesc(sa + 2 * a_bytes, sbo, lay), make_sdesc(sa + 2 * a_bytes + b_bytes, sbo, lay), s};
+            if (++s == p.stages) { s = 0; ph ^= 1; }
+            return o;
+        };
         auto release = [&](int st) {
             __syncwarp();
-            if (st >= 0 && lane == 0) mbar_arrive(&empty[st]);
+            if (lane == 0) mbar_arrive(&empty[st]);
+        };
+        auto issued = [&]() {
+            if (tr0 && g < p.trace_n) p.trace[4 * p.trace_n + g] = clock64();                  // [4] k-block g issued, previous one retired
+            ++g;
         };
         float tot[BN / 2], c[BN / 2];
         float amax = 0.f;
-        int s = 0, ph = 0, g = 0;
+        // the MMA mode and K steps per k-block are fixed per launch: one K loop per combination, chosen per tile outside the MMA chain
+        auto kloop = [&](auto m, auto k) { wg_tile_kloop<BN, F16, decltype(m)::value, decltype(k)::value>(tot, c, KB, p.chunk, acquire, release, issued); };
         for (int u = u0; u < units; u += ustep) {
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
-            int pend = -1;                                                                     // stage whose MMAs may still be running
-            for (int kb = 0; kb < KB; ++kb, ++g) {
-                const bool first = kb % p.chunk == 0, last = kb % p.chunk == p.chunk - 1 || kb == KB - 1;
-                const bool tr = tr0 && g < p.trace_n;
-                if (tr) p.trace[2 * p.trace_n + g] = clock64();                                // [2] waiting for the stage
-                mbar_wait(&full[s], ph);
-                if (tr) p.trace[3 * p.trace_n + g] = clock64();                                // [3] about to issue k-block g
-                const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-                const uint32_t aw = sa + (uint32_t)wg * 64u * rowb;
-                const uint64_t dA = make_sdesc(aw, sbo, lay), dAlo = make_sdesc(aw + a_bytes, sbo, lay);
-                const uint64_t dB = make_sdesc(sa + 2 * a_bytes, sbo, lay), dBlo = make_sdesc(sa + 2 * a_bytes + b_bytes, sbo, lay);
-                wg_fence();
-                wg_kblock<BN, F16>(c, dA, dAlo, dB, dBlo, ksteps, mode, first);
-                wg_commit();
-                if (last) {
-                    wg_wait<0>();
-                    release(pend); release(s); pend = -1;
-                    wg_promote(tot, c);
-                } else {
-                    wg_wait<1>();                                                              // the previous k-block's MMAs are done
-                    release(pend); pend = s;
-                }
-                if (tr) p.trace[4 * p.trace_n + g] = clock64();                                // [4] k-block g issued, previous one retired
-                if (++s == p.stages) { s = 0; ph ^= 1; }
+            if (!F16 || ksteps == 4) {
+                if (mode == 0) kloop(tc_int<0>(), tc_int<4>()); else if (mode == 2) kloop(tc_int<2>(), tc_int<4>()); else kloop(tc_int<1>(), tc_int<4>());
+            } else {
+                if (mode == 0) kloop(tc_int<0>(), tc_int<2>()); else if (mode == 2) kloop(tc_int<2>(), tc_int<2>()); else kloop(tc_int<1>(), tc_int<2>());
             }
             consumers_sync();                                   // everyone is done reading the previous tile's staged accumulator
             wg_stage<BN>(tot, tile, LD, wg, warp, lane);

@@ -94,32 +94,29 @@ deform_conv_fused_kernel(const __grid_constant__ CUtensorMap mapWhi, const __gri
         // ================= consumer warpgroups =================
         const int wg = warp >> 2;
         const int mode = (q.dbg & 8) ? 1 : 0;
+        int it = 0;
+        auto acquire = [&]() {
+            const int s = it % q.stages, ph = (it / q.stages) & 1;
+            mbar_wait(&fullB[s], ph);
+            mbar_wait(&fullA[s], ph);
+            const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+            const uint32_t aw = sa + (uint32_t)wg * 64u * 128u;
+            ++it;
+            return KbOperands{make_sdesc(aw), make_sdesc(aw + a_bytes), make_sdesc(sa + 2 * a_bytes), make_sdesc(sa + 2 * a_bytes + b_bytes), s};
+        };
         auto release = [&](int st) {
             __syncwarp();
-            if (st >= 0 && lane == 0) mbar_arrive(&empty[st]);
+            if (lane == 0) mbar_arrive(&empty[st]);
         };
+        auto issued = [] {};
         float tot[BN / 2], c[BN / 2];
         float amax = 0.f;
-        int it = 0;
         for (int u = u0; u < units; u += ustep) {
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
-            int pend = -1;
-            for (int kb = 0; kb < KB; ++kb, ++it) {
-                const bool first = kb % p.chunk == 0, last = kb % p.chunk == p.chunk - 1 || kb == KB - 1;
-                const int s = it % q.stages, ph = (it / q.stages) & 1;
-                mbar_wait(&fullB[s], ph);
-                mbar_wait(&fullA[s], ph);
-                const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
-                const uint32_t aw = sa + (uint32_t)wg * 64u * 128u;
-                const uint64_t dA = make_sdesc(aw), dAlo = make_sdesc(aw + a_bytes);
-                const uint64_t dB = make_sdesc(sa + 2 * a_bytes), dBlo = make_sdesc(sa + 2 * a_bytes + b_bytes);
-                wg_fence();
-                wg_kblock<BN, true>(c, dA, dAlo, dB, dBlo, 4, mode, first);      // small terms first (same order as conv2d_tcp_kernel)
-                wg_commit();
-                if (last) { wg_wait<0>(); release(pend); release(s); pend = -1; wg_promote(tot, c); }
-                else { wg_wait<1>(); release(pend); pend = s; }
-            }
+            // small terms first (same MMA order and chunking as conv2d_tcp_kernel)
+            if (mode == 0) wg_tile_kloop<BN, true, 0, 4>(tot, c, KB, p.chunk, acquire, release, issued);
+            else wg_tile_kloop<BN, true, 1, 4>(tot, c, KB, p.chunk, acquire, release, issued);
             consumers_sync();
             wg_stage<BN>(tot, tile, LD, wg, warp, lane);
             consumers_sync();
@@ -314,32 +311,27 @@ deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const 
         // ================= consumer warpgroups =================
         const int wg = warp >> 2;
         const int mode = (q.dbg & 8) ? 1 : 0;
+        int it = 0;
+        auto acquire = [&]() {
+            const int sa = it % DFS_A_STAGES, pa = (it / DFS_A_STAGES) & 1;
+            const int sw = it % WS, pw = (it / WS) & 1;
+            mbar_wait(&fullW[sw], pw);
+            mbar_wait(&fullA[sa], pa);
+            const uint32_t aa = smem_u32(smemA + (size_t)sa * DFS_A_STAGE) + (uint32_t)wg * 64u * 128u, ww = smem_u32(smemW + (size_t)sw * w_stage);
+            return KbOperands{make_sdesc(aa), make_sdesc(aa + a_bytes), make_sdesc(ww), make_sdesc(ww + b_bytes), it++};
+        };
         auto release = [&](int i) {
             __syncwarp();
-            if (i >= 0 && lane == 0) { mbar_arrive(&emptyA[i % DFS_A_STAGES]); mbar_arrive(&emptyW[i % WS]); }
+            if (lane == 0) { mbar_arrive(&emptyA[i % DFS_A_STAGES]); mbar_arrive(&emptyW[i % WS]); }
         };
+        auto issued = [] {};
         float tot[BN / 2], c[BN / 2];
         float amax = 0.f;
-        int it = 0;
         for (int u = u0; u < units; u += ustep) {
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
-            int pend = -1;
-            for (int kb = 0; kb < KB; ++kb, ++it) {
-                const bool first = kb % p.chunk == 0, last = kb % p.chunk == p.chunk - 1 || kb == KB - 1;
-                const int sa = it % DFS_A_STAGES, pa = (it / DFS_A_STAGES) & 1;
-                const int sw = it % WS, pw = (it / WS) & 1;
-                mbar_wait(&fullW[sw], pw);
-                mbar_wait(&fullA[sa], pa);
-                const uint32_t aa = smem_u32(smemA + (size_t)sa * DFS_A_STAGE) + (uint32_t)wg * 64u * 128u, ww = smem_u32(smemW + (size_t)sw * w_stage);
-                const uint64_t dA = make_sdesc(aa), dAlo = make_sdesc(aa + a_bytes);
-                const uint64_t dB = make_sdesc(ww), dBlo = make_sdesc(ww + b_bytes);
-                wg_fence();
-                wg_kblock<BN, true>(c, dA, dAlo, dB, dBlo, 4, mode, first);
-                wg_commit();
-                if (last) { wg_wait<0>(); release(pend); release(it); pend = -1; wg_promote(tot, c); }
-                else { wg_wait<1>(); release(pend); pend = it; }
-            }
+            if (mode == 0) wg_tile_kloop<BN, true, 0, 4>(tot, c, KB, p.chunk, acquire, release, issued);
+            else wg_tile_kloop<BN, true, 1, 4>(tot, c, KB, p.chunk, acquire, release, issued);
             consumers_sync();
             wg_stage<BN>(tot, tile, LD, wg, warp, lane);
             consumers_sync();

@@ -101,9 +101,11 @@ psm_cosine_tc_kernel(const __grid_constant__ CUtensorMap mapLhi, const __grid_co
                     wgmma_f16<PT_N>(acc, dLh + off, dRh + off, 1u);
                 }
                 wg_commit();
-                if (kb == p.kblocks - 1) { wg_wait<0>(); release(pend); release(s); }
-                else { wg_wait<1>(); release(pend); pend = s; }
+                wg_wait<1>();                                  // the previous k-block's MMAs are done
+                release(pend); pend = s;
             }
+            wg_wait<0>();                                      // (outside the loop: a drain under a branch in it would make ptxas drain every k-block)
+            release(pend);
             wg_fence_regs(acc);
             consumers_sync();                                  // the previous tile's band has been read
             {

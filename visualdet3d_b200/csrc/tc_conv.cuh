@@ -4,6 +4,7 @@
 #pragma once
 #include "tc_common.cuh"
 #include <cstdlib>
+#include <type_traits>
 
 namespace vd3d {
 
@@ -97,25 +98,25 @@ __device__ __forceinline__ void unit_tile(const TcParams& p, int u, int mt_units
 }
 __device__ __forceinline__ int unit_nt(const TcParams& p, int u, int mt_units) { int mu, nt; unit_tile(p, u, mt_units, mu, nt); return nt; }
 
-// One k-block of MMAs of a consumer warpgroup: `ksteps` K steps of 32 bytes (16 fp16 / 8 tf32) inside the operand rows, three products per
+// One k-block of MMAs of a consumer warpgroup: KSTEPS K steps of 32 bytes (16 fp16 / 8 tf32) inside the operand rows, three products per
 // step (A_lo W_hi, A_hi W_lo, A_hi W_hi: small terms first, then the main product), one (A W) or two (A W_lo, A W) in the experiment modes.
-// `first`: the first k-block of a promotion chunk (the accumulator restarts from zero).
+// `first`: the first k-block of a promotion chunk (the accumulator restarts from zero).  MODE and KSTEPS are template arguments so that the
+// MMA chain is straight-line code: wgmma instructions under a run-time branch make ptxas serialise them (warpgroup.arrive / wait injection).
 template <int N, bool F16>
 __device__ __forceinline__ void wg_mma(float (&c)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
     if constexpr (F16) wgmma_f16<N>(c, da, db, acc); else wgmma_tf32<N>(c, da, db, acc);
 }
-template <int N, bool F16>
-__device__ __forceinline__ void wg_kblock(float (&c)[N / 2], uint64_t dA, uint64_t dAlo, uint64_t dB, uint64_t dBlo, int ksteps, int mode, bool first) {
+template <int N, bool F16, int MODE, int KSTEPS>
+__device__ __forceinline__ void wg_kblock(float (&c)[N / 2], uint64_t dA, uint64_t dAlo, uint64_t dB, uint64_t dBlo, bool first) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        if (k == ksteps) break;
+    for (int k = 0; k < KSTEPS; ++k) {
         const uint64_t off = (uint64_t)((k * 32) >> 4);
         const uint32_t acc0 = (first && k == 0) ? 0u : 1u;
-        if (mode == 0) {
+        if constexpr (MODE == 0) {
             wg_mma<N, F16>(c, dAlo + off, dB + off, acc0);
             wg_mma<N, F16>(c, dA + off, dBlo + off, 1u);
             wg_mma<N, F16>(c, dA + off, dB + off, 1u);
-        } else if (mode == 2) {
+        } else if constexpr (MODE == 2) {
             wg_mma<N, F16>(c, dA + off, dBlo + off, acc0);
             wg_mma<N, F16>(c, dA + off, dB + off, 1u);
         } else {
@@ -127,12 +128,47 @@ __device__ __forceinline__ void wg_kblock(float (&c)[N / 2], uint64_t dA, uint64
 __host__ __device__ __forceinline__ int tc_mma_mode(const TcParams& p) { return (p.passes == 1 || (p.dbg & 1)) ? 1 : (p.two_pass ? 2 : 0); }
 
 // Chunked promotion: the tensor core adds every product into the fp32 accumulator with truncation, so the K loop is cut into chunks of
-// `chunk` k-blocks, each accumulated from zero in `c` and then added with round-to-nearest into the per-thread sum `tot`.
+// `chunk` k-blocks, each accumulated from zero in a chunk accumulator and then added with round-to-nearest into the per-thread sum `tot`.
 template <int R> __device__ __forceinline__ void wg_promote(float (&tot)[R], float (&c)[R]) {
     wg_fence_regs(c);
 #pragma unroll
     for (int i = 0; i < R; ++i) tot[i] += c[i];
 }
+
+// Shared-memory operands of one k-block, and the ring slot to hand back to the producers once its MMAs have completed.
+struct KbOperands { uint64_t dA, dAlo, dB, dBlo; int slot; };
+
+// One k-block: wait for its operands (acquire), issue its MMAs as one commit group, then wait until at most this group is outstanding and
+// release the slot of the previous k-block.  `pend`: slot of the k-block whose MMAs may still be running (-1: none).
+template <int N, bool F16, int MODE, int KSTEPS, class Acquire, class Release, class Issued>
+__device__ __forceinline__ void wg_kblock_step(float (&c)[N / 2], bool first, int& pend, Acquire& acquire, Release& release, Issued& issued) {
+    const KbOperands o = acquire();
+    wg_fence();
+    wg_kblock<N, F16, MODE, KSTEPS>(c, o.dA, o.dAlo, o.dB, o.dBlo, first);
+    wg_commit();
+    wg_wait<1>();                                       // every earlier k-block's MMAs are done
+    if (pend >= 0) release(pend);
+    pend = o.slot;
+    issued();
+}
+// K loop of one tile of a consumer warpgroup: KB k-blocks in chunks of `chunk`, the sum of the chunks in `tot` (which the caller zeroes).
+// Inside a chunk one k-block of MMAs stays in flight while the next one is issued; the chunk ends with a drain (wait 0) and its promotion.
+// The loop over a chunk's k-blocks is an inner loop and the promotion sits after it, never under a branch inside it: then no instruction
+// other than a wgmma touches the accumulator on a path where a wgmma writing it may still be outstanding, and ptxas keeps the chain
+// asynchronous (with a conditional promotion inside the k-block loop it injects a warpgroup.wait that drains the pipe after every k-block).
+template <int N, bool F16, int MODE, int KSTEPS, class Acquire, class Release, class Issued>
+__device__ __forceinline__ void wg_tile_kloop(float (&tot)[N / 2], float (&c)[N / 2], int KB, int chunk, Acquire& acquire, Release& release, Issued& issued) {
+    for (int kb0 = 0; kb0 < KB; kb0 += chunk) {
+        const int kb1 = min(KB, kb0 + chunk);
+        int pend = -1;
+        wg_kblock_step<N, F16, MODE, KSTEPS>(c, true, pend, acquire, release, issued);
+        for (int kb = kb0 + 1; kb < kb1; ++kb) wg_kblock_step<N, F16, MODE, KSTEPS>(c, false, pend, acquire, release, issued);
+        wg_wait<0>();
+        release(pend);
+        wg_promote(tot, c);
+    }
+}
+template <int V> using tc_int = std::integral_constant<int, V>;
 
 // Epilogue of one tile, run by the 256 consumer threads after the tile's accumulator has been staged in shared memory ([128][ld] fp32, row = tile
 // pixel): thread (warp, lane) owns pixel row 32 (warp % 4) + lane and column half warp / 4.  Scale / bias / residual / ReLU, then the fp32 value
