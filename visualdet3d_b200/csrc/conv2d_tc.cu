@@ -104,9 +104,13 @@ __global__ void pool_border_zero_kernel(float* __restrict__ out, int B, int Hp, 
 }
 
 // ----------------------------------------------------------------------------------------------------------------
-// Persistent kernel.  Shared memory: [stages][A hi | A lo | W hi | W lo] operand ring, the [128][BN + 4] fp32 staged accumulator, barriers.
+// Persistent kernel.  Shared memory: [stages][A hi | A lo | W hi | W lo] operand ring, the [128][BN + 4] fp32 staged accumulator (unless it is
+// staged in the ring: TcParams::tile_in_ring), barriers.
 // ----------------------------------------------------------------------------------------------------------------
 constexpr int TCP_THREADS = TC_CONSUMERS + 32;      // warps 0..7 = consumers, warp 8 = TMA producer
+// row pitch (floats) of the staged accumulator: BN + 4 (conflict-free rows); at BN = 128 unpadded rows with the chunk swizzle of wg_stage,
+// so that the 64 KB tile fits in one 64 KB operand stage
+__host__ __device__ constexpr int tcp_tile_ld(int BN) { return BN == TC_MAX_BN ? BN : BN + 4; }
 
 template <int BN, bool F16>
 __global__ void __launch_bounds__(TCP_THREADS, 1)
@@ -114,14 +118,15 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                   const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    constexpr int LD = BN + 4;
+    constexpr int LD = tcp_tile_ld(BN), swz = BN == TC_MAX_BN ? 7 : 0;
+    const bool in_ring = p.tile_in_ring != 0;
     const uint32_t rowb = (uint32_t)p.rowb;                        // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
     const uint32_t a_bytes = 128u * rowb;                          // one A plane of a stage: 128 pixel rows
     const uint32_t b_bytes = (uint32_t)BN * rowb;
     const uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;      // [A hi | A lo | W hi | W lo]
     const int kbc = (int)rowb / (F16 ? 2 : 4);                     // channels per k-block
-    float* tile = reinterpret_cast<float*>(smem + (size_t)p.stages * stage_bytes);
-    uint64_t* full = reinterpret_cast<uint64_t*>(tile + 128 * LD);  // [stages]  TMA -> consumers
+    float* const tile_sep = reinterpret_cast<float*>(smem + (size_t)p.stages * stage_bytes);      // (tile_in_ring == 0)
+    uint64_t* full = reinterpret_cast<uint64_t*>(in_ring ? smem + (size_t)p.stages * stage_bytes : reinterpret_cast<uint8_t*>(tile_sep + 128 * LD));  // [stages]  TMA -> consumers
     uint64_t* empty = full + p.stages;                              // [stages]  consumers (8 warps) -> TMA
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;      // (warp-uniform for the compiler)
@@ -206,22 +211,32 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         float tot[BN / 2], c[BN / 2];
         float amax = 0.f;
         // the MMA mode and K steps per k-block are fixed per launch: one K loop per combination, chosen per tile outside the MMA chain
-        auto kloop = [&](auto m, auto k) { wg_tile_kloop<BN, F16, decltype(m)::value, decltype(k)::value>(tot, c, KB, p.chunk, acquire, release, issued); };
+        auto kloop = [&](auto m, auto k) {
+            return wg_tile_kloop<BN, F16, decltype(m)::value, decltype(k)::value>(tot, c, KB, p.chunk, acquire, release, issued, in_ring);
+        };
         for (int u = u0; u < units; u += ustep) {
 #pragma unroll
             for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+            int held;                                           // (in_ring) slot of the tile's last k-block: the staging tile
             if (!F16 || ksteps == 4) {
-                if (mode == 0) kloop(tc_int<0>(), tc_int<4>()); else if (mode == 2) kloop(tc_int<2>(), tc_int<4>()); else kloop(tc_int<1>(), tc_int<4>());
+                if (mode == 0) held = kloop(tc_int<0>(), tc_int<4>()); else if (mode == 2) held = kloop(tc_int<2>(), tc_int<4>()); else held = kloop(tc_int<1>(), tc_int<4>());
             } else {
-                if (mode == 0) kloop(tc_int<0>(), tc_int<2>()); else if (mode == 2) kloop(tc_int<2>(), tc_int<2>()); else kloop(tc_int<1>(), tc_int<2>());
+                if (mode == 0) held = kloop(tc_int<0>(), tc_int<2>()); else if (mode == 2) held = kloop(tc_int<2>(), tc_int<2>()); else held = kloop(tc_int<1>(), tc_int<2>());
             }
-            consumers_sync();                                   // everyone is done reading the previous tile's staged accumulator
-            wg_stage<BN>(tot, tile, LD, wg, warp, lane);
+            // everyone is done reading the previous tile's staged accumulator, and (in_ring) both warpgroups' MMAs are done reading the held stage
             consumers_sync();
+            float* tile = in_ring ? reinterpret_cast<float*>(smem + (size_t)held * stage_bytes) : tile_sep;
+            wg_stage<BN>(tot, tile, LD, wg, warp, lane, swz);
+            consumers_sync();
+            bool pooled = false;
             if constexpr (BN == 64 && F16) {
-                if (p.pool_out) { tcp_pool_tile(p, tile, u, mt_units, warp, lane); continue; }
+                if (p.pool_out) { tcp_pool_tile(p, tile, u, mt_units, warp, lane); pooled = true; }
             }
-            amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane));
+            if (!pooled) amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane, swz));
+            if (in_ring) {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic accesses to the stage before the next TMA write into it
+                release(held);
+            }
         }
         note_fp16_range(amax, p.range_flag);
     }
@@ -343,17 +358,29 @@ static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAl
     if (p.rowb == 0) p.rowb = 128;
     VD3D_REQUIRE(BN % 16 == 0 && BN >= 16 && BN <= TC_MAX_BN, "conv2d_tc: BN must be a multiple of 16 in [16, %d]", TC_MAX_BN);
     const size_t stage_bytes = 2 * (size_t)128 * p.rowb + 2 * (size_t)BN * p.rowb;
-    const size_t tile_bytes = (size_t)128 * (BN + 4) * sizeof(float);
     VD3D_REQUIRE(!p.pool_out || (BN == 64 && p.f16 && p.relu && !p.res && !p.res_h16_hi), "conv2d_tc: the fused max-pool needs a 64-column fp16 tile with ReLU and no residual");
-    int stages = (int)((227 * 1024 - 1024 - 256 - tile_bytes) / stage_bytes);
+    // Staging tile: a separate tile after the ring, or the stage of the tile's last k-block (which then stays held through the epilogue) when
+    // the accumulator fits there and that buys a stage; the producer still gets as many stages for the next tile while the epilogue runs as
+    // with a separate tile.  VD3D_TC_TILE_IN_RING=0 always uses a separate tile.
+    const size_t avail = 227 * 1024 - 1024 - 256;
+    const size_t tile_bytes = (size_t)128 * tcp_tile_ld(BN) * sizeof(float);
+    int stages = (int)((avail - tile_bytes) / stage_bytes);
+    {
+        const char* e = getenv("VD3D_TC_TILE_IN_RING");
+        const int stages_in = (int)(avail / stage_bytes);
+        p.tile_in_ring = !(e && atoi(e) == 0) && tile_bytes <= stage_bytes && stages < 8 && stages_in > stages;
+        if (p.tile_in_ring) stages = stages_in;
+    }
     if (stages > 8) stages = 8;
     VD3D_REQUIRE(stages >= 2, "conv2d_tc: tile too large for shared memory");
     p.stages = stages;
-    const size_t smem = stages * stage_bytes + tile_bytes + ((2 * stages * sizeof(uint64_t) + 15) / 16 * 16) + 1024;
+    const size_t smem = stages * stage_bytes + (p.tile_in_ring ? 0 : tile_bytes) + ((2 * stages * sizeof(uint64_t) + 15) / 16 * 16) + 1024;
     const int units = p.m_tiles * p.n_tiles;
+    int grid = units < kNumSMs ? units : kNumSMs;
+    { const char* e = getenv("VD3D_TC_GRID"); const int cap = e ? atoi(e) : 0; if (cap > 0 && cap < grid) grid = cap; }     // diagnostics
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(units < kNumSMs ? units : kNumSMs));
+    cfg.gridDim = dim3((unsigned)grid);
     cfg.blockDim = dim3(TCP_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = (cudaStream_t)stream;

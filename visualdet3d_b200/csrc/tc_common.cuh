@@ -102,13 +102,18 @@ template <int R> __device__ __forceinline__ void wg_fence_regs(float (&d)[R]) {
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 // Writes the fp32 fragment of a 64 x N accumulator (warpgroup `wg` = rows 64 wg .. 64 wg + 63 of the tile) into a row-major [128][ld] shared-memory
-// tile: the per-pixel epilogues read their rows back from there.
-template <int N> __device__ __forceinline__ void wg_stage(const float (&d)[N / 2], float* tile, int ld, int wg, int warp, int lane) {
+// tile: the per-pixel epilogues read their rows back from there.  `swz` = 7: unpadded rows (ld = N, a multiple of 32) whose 16-byte chunk j of
+// row r sits at chunk j ^ (r & 7), which keeps these stores and the epilogue's row reads free of bank conflicts; 0: plain (padded) rows.
+template <int N> __device__ __forceinline__ void wg_stage(const float (&d)[N / 2], float* tile, int ld, int wg, int warp, int lane, int swz = 0) {
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    int sw = r0 & swz;                                   // (rows r0 and r0 + 8 share it)
+    if (swz) asm volatile("" : "+r"(sw));                // opaque per call: the N / 4 swizzled offsets are not hoisted out of the caller's tile loop
+                                                         // and kept live (spilled) through its MMAs
 #pragma unroll
     for (int j = 0; j < N / 8; ++j) {
-        *reinterpret_cast<float2*>(tile + r0 * ld + 8 * j + c0) = make_float2(d[4 * j], d[4 * j + 1]);
-        *reinterpret_cast<float2*>(tile + (r0 + 8) * ld + 8 * j + c0) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+        const int col = (((2 * j + (c0 >> 2)) ^ sw) << 2) + (c0 & 3);
+        *reinterpret_cast<float2*>(tile + r0 * ld + col) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(tile + (r0 + 8) * ld + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
     }
 }
 // named barrier of the 256 consumer threads (warps 0..7) of the tensor-core kernels

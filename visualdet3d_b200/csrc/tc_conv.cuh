@@ -32,6 +32,9 @@ struct TcParams {
     int two_pass;            // error-budget experiments (vd3d_conv2d_tc16 passes = 2): drop the A_lo * W_hi product (activations then carry 11 significant bits)
     int mblock;              // persistent kernels: scheduling units (tiles) per M block of the L2-aware tile order (0: one block)
     int rowb;                // bytes per operand row in shared memory = K bytes per k-block: 128 (SWIZZLE_128B) or 64 (32 fp16, SWIZZLE_64B)
+    // conv2d_tcp_kernel: where the accumulator is staged for the epilogue.  1: in the operand stage of the tile's last k-block, held until the
+    // epilogue is done (no separate staging tile: one more stage fits); 0: a separate tile after the ring
+    int tile_in_ring;
     int cout_pad;            // Cout rounded up to 16 (ragged last N tile = cout_pad - (n_tiles - 1) * BN columns)
     int v8;                  // output / residual / bias slices are 32-byte aligned (fp16 plane slices then take 16-byte accesses)
     long long* trace; int trace_n;   // VD3D diagnostics (vd3d_tc_set_trace): per-k-block clock64 stamps of CTA 0, [5][trace_n]
@@ -156,26 +159,31 @@ __device__ __forceinline__ void wg_kblock_step(float (&c)[N / 2], bool first, in
 // The loop over a chunk's k-blocks is an inner loop and the promotion sits after it, never under a branch inside it: then no instruction
 // other than a wgmma touches the accumulator on a path where a wgmma writing it may still be outstanding, and ptxas keeps the chain
 // asynchronous (with a conditional promotion inside the k-block loop it injects a warpgroup.wait that drains the pipe after every k-block).
+// `keep_last`: the slot of the tile's last k-block is not released but returned (the caller stages the accumulator there and releases it after
+// the epilogue); otherwise every slot is released and the result is -1.
 template <int N, bool F16, int MODE, int KSTEPS, class Acquire, class Release, class Issued>
-__device__ __forceinline__ void wg_tile_kloop(float (&tot)[N / 2], float (&c)[N / 2], int KB, int chunk, Acquire& acquire, Release& release, Issued& issued) {
+__device__ __forceinline__ int wg_tile_kloop(float (&tot)[N / 2], float (&c)[N / 2], int KB, int chunk, Acquire& acquire, Release& release, Issued& issued,
+                                             bool keep_last = false) {
+    int pend = -1;
     for (int kb0 = 0; kb0 < KB; kb0 += chunk) {
         const int kb1 = min(KB, kb0 + chunk);
-        int pend = -1;
+        pend = -1;
         wg_kblock_step<N, F16, MODE, KSTEPS>(c, true, pend, acquire, release, issued);
         for (int kb = kb0 + 1; kb < kb1; ++kb) wg_kblock_step<N, F16, MODE, KSTEPS>(c, false, pend, acquire, release, issued);
         wg_wait<0>();
-        release(pend);
+        if (!keep_last || kb1 < KB) { release(pend); pend = -1; }
         wg_promote(tot, c);
     }
+    return pend;
 }
 template <int V> using tc_int = std::integral_constant<int, V>;
 
 // Epilogue of one tile, run by the 256 consumer threads after the tile's accumulator has been staged in shared memory ([128][ld] fp32, row = tile
 // pixel): thread (warp, lane) owns pixel row 32 (warp % 4) + lane and column half warp / 4.  Scale / bias / residual / ReLU, then the fp32 value
 // (and its tf32 `lo` companion when asked) and / or the fp16 (hi, lo) planes the next tensor-core conv reads.  Returns the largest magnitude
-// written to fp16 planes (fp16-range guard).
+// written to fp16 planes (fp16-range guard).  `swz`: the staged tile's chunk swizzle (wg_stage).
 template <int N>
-__device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int warp, int lane) {
+__device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int warp, int lane, int swz = 0) {
     constexpr int HALF = ((N + 31) / 32) * 16;                     // accumulator columns per thread
     const int q = warp & 3, half = warp >> 2;
     const int cb = half * HALF;
@@ -190,7 +198,9 @@ __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* 
     float amax = 0.f;
     if (!(ho < p.Ho && wo < p.Wo) || ncols <= 0 || (p.dbg & 16)) return amax;
     const long long pix = ((long long)b * p.Ho + ho) * p.Wo + wo;
-    const float* acc = tile + r * ld + cb;
+    const float* acc = tile + r * ld;
+    int sw = r & swz;
+    if (swz) asm volatile("" : "+r"(sw));                           // (as in wg_stage)
     const float* rp = (p.res && !(p.dbg & 32)) ? p.res + pix * p.res_cs + p.res_co : nullptr;
     const __half* rph = (p.res_h16_hi && !(p.dbg & 32)) ? reinterpret_cast<const __half*>(p.res_h16_hi) + pix * p.res_cs + p.res_co : nullptr;
     const __half* rpl = rph ? reinterpret_cast<const __half*>(p.res_h16_lo) + pix * p.res_cs + p.res_co : nullptr;
@@ -215,7 +225,8 @@ __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* 
             } else if (rph) {
                 if (full8) ld8_planes(rph + n, rpl + n, v8, rr); else ld4_planes(rph + n, rpl + n, rr);
             }
-            const float4 a0 = *reinterpret_cast<const float4*>(acc + col), a1 = *reinterpret_cast<const float4*>(acc + col + 4);
+            const int j = (cb + col) >> 2;                       // 16-byte chunk of the staged row
+            const float4 a0 = *reinterpret_cast<const float4*>(acc + ((j ^ sw) << 2)), a1 = *reinterpret_cast<const float4*>(acc + (((j + 1) ^ sw) << 2));
             const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
             float a[8];
 #pragma unroll
