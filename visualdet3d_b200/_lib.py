@@ -94,6 +94,9 @@ _SIGS = {
     "vd3d_anchor_mask": (I, [P, P, P, I, I, I, F, F, F, P, P]),
     "vd3d_decode_nms_workspace": (c_longlong, [I, I]),
     "vd3d_decode_nms": (I, [P, P, P, P, P, I, I, I, I, F, c_double, F, F, I, P, P, P, P, P, P, P, P]),
+    "vd3d_kitti_rotate_iou": (I, [P, I, P, I, I, P, P]),
+    "vd3d_kitti_eval_workspace_bytes": (c_longlong, [I, c_longlong, c_longlong, c_longlong, I]),
+    "vd3d_kitti_eval": (I, [P, P, P, I, c_longlong, c_longlong, c_longlong, c_longlong, P, I, P, I, P, P, P, P, P, P, c_longlong, P]),
 }
 
 

@@ -76,3 +76,15 @@ def install_into_reference(force: bool = True):
     for fn in PIPELINE_DICT.module_dict.values():
         ref.PIPELINE_DICT._register_module(fn, force=force)
     return ref
+
+
+def install_evaluator_into_reference():
+    """Make the REFERENCE's KITTI evaluation run on the native evaluator (`kitti_eval.evaluate`, same signature and strings):
+    rebinds `visualDet3D.evaluator.kitti.evaluate.evaluate` and the name `evaluators.py` imported from it at module level, so the
+    unmodified `evaluate_kitti_obj` (scripts/eval.py, and scripts/train.py after each evaluation epoch) uses it."""
+    from visualDet3D.evaluator.kitti import evaluate as ref_evaluate      # ImportError if the reference is not on sys.path
+    from visualDet3D.networks.pipelines import evaluators as ref_evaluators
+    from .kitti_eval import evaluate
+    ref_evaluate.evaluate = evaluate
+    ref_evaluators.evaluate = evaluate
+    return evaluate
