@@ -10,10 +10,11 @@
 // * No im2col: for k-block (tap, channel chunk) the A operand is ONE 4-D TMA box [chunk][16 w][8 h][1 b] of the input shifted by the tap
 //   offset; conv zero padding is TMA out-of-bounds fill.  Swizzled K-major operands (128-byte rows; 64-byte rows for the 32-element stem window).
 // * Persistent: one CTA per SM strides over the 128-pixel x BN-channel output tiles (unit_tile: M fastest inside L2-sized M blocks).
-//   Warp 8 = TMA producer (one lane) feeding a multi-stage mbarrier ring; warps 0..7 = two consumer warpgroups.  Warpgroup w issues the
-//   wgmma of tile rows 64 w .. 64 w + 63 as soon as a stage has landed, keeps one k-block in flight, frees a stage when its MMAs are done,
-//   promotes every chunk (wg_promote) and at the end of the tile stages its accumulator in shared memory for the epilogue (tcp_store_tile),
-//   while the producer is already filling the ring with the next tile's operands.
+//   Warp 8 = TMA producer (one lane) feeding a multi-stage mbarrier ring; warps 0..7 = two consumer warpgroups; warps 9..11 = epilogue
+//   (tiles wider than 64 columns; narrower tiles run it on the consumers, tcp_store_tile / tcp_pool_tile).
+//   Warpgroup w issues the wgmma of tile rows 64 w .. 64 w + 63 as soon as a stage has landed, keeps one k-block in flight, frees a stage when
+//   its MMAs are done, promotes every chunk (wg_promote) and at the end of the tile stages its accumulator in shared memory and hands it to the
+//   epilogue warps (tcp_epi_tile), then goes straight on with the next tile's MMAs while the epilogue runs.
 // * K order: channel chunk outermost, taps inside, and the same chunking for every tile width: a layer gives bit-identical results
 //   whichever tile width the host picks.
 #include "tc_conv.cuh"
@@ -107,10 +108,59 @@ __global__ void pool_border_zero_kernel(float* __restrict__ out, int B, int Hp, 
 // Persistent kernel.  Shared memory: [stages][A hi | A lo | W hi | W lo] operand ring, the [128][BN + 4] fp32 staged accumulator (unless it is
 // staged in the ring: TcParams::tile_in_ring), barriers.
 // ----------------------------------------------------------------------------------------------------------------
-constexpr int TCP_THREADS = TC_CONSUMERS + 32;      // warps 0..7 = consumers, warp 8 = TMA producer
+// Warps 0..7 = consumers, warp 8 = TMA producer, warps 9..11 = epilogue.  ptxas budgets registers per whole warpgroup (65536 / 384 = 168 per
+// thread here; a fourth warpgroup would cap every thread at 128, below what the 128-column consumers need), so the epilogue gets the three
+// warps of the producer's warpgroup.
+constexpr int TCP_EPI = 96;
+constexpr int TCP_THREADS = TC_CONSUMERS + 32 + TCP_EPI;
 // row pitch (floats) of the staged accumulator: BN + 4 (conflict-free rows); at BN = 128 unpadded rows with the chunk swizzle of wg_stage,
 // so that the 64 KB tile fits in one 64 KB operand stage
 __host__ __device__ constexpr int tcp_tile_ld(int BN) { return BN == TC_MAX_BN ? BN : BN + 4; }
+// named barrier of the epilogue warps
+__device__ __forceinline__ void epilogue_sync() { asm volatile("bar.sync 3, %0;" ::"n"(TCP_EPI) : "memory"); }
+
+// Epilogue of one staged tile by the epilogue warps (thread et of TCP_EPI).  Item = (pixel row r, 8-column group g), items numbered row-major,
+// thread et takes items et, et + TCP_EPI, ...: consecutive lanes cover consecutive column groups of one pixel, so a warp's residual loads and
+// output stores are whole runs of a pixel's channels (at BN = 128, 256 contiguous bytes per fp16 plane).  The residual loads of U items are
+// issued before the first of them is computed.  Per element the arithmetic is that of tcp_store_tile.
+template <int BN>
+__device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int et, int swz) {
+    constexpr int CG = BN / 8;                                   // column groups per pixel
+    constexpr int ITEMS = 128 * CG, U = 8;
+    int mu, nt;
+    unit_tile(p, u, mt_units, mu, nt);
+    const int ncols = min(BN, p.cout_pad - nt * BN);              // valid columns of this tile
+    int mt = mu;
+    const int tw = mt % p.tiles_w; mt /= p.tiles_w;
+    const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
+    float amax = 0.f;
+    if (p.dbg & 16) return amax;
+    for (int i0 = et; i0 < ITEMS; i0 += U * TCP_EPI) {
+        float rr[U][8];
+        long long pix[U];
+        int rg[U];                                               // item = r * CG + g, or -1: nothing to write
+#pragma unroll
+        for (int i = 0; i < U; ++i) {
+            const int idx = i0 + i * TCP_EPI;
+            const int r = idx / CG, g = idx - r * CG;
+            const int ho = th * TC_TH + r / TC_TW, wo = tw * TC_TW + r % TC_TW;
+            const int n = nt * BN + 8 * g;
+            rg[i] = (idx < ITEMS && ho < p.Ho && wo < p.Wo && 8 * g < ncols && n + 4 <= p.Cout) ? idx : -1;
+            pix[i] = ((long long)b * p.Ho + ho) * p.Wo + wo;
+            if (rg[i] >= 0) tcp_epi_res(p, pix[i], n, rr[i]);
+        }
+#pragma unroll
+        for (int i = 0; i < U; ++i) {
+            if (rg[i] < 0) continue;
+            const int r = rg[i] / CG, g = rg[i] - r * CG;
+            const float* acc = tile + r * ld;
+            const int sw = r & swz, j = 2 * g;                   // 16-byte chunks j, j + 1 of the staged row (wg_stage's swizzle)
+            const float4 a0 = *reinterpret_cast<const float4*>(acc + ((j ^ sw) << 2)), a1 = *reinterpret_cast<const float4*>(acc + (((j + 1) ^ sw) << 2));
+            amax = fmaxf(amax, tcp_epi_out(p, pix[i], nt * BN + 8 * g, a0, a1, rr[i]));
+        }
+    }
+    return amax;
+}
 
 template <int BN, bool F16>
 __global__ void __launch_bounds__(TCP_THREADS, 1)
@@ -127,7 +177,10 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     const int kbc = (int)rowb / (F16 ? 2 : 4);                     // channels per k-block
     float* const tile_sep = reinterpret_cast<float*>(smem + (size_t)p.stages * stage_bytes);      // (tile_in_ring == 0)
     uint64_t* full = reinterpret_cast<uint64_t*>(in_ring ? smem + (size_t)p.stages * stage_bytes : reinterpret_cast<uint8_t*>(tile_sep + 128 * LD));  // [stages]  TMA -> consumers
-    uint64_t* empty = full + p.stages;                              // [stages]  consumers (8 warps) -> TMA
+    uint64_t* empty = full + p.stages;                              // [stages]  consumers (8 warps; the held stage: epilogue warps) -> TMA
+    uint64_t* acc_full = empty + p.stages;                          // consumers (256 threads) -> epilogue: a tile is staged
+    uint64_t* acc_empty = acc_full + 1;                             // epilogue -> consumers: the staged tile has been read
+    int* mailbox = reinterpret_cast<int*>(acc_empty + 1);           // (in_ring) ring slot of the staged tile
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;      // (warp-uniform for the compiler)
     const int cchunks = p.cin_pad / kbc;
@@ -136,16 +189,47 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     const int units = mt_units * p.n_tiles;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
     const int mode = tc_mma_mode(p);
+    // Tiles wider than 64 columns hand their epilogue to the epilogue warps.  Narrower tiles keep it on the consumers (the stem's fused
+    // max-pool among them): their K loop is short (64 columns: 9 k-blocks of ~890 clocks for a 64-channel 3x3 conv, H100) and the three
+    // epilogue warps take longer per tile (~11 k clocks) than the 256 consumer threads, so overlapping made those layers slower.
+    constexpr bool epi_warps = BN > 64;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], TC_CONSUMERS / 32); }
+        mbar_init(acc_full, TC_CONSUMERS);
+        mbar_init(acc_empty, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     pdl_launch_dependents();
     pdl_wait();                            // (PDL launches only) the producer of the activations / residual has completed
 
-    if (warp == TC_CONSUMERS / 32) {
+    if (warp > TC_CONSUMERS / 32) {
+        // ================= epilogue warps: tile i of this CTA is handed over through acc_full / acc_empty phase i =================
+        if (!epi_warps) return;
+        const int et = (int)threadIdx.x - (TC_CONSUMERS + 32);
+        const bool tr0 = p.trace && blockIdx.x == 0 && et == 0;
+        float amax = 0.f;
+        int i = 0;
+        for (int u = u0; u < units; u += ustep, ++i) {
+            const bool tr = tr0 && i < p.trace_n;
+            mbar_wait(acc_full, i & 1);
+            if (tr) p.trace[7 * p.trace_n + i] = clock64();                                     // [7] epilogue starts
+            const int held = *mailbox;
+            const float* tile = in_ring ? reinterpret_cast<const float*>(smem + (size_t)held * stage_bytes) : tile_sep;
+            amax = fmaxf(amax, tcp_epi_tile<BN>(p, tile, LD, u, mt_units, et, swz));
+            // every epilogue thread is done reading the staged tile (and the mailbox): give the stage back to the producer (empty[] counts the
+            // 8 consumer warps' arrivals) and the staging buffer to the consumers
+            if (in_ring) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic accesses to the stage before the next TMA write into it
+            epilogue_sync();
+            if (et == 0) {
+                if (in_ring) mbar_arrive(&empty[held], TC_CONSUMERS / 32);
+                mbar_arrive(acc_empty);
+                if (tr) p.trace[8 * p.trace_n + i] = clock64();                                 // [8] stage released, epilogue done
+            }
+        }
+        note_fp16_range(amax, p.range_flag);
+    } else if (warp == TC_CONSUMERS / 32) {
         if (lane == 0) {
             // ================= TMA producer =================
             const bool lo_too = mode != 1 && !(p.dbg & 2);
@@ -209,33 +293,47 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
             ++g;
         };
         float tot[BN / 2], c[BN / 2];
-        float amax = 0.f;
+        float amax = 0.f;                                       // (epilogue on the consumers)
         // the MMA mode and K steps per k-block are fixed per launch: one K loop per combination, chosen per tile outside the MMA chain
         auto kloop = [&](auto m, auto k) {
             return wg_tile_kloop<BN, F16, decltype(m)::value, decltype(k)::value>(tot, c, KB, p.chunk, acquire, release, issued, in_ring);
         };
-        for (int u = u0; u < units; u += ustep) {
+        int i = 0;
+        for (int u = u0; u < units; u += ustep, ++i) {
 #pragma unroll
-            for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+            for (int k = 0; k < BN / 2; ++k) tot[k] = 0.f;
             int held;                                           // (in_ring) slot of the tile's last k-block: the staging tile
             if (!F16 || ksteps == 4) {
                 if (mode == 0) held = kloop(tc_int<0>(), tc_int<4>()); else if (mode == 2) held = kloop(tc_int<2>(), tc_int<4>()); else held = kloop(tc_int<1>(), tc_int<4>());
             } else {
                 if (mode == 0) held = kloop(tc_int<0>(), tc_int<2>()); else if (mode == 2) held = kloop(tc_int<2>(), tc_int<2>()); else held = kloop(tc_int<1>(), tc_int<2>());
             }
-            // everyone is done reading the previous tile's staged accumulator, and (in_ring) both warpgroups' MMAs are done reading the held stage
-            consumers_sync();
+            const bool tr = tr0 && i < p.trace_n;
+            if (tr) p.trace[5 * p.trace_n + i] = clock64();                                     // [5] the tile's last MMAs are done
             float* tile = in_ring ? reinterpret_cast<float*>(smem + (size_t)held * stage_bytes) : tile_sep;
-            wg_stage<BN>(tot, tile, LD, wg, warp, lane, swz);
-            consumers_sync();
-            bool pooled = false;
-            if constexpr (BN == 64 && F16) {
-                if (p.pool_out) { tcp_pool_tile(p, tile, u, mt_units, warp, lane); pooled = true; }
-            }
-            if (!pooled) amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane, swz));
-            if (in_ring) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic accesses to the stage before the next TMA write into it
-                release(held);
+            if constexpr (!epi_warps) {
+                // everyone is done reading the previous tile's staged accumulator, and (in_ring) both warpgroups' MMAs are done reading the held stage
+                consumers_sync();
+                wg_stage<BN>(tot, tile, LD, wg, warp, lane, swz);
+                consumers_sync();
+                bool pooled = false;
+                if constexpr (BN == 64 && F16) {
+                    if (p.pool_out) { tcp_pool_tile(p, tile, u, mt_units, warp, lane); pooled = true; }
+                }
+                if (!pooled) amax = fmaxf(amax, tcp_store_tile<BN>(p, tile, LD, u, mt_units, warp, lane, swz));
+                if (in_ring) {
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic accesses to the stage before the next TMA write into it
+                    release(held);
+                }
+            } else {
+                // hand the tile to the epilogue warps and go on with the next one: the epilogue is done with the previous staged tile and the
+                // mailbox (phase i - 1 of acc_empty; a fresh barrier passes parity 1), and (in_ring) both warpgroups' MMAs are done reading the held stage
+                mbar_wait(acc_empty, (i & 1) ^ 1);
+                consumers_sync();
+                wg_stage<BN>(tot, tile, LD, wg, warp, lane, swz);
+                if (threadIdx.x == 0) *mailbox = held;
+                mbar_arrive(acc_full);
+                if (tr) p.trace[6 * p.trace_n + i] = clock64();                                 // [6] staged and handed over
             }
         }
         note_fp16_range(amax, p.range_flag);
@@ -333,7 +431,7 @@ extern "C" int vd3d_tc_pick_bn(int Cout) {
     return Cout <= 128 ? (Cout + 15) / 16 * 16 : 128;
 }
 
-// diagnostics: clock64 stamps of the TMA / MMA pipeline of CTA 0 ([5][n] int64 device buffer; NULL disables)
+// diagnostics: clock64 stamps of the TMA / MMA pipeline and the tile hand-off of CTA 0 ([9][n] int64 device buffer; NULL disables)
 static long long* g_trace = nullptr;
 static int g_trace_n = 0;
 extern "C" void vd3d_tc_set_trace(void* dev_i64, int n) { g_trace = (long long*)dev_i64; g_trace_n = n; }
@@ -374,7 +472,8 @@ static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAl
     if (stages > 8) stages = 8;
     VD3D_REQUIRE(stages >= 2, "conv2d_tc: tile too large for shared memory");
     p.stages = stages;
-    const size_t smem = stages * stage_bytes + (p.tile_in_ring ? 0 : tile_bytes) + ((2 * stages * sizeof(uint64_t) + 15) / 16 * 16) + 1024;
+    // barrier area: full[stages], empty[stages], acc_full, acc_empty, the mailbox
+    const size_t smem = stages * stage_bytes + (p.tile_in_ring ? 0 : tile_bytes) + (((2 * stages + 3) * sizeof(uint64_t) + 15) / 16 * 16) + 1024;
     const int units = p.m_tiles * p.n_tiles;
     int grid = units < kNumSMs ? units : kNumSMs;
     { const char* e = getenv("VD3D_TC_GRID"); const int cap = e ? atoi(e) : 0; if (cap > 0 && cap < grid) grid = cap; }     // diagnostics

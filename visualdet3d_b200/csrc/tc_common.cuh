@@ -66,6 +66,10 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// `count` arrivals at once
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
 // Programmatic dependent launch (VD3D_PDL=1): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may become resident while its
 // predecessor is still draining; everything it does before pdl_wait() (barrier init) overlaps the predecessor's tail, and
 // pdl_wait() returns when the predecessor has completed and its writes are visible.  Both are no-ops in an ordinary launch.

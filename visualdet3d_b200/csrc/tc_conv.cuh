@@ -37,7 +37,7 @@ struct TcParams {
     int tile_in_ring;
     int cout_pad;            // Cout rounded up to 16 (ragged last N tile = cout_pad - (n_tiles - 1) * BN columns)
     int v8;                  // output / residual / bias slices are 32-byte aligned (fp16 plane slices then take 16-byte accesses)
-    long long* trace; int trace_n;   // VD3D diagnostics (vd3d_tc_set_trace): per-k-block clock64 stamps of CTA 0, [5][trace_n]
+    long long* trace; int trace_n;   // VD3D diagnostics (vd3d_tc_set_trace): clock64 stamps of CTA 0, [9][trace_n]: rows 0..4 per k-block, 5..8 per tile
     int dbg;                 // timing experiments only (VD3D_TC_DEBUG; results are wrong): bit 0 = one MMA per k-step, bit 1 = skip the lo-plane loads, bit 4 = no epilogue output, bit 5 = no residual loads
     int out_cs, out_co, res_cs, res_co, relu;
     const float* bias; const float* res; float* out; float* out_lo;
@@ -178,10 +178,90 @@ __device__ __forceinline__ int wg_tile_kloop(float (&tot)[N / 2], float (&c)[N /
 }
 template <int V> using tc_int = std::integral_constant<int, V>;
 
-// Epilogue of one tile, run by the 256 consumer threads after the tile's accumulator has been staged in shared memory ([128][ld] fp32, row = tile
-// pixel): thread (warp, lane) owns pixel row 32 (warp % 4) + lane and column half warp / 4.  Scale / bias / residual / ReLU, then the fp32 value
-// (and its tf32 `lo` companion when asked) and / or the fp16 (hi, lo) planes the next tensor-core conv reads.  Returns the largest magnitude
-// written to fp16 planes (fp16-range guard).  `swz`: the staged tile's chunk swizzle (wg_stage).
+// Epilogue arithmetic of the persistent kernels, per 8 output channels n .. n + 7 of one output pixel `pix` (n + 4 <= Cout; when n + 8 > Cout,
+// the Cout % 8 == 4 tail, only the first four are read and written).  Split in two so that an epilogue can have the residual loads of
+// several groups in flight before it computes the first.
+// (1) the residual (zeros without one)
+__device__ __forceinline__ void tcp_epi_res(const TcParams& p, long long pix, int n, float (&rr)[8]) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) rr[k] = 0.f;
+    if (p.dbg & 32) return;
+    const bool full8 = n + 8 <= p.Cout;
+    if (p.res) {
+        const float* rp = p.res + pix * p.res_cs + p.res_co + n;
+        if (full8) ld8(rp, rr);
+        else { const float4 t4 = ldg4(rp); rr[0] = t4.x; rr[1] = t4.y; rr[2] = t4.z; rr[3] = t4.w; }
+    } else if (p.res_h16_hi) {
+        const __half* rph = reinterpret_cast<const __half*>(p.res_h16_hi) + pix * p.res_cs + p.res_co + n;
+        const __half* rpl = reinterpret_cast<const __half*>(p.res_h16_lo) + pix * p.res_cs + p.res_co + n;
+        if (full8) ld8_planes(rph, rpl, p.v8 != 0, rr); else ld4_planes(rph, rpl, rr);
+    }
+}
+// (2) scale / residual / bias / ReLU of the staged accumulator values (a0, a1), then the fp32 value (and its tf32 `lo` companion when asked)
+// and / or the fp16 (hi, lo) planes the next tensor-core conv reads.  Returns the largest magnitude written to fp16 planes (fp16-range guard).
+__device__ __forceinline__ float tcp_epi_out(const TcParams& p, long long pix, int n, const float4& a0, const float4& a1, const float (&rr)[8]) {
+    const bool full8 = n + 8 <= p.Cout;
+    const float osc = p.out_scale;
+    float amax = 0.f;
+    const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+    float a[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) a[k] = av[k] * osc + rr[k];
+    if (p.bias) {
+        if (full8) {
+            float bb[8];
+            ld8(p.bias + n, bb);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) a[k] += bb[k];
+        } else {
+            const float4 b4 = ldg4(p.bias + n);
+            a[0] += b4.x; a[1] += b4.y; a[2] += b4.z; a[3] += b4.w;
+        }
+    }
+    if (p.relu) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) a[k] = fmaxf(a[k], 0.f);
+    }
+    if (p.out) {      // (nullptr: planes-only output, no fp32 copy is written)
+        float* op = p.out + pix * p.out_cs + p.out_co + n;
+        if (full8) st8(op, a);
+        else *reinterpret_cast<float4*>(op) = make_float4(a[0], a[1], a[2], a[3]);
+    }
+    if (p.out_lo) {   // tf32 companion for the next 3xTF32 conv: the part of the value the MMA does not see
+        float* olo = p.out_lo + pix * p.out_cs + p.out_co + n;
+        float l[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) l[k] = a[k] - __uint_as_float(__float_as_uint(a[k]) & 0xFFFFE000u);
+        if (full8) st8(olo, l);
+        else *reinterpret_cast<float4*>(olo) = make_float4(l[0], l[1], l[2], l[3]);
+    }
+    if (p.out_h16_hi) {      // fp16 hi/lo planes for the next fp16-split conv
+        __half* oh = reinterpret_cast<__half*>(p.out_h16_hi) + pix * p.out_cs + p.out_co + n;
+        __half* ol16 = reinterpret_cast<__half*>(p.out_h16_lo) + pix * p.out_cs + p.out_co + n;
+        uint2 h0, l0, h1, l1;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) amax = fmaxf(amax, fabsf(a[k]));     // (in the Cout % 8 == 4 tail a[4..7] belong to zero-weight padding columns)
+        split4(a, h0, l0);
+        if (full8) {
+            split4(a + 4, h1, l1);
+            if (p.v8) {
+                *reinterpret_cast<uint4*>(oh) = make_uint4(h0.x, h0.y, h1.x, h1.y);
+                *reinterpret_cast<uint4*>(ol16) = make_uint4(l0.x, l0.y, l1.x, l1.y);
+            } else {
+                *reinterpret_cast<uint2*>(oh) = h0; *reinterpret_cast<uint2*>(oh + 4) = h1;
+                *reinterpret_cast<uint2*>(ol16) = l0; *reinterpret_cast<uint2*>(ol16 + 4) = l1;
+            }
+        } else {
+            *reinterpret_cast<uint2*>(oh) = h0;
+            *reinterpret_cast<uint2*>(ol16) = l0;
+        }
+    }
+    return amax;
+}
+
+// Epilogue of one tile run by the 256 consumer threads (dcn_fused.cu) after the tile's accumulator has been staged in shared memory ([128][ld]
+// fp32, row = tile pixel): thread (warp, lane) owns pixel row 32 (warp % 4) + lane and column half warp / 4.  Returns the largest magnitude
+// written to fp16 planes.  `swz`: the staged tile's chunk swizzle (wg_stage).
 template <int N>
 __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int warp, int lane, int swz = 0) {
     constexpr int HALF = ((N + 31) / 32) * 16;                     // accumulator columns per thread
@@ -201,81 +281,16 @@ __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* 
     const float* acc = tile + r * ld;
     int sw = r & swz;
     if (swz) asm volatile("" : "+r"(sw));                           // (as in wg_stage)
-    const float* rp = (p.res && !(p.dbg & 32)) ? p.res + pix * p.res_cs + p.res_co : nullptr;
-    const __half* rph = (p.res_h16_hi && !(p.dbg & 32)) ? reinterpret_cast<const __half*>(p.res_h16_hi) + pix * p.res_cs + p.res_co : nullptr;
-    const __half* rpl = rph ? reinterpret_cast<const __half*>(p.res_h16_lo) + pix * p.res_cs + p.res_co : nullptr;
-    float* op = p.out ? p.out + pix * p.out_cs + p.out_co : nullptr;            // nullptr: planes-only output, no fp32 copy is written
-    float* olo = p.out_lo ? p.out_lo + pix * p.out_cs + p.out_co : nullptr;
-    __half* oh = p.out_h16_hi ? reinterpret_cast<__half*>(p.out_h16_hi) + pix * p.out_cs + p.out_co : nullptr;
-    __half* ol16 = p.out_h16_lo ? reinterpret_cast<__half*>(p.out_h16_lo) + pix * p.out_cs + p.out_co : nullptr;
     const int nbase = nt * p.BN + cb;
-    const bool v8 = p.v8 != 0;
-    const float osc = p.out_scale;
 #pragma unroll
     for (int col = 0; col < HALF; col += 8) {
         const int n = nbase + col;
         if (col < ncols && n + 4 <= p.Cout) {
-            const bool full8 = n + 8 <= p.Cout;                  // else the Cout % 8 == 4 tail
             float rr[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) rr[k] = 0.f;
-            if (rp) {
-                if (full8) ld8(rp + n, rr);
-                else { const float4 t4 = ldg4(rp + n); rr[0] = t4.x; rr[1] = t4.y; rr[2] = t4.z; rr[3] = t4.w; }
-            } else if (rph) {
-                if (full8) ld8_planes(rph + n, rpl + n, v8, rr); else ld4_planes(rph + n, rpl + n, rr);
-            }
+            tcp_epi_res(p, pix, n, rr);
             const int j = (cb + col) >> 2;                       // 16-byte chunk of the staged row
             const float4 a0 = *reinterpret_cast<const float4*>(acc + ((j ^ sw) << 2)), a1 = *reinterpret_cast<const float4*>(acc + (((j + 1) ^ sw) << 2));
-            const float av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            float a[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) a[k] = av[k] * osc + rr[k];
-            if (p.bias) {
-                if (full8) {
-                    float bb[8];
-                    ld8(p.bias + n, bb);
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) a[k] += bb[k];
-                } else {
-                    const float4 b4 = ldg4(p.bias + n);
-                    a[0] += b4.x; a[1] += b4.y; a[2] += b4.z; a[3] += b4.w;
-                }
-            }
-            if (p.relu) {
-#pragma unroll
-                for (int k = 0; k < 8; ++k) a[k] = fmaxf(a[k], 0.f);
-            }
-            if (op) {
-                if (full8) st8(op + n, a);
-                else *reinterpret_cast<float4*>(op + n) = make_float4(a[0], a[1], a[2], a[3]);
-            }
-            if (olo) {      // tf32 companion for the next 3xTF32 conv: the part of the value the MMA does not see
-                float l[8];
-#pragma unroll
-                for (int k = 0; k < 8; ++k) l[k] = a[k] - __uint_as_float(__float_as_uint(a[k]) & 0xFFFFE000u);
-                if (full8) st8(olo + n, l);
-                else *reinterpret_cast<float4*>(olo + n) = make_float4(l[0], l[1], l[2], l[3]);
-            }
-            if (oh) {      // fp16 hi/lo planes for the next fp16-split conv
-                uint2 h0, l0, h1, l1;
-#pragma unroll
-                for (int k = 0; k < 8; ++k) amax = fmaxf(amax, fabsf(a[k]));     // (in the Cout % 8 == 4 tail a[4..7] belong to zero-weight padding columns)
-                split4(a, h0, l0);
-                if (full8) {
-                    split4(a + 4, h1, l1);
-                    if (v8) {
-                        *reinterpret_cast<uint4*>(oh + n) = make_uint4(h0.x, h0.y, h1.x, h1.y);
-                        *reinterpret_cast<uint4*>(ol16 + n) = make_uint4(l0.x, l0.y, l1.x, l1.y);
-                    } else {
-                        *reinterpret_cast<uint2*>(oh + n) = h0; *reinterpret_cast<uint2*>(oh + n + 4) = h1;
-                        *reinterpret_cast<uint2*>(ol16 + n) = l0; *reinterpret_cast<uint2*>(ol16 + n + 4) = l1;
-                    }
-                } else {
-                    *reinterpret_cast<uint2*>(oh + n) = h0;
-                    *reinterpret_cast<uint2*>(ol16 + n) = l0;
-                }
-            }
+            amax = fmaxf(amax, tcp_epi_out(p, pix, n, a0, a1, rr));
         }
     }
     return amax;
