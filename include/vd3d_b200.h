@@ -133,9 +133,10 @@ int vd3d_image_to_h16_rows_c(const float* img, int B, int C, int H, int W, void*
 int vd3d_row_conv(const void* in_hi, const void* in_lo, int B, int H, int W, int Wp, int xoff, int pc, int KH, int KW, int S, int P,
                   const void* w_hi, const void* w_lo, float out_scale, const float* bias, int relu, int N,
                   float* out, void* out_hi16, void* out_lo16, int out_W, int out_xoff, int out_cs, int out_co, void* stream);
-/* Diagnostics: when set, CTA 0 of every persistent tensor-core conv writes clock64 stamps into a [9][n] int64 device buffer: per k-block
- * 0 stage free / 1 loads issued / 2 MMA thread waits / 3 stage landed / 4 MMAs issued, per tile 5 last MMAs done / 6 staged and handed to
- * the epilogue warps / 7 epilogue start / 8 epilogue done and stage released; NULL disables (tools/trace_conv.py). */
+/* Diagnostics: when set, CTA 0 of every persistent tensor-core conv writes clock64 stamps into a [12][n] int64 device buffer: per k-block
+ * 0 stage free / 1 loads issued / 2 MMA thread waits / 3 stage landed / 4 MMAs issued / 9 ring slot (a value, not a stamp), per tile
+ * 5 last MMAs done / 6 staged and handed to the epilogue warps / 7 epilogue start / 8 stage released / 10 times the producer passed over
+ * the held slot (a count) / 11 epilogue done; NULL disables (tools/trace_conv.py). */
 void vd3d_tc_set_trace(void* dev_i64, int n);
 /* fp32 channel slice -> fp16 (hi, lo) planes (producers that are not tensor-core convs). */
 int vd3d_split_h16_nhwc(const float* in, void* hi16, void* lo16, long long npix, int C, int cs, int co, void* stream);

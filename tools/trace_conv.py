@@ -24,27 +24,45 @@ for si in sel:
         os.environ["VD3D_TC_CG"] = str(cg)
         layer.bn_tile = bn
         layer(x, out); torch.cuda.synchronize()
-        tr = torch.zeros(9, N, dtype=torch.int64, device="cuda")
+        tr = torch.zeros(12, N, dtype=torch.int64, device="cuda")
         lib.vd3d_tc_set_trace(tr.data_ptr(), N)
         layer(x, out); torch.cuda.synchronize()
         lib.vd3d_tc_set_trace(None, 0)
         t = tr.cpu().numpy().astype(np.float64)
-        # per tile (rows 5..8): last MMAs done, staged and handed over, epilogue start, stage released / epilogue done; the next tile's first
-        # MMAs start at k-block (i + 1) * KB of row 3
+        # per tile (rows 5..8, 11): last MMAs done, staged and handed over, epilogue start, stage released, epilogue done; the next tile's
+        # first MMAs start at k-block (i + 1) * KB of row 3
         KB = 9 * ((Cin + 63) // 64)
-        first = t[3, :int((t[3] > 0).sum()):KB]                      # first MMAs of each tile
+        nkb = int((t[3] > 0).sum())
+        first = t[3, :nkb:KB]                                        # first MMAs of each tile
         if len(first) > 2:
             print(f"{name:30s} cg={cg} bn={bn:3d} tile period (first MMA to first MMA) {np.median(np.diff(first)):7.0f} clk", flush=True)
         nt = int((t[5] > 0).sum())
         if nt > 2 and (t[7, :nt] > 0).all():                        # (tiles of <= 64 columns run the epilogue on the consumers: no hand-off)
             ti = np.arange(nt - 1)
-            last, staged, estart, edone = t[5, ti], t[6, ti], t[7, ti], t[8, ti]
+            last, staged, estart, erel, edone = t[5, ti], t[6, ti], t[7, ti], t[8, ti], t[11, ti]
             nxt = t[3, np.minimum((ti + 1) * KB, N - 1)]
-            ok = (ti + 1) * KB < int((t[3] > 0).sum())
+            ok = (ti + 1) * KB < nkb
             med = lambda v: np.median(v[ok]) if ok.any() else float("nan")
             print(f"{name:30s} cg={cg} bn={bn:3d} tiles={nt} k-blocks/tile={KB}  tile period {np.median(np.diff(t[5, :nt])):7.0f}  "
                   f"last MMA -> staged {med(staged - last):6.0f}  staged -> epilogue start {med(estart - staged):6.0f}  "
-                  f"epilogue (stage held) {med(edone - estart):6.0f}  last MMA -> next tile's first MMA {med(nxt - last):6.0f} clk", flush=True)
+                  f"stage held {med(erel - estart):6.0f}  epilogue {med(edone - estart):6.0f}  "
+                  f"last MMA -> next tile's first MMA {med(nxt - last):6.0f} clk", flush=True)
+        # per tile: ring slot of every k-block (row 9), the longest wait for a stage ([3] - [2]) and where it fell, how often the producer
+        # passed over the held slot (row 10).  With the held slot passed over, no k-block after a tile's second should wait about as long
+        # as the epilogue holds its stage.
+        wait_kb = t[3, :nkb] - t[2, :nkb]
+        late = []
+        for i in range(min(nt, nkb // KB)):
+            w = wait_kb[i * KB:(i + 1) * KB]
+            if KB > 2:
+                late.append(w[2:].max())
+            if i < 6:
+                sl = "".join(str(int(v)) for v in t[9, i * KB:(i + 1) * KB][:48]) + ("..." if KB > 48 else "")
+                print(f"   tile {i:3d}: slots {sl}  longest stage wait {w.max():7.0f} clk at k-block {int(w.argmax()):3d}  "
+                      f"held slot passed over {int(t[10, i])}x", flush=True)
+        if late:
+            print(f"{name:30s} cg={cg} bn={bn:3d} longest stage wait after a tile's second k-block: median over tiles {np.median(late):7.0f}, "
+                  f"max {np.max(late):7.0f} clk; held slot passed over {int(t[10, :nt].sum())}x in {nt} tiles", flush=True)
         n = int((t[0] > 0).sum())
         t = t[:, :n]
         t0 = t[0, 0]

@@ -106,7 +106,15 @@ __global__ void pool_border_zero_kernel(float* __restrict__ out, int B, int Hp, 
 
 // ----------------------------------------------------------------------------------------------------------------
 // Persistent kernel.  Shared memory: [stages][A hi | A lo | W hi | W lo] operand ring, the [128][BN + 4] fp32 staged accumulator (unless it is
-// staged in the ring: TcParams::tile_in_ring), barriers.
+// staged in the ring: TcParams::tile_in_ring; then rows 64..127 of it when TcParams::split_stage), barriers, the slot log.
+//
+// Ring slots.  The producer takes the slots round-robin, but passes over the held slot (the stage of a tile's last k-block, where the
+// accumulator is staged) while the epilogue has not released it, so the next tile's K loop keeps the other stages flowing, and takes the
+// held slot back as soon as it is released (also while it waits for another slot).  The consumers
+// cannot predict that order: the producer writes the slot of every k-block into a log of stages + 1 entries, each with a one-arrival
+// mbarrier, and the consumers read it before they wait on full[slot].  stages + 1 entries suffice: of any stages + 1 consecutive k-blocks two
+// share a slot, so the later one was loaded only after the consumers (or the epilogue, after the consumers staged the tile) released the
+// earlier one, and they had read its log entry by then.  Every slot keeps its own phase bit on both sides.
 // ----------------------------------------------------------------------------------------------------------------
 // Warps 0..7 = consumers, warp 8 = TMA producer, warps 9..11 = epilogue.  ptxas budgets registers per whole warpgroup (65536 / 384 = 168 per
 // thread here; a fourth warpgroup would cap every thread at 128, below what the 128-column consumers need), so the epilogue gets the three
@@ -116,17 +124,23 @@ constexpr int TCP_THREADS = TC_CONSUMERS + 32 + TCP_EPI;
 // row pitch (floats) of the staged accumulator: BN + 4 (conflict-free rows); at BN = 128 unpadded rows with the chunk swizzle of wg_stage,
 // so that the 64 KB tile fits in one 64 KB operand stage
 __host__ __device__ constexpr int tcp_tile_ld(int BN) { return BN == TC_MAX_BN ? BN : BN + 4; }
+// Tiles wider than 64 columns hand their epilogue to the epilogue warps.  Narrower tiles keep it on the consumers (the stem's fused
+// max-pool among them): their K loop is short (64 columns: 9 k-blocks of ~890 clocks for a 64-channel 3x3 conv, H100) and the three
+// epilogue warps take longer per tile (~11 k clocks) than the 256 consumer threads, so overlapping made those layers slower.
+__host__ __device__ constexpr bool tcp_epi_warps(int BN) { return BN > 64; }
 // named barrier of the epilogue warps
 __device__ __forceinline__ void epilogue_sync() { asm volatile("bar.sync 3, %0;" ::"n"(TCP_EPI) : "memory"); }
 
 // Epilogue of one staged tile by the epilogue warps (thread et of TCP_EPI).  Item = (pixel row r, 8-column group g), items numbered row-major,
 // thread et takes items et, et + TCP_EPI, ...: consecutive lanes cover consecutive column groups of one pixel, so a warp's residual loads and
 // output stores are whole runs of a pixel's channels (at BN = 128, 256 contiguous bytes per fp16 plane).  The residual loads of U items are
-// issued before the first of them is computed.  Per element the arithmetic is that of tcp_store_tile.
+// issued before the first of them is computed.  Per element the arithmetic is that of tcp_store_tile.  Covers tile rows r0 .. r1 - 1; row r
+// is read at tile + r * ld.
 template <int BN>
-__device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int et, int swz) {
+__device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int et, int swz, int r0, int r1) {
     constexpr int CG = BN / 8;                                   // column groups per pixel
-    constexpr int ITEMS = 128 * CG, U = 8;
+    constexpr int U = 8;
+    const int ITEMS = r1 * CG;
     int mu, nt;
     unit_tile(p, u, mt_units, mu, nt);
     const int ncols = min(BN, p.cout_pad - nt * BN);              // valid columns of this tile
@@ -135,7 +149,7 @@ __device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* ti
     const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
     float amax = 0.f;
     if (p.dbg & 16) return amax;
-    for (int i0 = et; i0 < ITEMS; i0 += U * TCP_EPI) {
+    for (int i0 = r0 * CG + et; i0 < ITEMS; i0 += U * TCP_EPI) {
         float rr[U][8];
         long long pix[U];
         int rg[U];                                               // item = r * CG + g, or -1: nothing to write
@@ -175,12 +189,20 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     const uint32_t b_bytes = (uint32_t)BN * rowb;
     const uint32_t stage_bytes = 2u * a_bytes + 2u * b_bytes;      // [A hi | A lo | W hi | W lo]
     const int kbc = (int)rowb / (F16 ? 2 : 4);                     // channels per k-block
-    float* const tile_sep = reinterpret_cast<float*>(smem + (size_t)p.stages * stage_bytes);      // (tile_in_ring == 0)
-    uint64_t* full = reinterpret_cast<uint64_t*>(in_ring ? smem + (size_t)p.stages * stage_bytes : reinterpret_cast<uint8_t*>(tile_sep + 128 * LD));  // [stages]  TMA -> consumers
+    constexpr bool epi_warps = tcp_epi_warps(BN);
+    // (in_ring) split staging: rows 0..63 of the accumulator go to the held stage, rows 64..127 to a separate half tile, so the epilogue can
+    // release the stage after the first half
+    const bool split = epi_warps && in_ring && p.split_stage != 0;
+    float* const tile_sep = reinterpret_cast<float*>(smem + (size_t)p.stages * stage_bytes);      // (tile_in_ring == 0) the tile; (split) rows 64..127
+    float* const tile_hi = tile_sep - 64 * LD;                      // (split) row r >= 64 at tile_hi + r * LD
+    const int sep_rows = in_ring ? (split ? 64 : 0) : 128;
+    uint64_t* full = reinterpret_cast<uint64_t*>(tile_sep + sep_rows * LD);     // [stages]  TMA -> consumers
     uint64_t* empty = full + p.stages;                              // [stages]  consumers (8 warps; the held stage: epilogue warps) -> TMA
-    uint64_t* acc_full = empty + p.stages;                          // consumers (256 threads) -> epilogue: a tile is staged
+    uint64_t* log_bar = empty + p.stages;                           // [stages + 1]  producer -> consumers: slot_log entry written
+    uint64_t* acc_full = log_bar + p.stages + 1;                    // consumers (256 threads) -> epilogue: a tile is staged
     uint64_t* acc_empty = acc_full + 1;                             // epilogue -> consumers: the staged tile has been read
     int* mailbox = reinterpret_cast<int*>(acc_empty + 1);           // (in_ring) ring slot of the staged tile
+    int* slot_log = mailbox + 1;                                    // [stages + 1]  ring slot of k-block g at entry g % (stages + 1)
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;      // (warp-uniform for the compiler)
     const int cchunks = p.cin_pad / kbc;
@@ -189,13 +211,10 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     const int units = mt_units * p.n_tiles;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
     const int mode = tc_mma_mode(p);
-    // Tiles wider than 64 columns hand their epilogue to the epilogue warps.  Narrower tiles keep it on the consumers (the stem's fused
-    // max-pool among them): their K loop is short (64 columns: 9 k-blocks of ~890 clocks for a 64-channel 3x3 conv, H100) and the three
-    // epilogue warps take longer per tile (~11 k clocks) than the 256 consumer threads, so overlapping made those layers slower.
-    constexpr bool epi_warps = BN > 64;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], TC_CONSUMERS / 32); }
+        for (int e = 0; e <= p.stages; ++e) mbar_init(&log_bar[e], 1);
         mbar_init(acc_full, TC_CONSUMERS);
         mbar_init(acc_empty, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -217,15 +236,24 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
             if (tr) p.trace[7 * p.trace_n + i] = clock64();                                     // [7] epilogue starts
             const int held = *mailbox;
             const float* tile = in_ring ? reinterpret_cast<const float*>(smem + (size_t)held * stage_bytes) : tile_sep;
-            amax = fmaxf(amax, tcp_epi_tile<BN>(p, tile, LD, u, mt_units, et, swz));
-            // every epilogue thread is done reading the staged tile (and the mailbox): give the stage back to the producer (empty[] counts the
-            // 8 consumer warps' arrivals) and the staging buffer to the consumers
-            if (in_ring) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic accesses to the stage before the next TMA write into it
-            epilogue_sync();
-            if (et == 0) {
-                if (in_ring) mbar_arrive(&empty[held], TC_CONSUMERS / 32);
-                mbar_arrive(acc_empty);
-                if (tr) p.trace[8 * p.trace_n + i] = clock64();                                 // [8] stage released, epilogue done
+            // split: the held stage's rows first, then give the stage back and do the rest from the half tile
+            for (int part = 0; part < (split ? 2 : 1); ++part) {
+                const bool last = !split || part == 1;
+                amax = fmaxf(amax, tcp_epi_tile<BN>(p, part == 0 ? tile : tile_hi, LD, u, mt_units, et, swz, 64 * part, last ? 128 : 64));
+                // every epilogue thread is done reading the held stage (and the mailbox): give the stage back to the producer (empty[] counts
+                // the 8 consumer warps' arrivals), and at the end the staging buffers to the consumers
+                if (in_ring && part == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic accesses to the stage before the next TMA write into it
+                epilogue_sync();
+                if (et == 0) {
+                    if (in_ring && part == 0) {
+                        mbar_arrive(&empty[held], TC_CONSUMERS / 32);
+                        if (tr) p.trace[8 * p.trace_n + i] = clock64();                         // [8] stage released
+                    }
+                    if (last) {
+                        mbar_arrive(acc_empty);
+                        if (tr) p.trace[11 * p.trace_n + i] = clock64();                        // [11] epilogue done
+                    }
+                }
             }
         }
         note_fp16_range(amax, p.range_flag);
@@ -234,8 +262,12 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
             // ================= TMA producer =================
             const bool lo_too = mode != 1 && !(p.dbg & 2);
             const uint32_t tx = lo_too ? stage_bytes : a_bytes + b_bytes;
-            int it = 0, s = 0, ph = 0;
-            for (int u = u0; u < units; u += ustep) {
+            int it = 0, s = 0, i = 0;
+            int ph = 0;                                         // bit s: parity of slot s's next fill
+            int held = -1;                                      // (in_ring) slot of the latest tile's last k-block, until seen released
+            int le = 0;                                         // slot_log entry of k-block it
+            for (int u = u0; u < units; u += ustep, ++i) {
+                int skips = 0;
                 int mu, nt;
                 unit_tile(p, u, mt_units, mu, nt);
                 int mt = mu;
@@ -245,24 +277,47 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                 const int n0 = nt * BN;
                 int tap = 0, kh = 0, kw = 0, c0 = 0;
                 for (int kb = 0; kb < KB; ++kb, ++it) {
-                    mbar_wait(&empty[s], ph ^ 1);
+                    int slot = s;
+                    if (held < 0) mbar_wait(&empty[s], ((ph >> s) & 1) ^ 1);
+                    else {
+                        // The epilogue may still be reading the held stage.  Take it as soon as it is released; until then take the next
+                        // slot in round-robin order, passing over the held one (the slot after it is not held).
+                        const bool at_held = s == held;
+                        if (at_held && ++s == p.stages) s = 0;
+                        const uint32_t hpar = ((ph >> held) & 1) ^ 1, spar = ((ph >> s) & 1) ^ 1;
+                        long long t0 = 0;
+                        for (uint32_t spins = 1;; ++spins) {
+                            if (mbar_test(&empty[held], hpar)) { slot = held; held = -1; break; }
+                            if (mbar_test(&empty[s], spar)) { slot = s; skips += at_held; break; }
+                            if ((spins & 0xFFFu) == 0) {                // bounded, as mbar_wait
+                                const long long t = clock64();
+                                if (t0 == 0) t0 = t; else if (t - t0 > 4000000000LL) __trap();
+                            }
+                        }
+                    }
+                    if (slot == s && ++s == p.stages) s = 0;
+                    ph ^= 1 << slot;
                     const bool tr = p.trace && blockIdx.x == 0 && it < p.trace_n;
                     if (tr) p.trace[it] = clock64();                                          // [0] stage free, about to issue the loads
-                    uint8_t* st = smem + (size_t)s * stage_bytes;
+                    slot_log[le] = slot;
+                    mbar_arrive(&log_bar[le]);
+                    if (++le > p.stages) le = 0;
+                    if (in_ring && kb == KB - 1) held = slot;
+                    uint8_t* st = smem + (size_t)slot * stage_bytes;
                     const int wi = wi0 + kw * p.dil, hi = hi0 + kh * p.dil;
                     const int kcol = tap * p.cin_pad + c0;
-                    mbar_expect_tx(&full[s], tx);
-                    tma_load_4d(st, &mapA, &full[s], c0, wi, hi, b);
-                    if (lo_too) tma_load_4d(st + a_bytes, &mapAlo, &full[s], c0, wi, hi, b);
-                    tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[s], kcol, n0);
-                    if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[s], kcol, n0);
-                    if (tr) p.trace[p.trace_n + it] = clock64();                              // [1] loads issued
-                    if (++s == p.stages) { s = 0; ph ^= 1; }
+                    mbar_expect_tx(&full[slot], tx);
+                    tma_load_4d(st, &mapA, &full[slot], c0, wi, hi, b);
+                    if (lo_too) tma_load_4d(st + a_bytes, &mapAlo, &full[slot], c0, wi, hi, b);
+                    tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[slot], kcol, n0);
+                    if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[slot], kcol, n0);
+                    if (tr) { p.trace[p.trace_n + it] = clock64(); p.trace[9 * p.trace_n + it] = slot; }  // [1] loads issued, [9] slot
                     // k-block order: channel chunk outermost, taps inside
                     ++tap;
                     if (++kw == p.KW) { kw = 0; ++kh; }
                     if (tap == p.KH * p.KW) { tap = 0; kh = 0; kw = 0; c0 += kbc; }
                 }
+                if (p.trace && blockIdx.x == 0 && i < p.trace_n) p.trace[10 * p.trace_n + i] = skips;     // [10] held slot passed over
             }
         }
     } else {
@@ -271,18 +326,22 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
         const uint32_t sbo = 8u * rowb, lay = rowb == 128u ? 2u : 4u;
         const int ksteps = (int)rowb / 32;
         const bool tr0 = p.trace && blockIdx.x == 0 && threadIdx.x == 0;
-        int s = 0, ph = 0, g = 0;
+        int ph = 0, g = 0;                                      // ph bit s: parity of slot s's next fill
+        int le = 0, lph = 0;                                    // slot_log entry of k-block g and the parity of its barrier
         auto acquire = [&]() {
             const bool tr = tr0 && g < p.trace_n;
             if (tr) p.trace[2 * p.trace_n + g] = clock64();                                    // [2] waiting for the stage
-            mbar_wait(&full[s], ph);
+            mbar_wait(&log_bar[le], lph);
+            // (a shuffle makes the slot warp-uniform for the compiler: read per thread, it costs the K loop ~20 registers and spills at BN = 128)
+            const int s = __shfl_sync(0xffffffffu, slot_log[le], 0);
+            if (++le > p.stages) { le = 0; lph ^= 1; }
+            mbar_wait(&full[s], (ph >> s) & 1);
+            ph ^= 1 << s;
             if (tr) p.trace[3 * p.trace_n + g] = clock64();                                    // [3] about to issue k-block g
             const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
             const uint32_t aw = sa + (uint32_t)wg * 64u * rowb;
-            const KbOperands o = {make_sdesc(aw, sbo, lay), make_sdesc(aw + a_bytes, sbo, lay),
-                                  make_sdesc(sa + 2 * a_bytes, sbo, lay), make_sdesc(sa + 2 * a_bytes + b_bytes, sbo, lay), s};
-            if (++s == p.stages) { s = 0; ph ^= 1; }
-            return o;
+            return KbOperands{make_sdesc(aw, sbo, lay), make_sdesc(aw + a_bytes, sbo, lay),
+                              make_sdesc(sa + 2 * a_bytes, sbo, lay), make_sdesc(sa + 2 * a_bytes + b_bytes, sbo, lay), s};
         };
         auto release = [&](int st) {
             __syncwarp();
@@ -330,7 +389,7 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                 // mailbox (phase i - 1 of acc_empty; a fresh barrier passes parity 1), and (in_ring) both warpgroups' MMAs are done reading the held stage
                 mbar_wait(acc_empty, (i & 1) ^ 1);
                 consumers_sync();
-                wg_stage<BN>(tot, tile, LD, wg, warp, lane, swz);
+                wg_stage<BN>(tot, split && wg == 1 ? tile_hi : tile, LD, wg, warp, lane, swz);
                 if (threadIdx.x == 0) *mailbox = held;
                 mbar_arrive(acc_full);
                 if (tr) p.trace[6 * p.trace_n + i] = clock64();                                 // [6] staged and handed over
@@ -431,7 +490,7 @@ extern "C" int vd3d_tc_pick_bn(int Cout) {
     return Cout <= 128 ? (Cout + 15) / 16 * 16 : 128;
 }
 
-// diagnostics: clock64 stamps of the TMA / MMA pipeline and the tile hand-off of CTA 0 ([9][n] int64 device buffer; NULL disables)
+// diagnostics: clock64 stamps of the TMA / MMA pipeline and the tile hand-off of CTA 0 ([12][n] int64 device buffer; NULL disables)
 static long long* g_trace = nullptr;
 static int g_trace_n = 0;
 extern "C" void vd3d_tc_set_trace(void* dev_i64, int n) { g_trace = (long long*)dev_i64; g_trace_n = n; }
@@ -472,8 +531,14 @@ static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAl
     if (stages > 8) stages = 8;
     VD3D_REQUIRE(stages >= 2, "conv2d_tc: tile too large for shared memory");
     p.stages = stages;
-    // barrier area: full[stages], empty[stages], acc_full, acc_empty, the mailbox
-    const size_t smem = stages * stage_bytes + (p.tile_in_ring ? 0 : tile_bytes) + (((2 * stages + 3) * sizeof(uint64_t) + 15) / 16 * 16) + 1024;
+    // Split staging (epilogue warps only): when half a staging tile fits next to the ring, rows 64..127 of the accumulator go there and the
+    // held stage is released halfway through the epilogue.  Never at the cost of a stage.
+    const size_t half_bytes = tile_bytes / 2;
+    p.split_stage = p.tile_in_ring && tcp_epi_warps(BN) && stages * stage_bytes + half_bytes <= avail;
+    // barrier area: full[stages], empty[stages], log_bar[stages + 1], acc_full, acc_empty; then the mailbox and slot_log[stages + 1]
+    // (at most 256 bytes: 8 stages)
+    const size_t bar_bytes = ((3 * stages + 3) * sizeof(uint64_t) + (stages + 2) * sizeof(int) + 15) / 16 * 16;
+    const size_t smem = stages * stage_bytes + (p.tile_in_ring ? (p.split_stage ? half_bytes : 0) : tile_bytes) + bar_bytes + 1024;
     const int units = p.m_tiles * p.n_tiles;
     int grid = units < kNumSMs ? units : kNumSMs;
     { const char* e = getenv("VD3D_TC_GRID"); const int cap = e ? atoi(e) : 0; if (cap > 0 && cap < grid) grid = cap; }     // diagnostics

@@ -35,9 +35,10 @@ struct TcParams {
     // conv2d_tcp_kernel: where the accumulator is staged for the epilogue.  1: in the operand stage of the tile's last k-block, held until the
     // epilogue is done (no separate staging tile: one more stage fits); 0: a separate tile after the ring
     int tile_in_ring;
-    int cout_pad;            // Cout rounded up to 16 (ragged last N tile = cout_pad - (n_tiles - 1) * BN columns)
+    int split_stage;         // (tile_in_ring, epilogue warps) rows 64..127 of the staged accumulator go to a half tile after the ring
+    int cout_pad;           // Cout rounded up to 16 (ragged last N tile = cout_pad - (n_tiles - 1) * BN columns)
     int v8;                  // output / residual / bias slices are 32-byte aligned (fp16 plane slices then take 16-byte accesses)
-    long long* trace; int trace_n;   // VD3D diagnostics (vd3d_tc_set_trace): clock64 stamps of CTA 0, [9][trace_n]: rows 0..4 per k-block, 5..8 per tile
+    long long* trace; int trace_n;   // VD3D diagnostics (vd3d_tc_set_trace): clock64 stamps of CTA 0, [12][trace_n]: rows 0..4 and 9 per k-block, 5..8, 10 and 11 per tile
     int dbg;                 // timing experiments only (VD3D_TC_DEBUG; results are wrong): bit 0 = one MMA per k-step, bit 1 = skip the lo-plane loads, bit 4 = no epilogue output, bit 5 = no residual loads
     int out_cs, out_co, res_cs, res_co, relu;
     const float* bias; const float* res; float* out; float* out_lo;
