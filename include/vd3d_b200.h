@@ -92,6 +92,23 @@ int vd3d_conv2d_tc16_planes(const void* in_hi, const void* in_lo, int B, int H, 
                             const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
                             int stride, const float* res, const void* res_hi16, const void* res_lo16, int res_cs, int res_co,
                             float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
+/* vd3d_conv2d_tc16 with the FPN top-down add fused into the epilogue (R/detectors/retinanet_2d.py:49-52): out = conv(in) + bias +
+ * nearest_up2(res), where res is the fp32 tensor [B][res_H][res_W][res_cs] at exactly half the output size (Ho = 2 res_H, Wo = 2 res_W):
+ * output pixel (y, x) reads residual pixel (y >> 1, x >> 1).  3 passes; bn <= 0 = the library's tile policy. */
+int vd3d_conv2d_tc16_res_up2(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                             const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
+                             int stride, const float* res, int res_cs, int res_co, int res_H, int res_W,
+                             float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
+/* One launch of the same conv over L <= 5 tensors of different sizes (the shared-weight RetinaNet head over the pyramid levels, whole batch):
+ * level l reads in_hi[l] / in_lo[l] [B][H[l]][W[l]][in_cs] (its own zero padding) and writes out[l] / out_hi16[l] / out_lo16[l]; the M tiles of all
+ * levels form one persistent tile schedule.  Every output form of level l must lie at a whole-pixel offset from level 0's, the same for all
+ * forms (levels concatenated in one allocation per form); likewise res[l] (fp32, optional; res_W[l] > 0: [B][res_H[l]][res_W[l]] at half the
+ * output size, read nearest-upsampled).  Bit-identical to L separate vd3d_conv2d_tc16 launches (same K order per output pixel). */
+int vd3d_conv2d_tc16_levels(int L, const void* const* in_hi, const void* const* in_lo, const int* H, const int* W, int B, int Cin, int in_cs,
+                            int in_co, const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad,
+                            int dil, int stride, const void* const* res, const int* res_H, const int* res_W, int res_cs, int res_co,
+                            const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
+                            int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
 /* Few-channel KHxKW convolution (the ResNet / DLA stem: conv1 7x7 stride 2, R/backbones/resnet.py:120,186) on the tensor cores.
  * The image is held as fp16 (hi, lo) planes [B][H][Wp][4] (pixel x at column x + pad, zeros elsewhere: the buffer must be
  * zero-initialised once); Wp = vd3d_stem_row_pitch(W, KW, stride, pad).  vd3d_image_to_h16_rows fills the planes from an
@@ -211,6 +228,21 @@ int vd3d_decode_nms(const float* cls, const float* reg, const float* anchors, co
                     float img_w, float img_h, int cap, void* ws,
                     float* out_scores, float* out_boxes, int64_t* out_cls, int32_t* out_anchor,
                     int32_t* out_count, int32_t* out_ncand, void* stream);
+
+/* RetinanetHead.get_bboxes (R/heads/retinanet_head.py:257-307, test mode) batched: max-sigmoid score and label per anchor, top-k
+ * (k = min(nms_pre, N); nms_pre <= 0: k = N) by radix select on the key (score desc, anchor index asc), _decode (:227-255, no clipping),
+ * class-agnostic torchvision NMS (the vd3d_decode_nms sort / NMS stage) and the post-NMS `score > score_thr` as a prefix count.
+ *   level l (of L <= 8) of the head outputs: cls_levels[l] NHWC [B][level_pix[l]][cls_cs] (anchor a, class c at channel a * ncls + c),
+ *   reg_levels[l] [B][level_pix[l]][reg_cs] (a * 4 + j); anchor n = level offset + pixel * A + a; anchors [N][4] f32;
+ *   means4 / stds4: host float[4] (target_means / target_stds).  The arrays cls_levels, reg_levels, level_pix are read on the host.
+ *   workspace: ws, at least vd3d_retina_decode_workspace(B, N, cap) bytes; k must not exceed cap (<= 4096).
+ *   outputs as vd3d_decode_nms (box columns 4..10 are zero; out_count = rows above score_thr) */
+long long vd3d_retina_decode_workspace(int B, int N, int cap);
+int vd3d_retina_decode(int L, const void* const* cls_levels, const void* const* reg_levels, const int* level_pix, int cls_cs, int reg_cs,
+                       const float* anchors, int B, int N, int A, int ncls, int nms_pre, const float* means4, const float* stds4,
+                       float score_thr, double iou_thr, int cap, void* ws,
+                       float* out_scores, float* out_boxes, int64_t* out_cls, int32_t* out_anchor,
+                       int32_t* out_count, int32_t* out_ncand, void* stream);
 
 /* fp16-range guard of the fp16-split tensor-core engine.  Activations travel between tensor-core convs as two fp16 planes (hi, lo) of
  * the UNSCALED fp32 value (the reference's fp32 path has no such limit): |v| >= 65520 would become hi = inf.  Every kernel that writes

@@ -55,6 +55,8 @@ _SIGS = {
     "vd3d_conv2d_tc": (I, [P, P, I, I, I, I, I, I, P, P, P, I, I, I, I, P, I, I, P, P, I, I, I, I, I, I, P]),
     "vd3d_conv2d_tc16": (I, [P, P, I, I, I, I, I, I, P, P, F, P, I, I, I, I, I, P, I, I, P, P, P, I, I, I, I, I, I, P]),
     "vd3d_conv2d_tc16_planes": (I, [P, P, I, I, I, I, I, I, P, P, F, P, I, I, I, I, I, P, P, P, I, I, P, P, P, I, I, I, I, I, P]),
+    "vd3d_conv2d_tc16_res_up2": (I, [P, P, I, I, I, I, I, I, P, P, F, P, I, I, I, I, I, P, I, I, I, I, P, P, P, I, I, I, I, I, P]),
+    "vd3d_conv2d_tc16_levels": (I, [I, P, P, P, P, I, I, I, I, P, P, F, P, I, I, I, I, I, P, P, P, I, I, P, P, P, I, I, I, I, I, P]),
     "vd3d_stem_row_pitch": (I, [I, I, I, I]),
     "vd3d_image_to_h16_rows": (I, [P, I, I, I, I, P, P, I, I, P]),
     "vd3d_conv2d_tc16_stem": (I, [P, P, I, I, I, I, I, I, I, I, I, P, P, F, P, P, P, P, I, I, I, I, P]),
@@ -94,6 +96,8 @@ _SIGS = {
     "vd3d_anchor_mask": (I, [P, P, P, I, I, I, F, F, F, P, P]),
     "vd3d_decode_nms_workspace": (c_longlong, [I, I]),
     "vd3d_decode_nms": (I, [P, P, P, P, P, I, I, I, I, F, c_double, F, F, I, P, P, P, P, P, P, P, P]),
+    "vd3d_retina_decode_workspace": (c_longlong, [I, I, I]),
+    "vd3d_retina_decode": (I, [I, P, P, P, I, I, P, I, I, I, I, I, P, P, F, c_double, I, P, P, P, P, P, P, P, P]),
     "vd3d_kitti_rotate_iou": (I, [P, I, P, I, I, P, P]),
     "vd3d_kitti_eval_workspace_bytes": (c_longlong, [I, c_longlong, c_longlong, c_longlong, I]),
     "vd3d_kitti_eval": (I, [P, P, P, I, c_longlong, c_longlong, c_longlong, c_longlong, P, I, P, I, P, P, P, P, P, P, c_longlong, P]),

@@ -144,9 +144,7 @@ __device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* ti
     int mu, nt;
     unit_tile(p, u, mt_units, mu, nt);
     const int ncols = min(BN, p.cout_pad - nt * BN);              // valid columns of this tile
-    int mt = mu;
-    const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-    const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
+    const TcGeom geo = tile_geom(p, mu);
     float amax = 0.f;
     if (p.dbg & 16) return amax;
     for (int i0 = r0 * CG + et; i0 < ITEMS; i0 += U * TCP_EPI) {
@@ -157,11 +155,11 @@ __device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* ti
         for (int i = 0; i < U; ++i) {
             const int idx = i0 + i * TCP_EPI;
             const int r = idx / CG, g = idx - r * CG;
-            const int ho = th * TC_TH + r / TC_TW, wo = tw * TC_TW + r % TC_TW;
+            const int ho = geo.th * TC_TH + r / TC_TW, wo = geo.tw * TC_TW + r % TC_TW;
             const int n = nt * BN + 8 * g;
-            rg[i] = (idx < ITEMS && ho < p.Ho && wo < p.Wo && 8 * g < ncols && n + 4 <= p.Cout) ? idx : -1;
-            pix[i] = ((long long)b * p.Ho + ho) * p.Wo + wo;
-            if (rg[i] >= 0) tcp_epi_res(p, pix[i], n, rr[i]);
+            rg[i] = (idx < ITEMS && ho < geo.Ho && wo < geo.Wo && 8 * g < ncols && n + 4 <= p.Cout) ? idx : -1;
+            pix[i] = tcp_out_pix(geo, ho, wo);
+            if (rg[i] >= 0) tcp_epi_res(p, tcp_res_pix(geo, ho, wo), n, rr[i]);
         }
 #pragma unroll
         for (int i = 0; i < U; ++i) {
@@ -176,10 +174,15 @@ __device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* ti
     return amax;
 }
 
-template <int BN, bool F16>
+// activation maps of the levels of a multi-level launch (LV); a one-tensor launch passes the empty form
+struct TcLevelMaps { CUtensorMap a[TC_MAX_LEVELS], alo[TC_MAX_LEVELS]; };
+struct TcNoLevelMaps { int unused; };
+
+template <int BN, bool F16, bool LV>
 __global__ void __launch_bounds__(TCP_THREADS, 1)
 conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAlo,
-                  const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
+                  const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p,
+                  const __grid_constant__ std::conditional_t<LV, TcLevelMaps, TcNoLevelMaps> lmaps) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     constexpr int LD = tcp_tile_ld(BN), swz = BN == TC_MAX_BN ? 7 : 0;
@@ -270,10 +273,12 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                 int skips = 0;
                 int mu, nt;
                 unit_tile(p, u, mt_units, mu, nt);
-                int mt = mu;
-                const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-                const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
-                const int wi0 = tw * TC_TW * p.stride_w - p.pad_w, hi0 = th * TC_TH * p.stride - p.pad;
+                const TcGeom geo = tile_geom(p, mu);
+                const int b = geo.b;
+                const int wi0 = geo.tw * TC_TW * p.stride_w - p.pad_w, hi0 = geo.th * TC_TH * p.stride - p.pad;
+                const CUtensorMap* mA = &mapA;
+                const CUtensorMap* mAlo = &mapAlo;
+                if constexpr (LV) { mA = &lmaps.a[geo.lvl]; mAlo = &lmaps.alo[geo.lvl]; }
                 const int n0 = nt * BN;
                 int tap = 0, kh = 0, kw = 0, c0 = 0;
                 for (int kb = 0; kb < KB; ++kb, ++it) {
@@ -307,8 +312,8 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                     const int wi = wi0 + kw * p.dil, hi = hi0 + kh * p.dil;
                     const int kcol = tap * p.cin_pad + c0;
                     mbar_expect_tx(&full[slot], tx);
-                    tma_load_4d(st, &mapA, &full[slot], c0, wi, hi, b);
-                    if (lo_too) tma_load_4d(st + a_bytes, &mapAlo, &full[slot], c0, wi, hi, b);
+                    tma_load_4d(st, mA, &full[slot], c0, wi, hi, b);
+                    if (lo_too) tma_load_4d(st + a_bytes, mAlo, &full[slot], c0, wi, hi, b);
                     tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[slot], kcol, n0);
                     if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[slot], kcol, n0);
                     if (tr) { p.trace[p.trace_n + it] = clock64(); p.trace[9 * p.trace_n + it] = slot; }  // [1] loads issued, [9] slot
@@ -495,20 +500,22 @@ static long long* g_trace = nullptr;
 static int g_trace_n = 0;
 extern "C" void vd3d_tc_set_trace(void* dev_i64, int n) { g_trace = (long long*)dev_i64; g_trace_n = n; }
 
-template <int BN, bool F16>
+template <int BN, bool F16, bool LV>
 static cudaError_t tcp_launch_kernel(const cudaLaunchConfig_t& cfg, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi,
-                                     const CUtensorMap& mWlo, const TcParams& p) {
+                                     const CUtensorMap& mWlo, const TcParams& p, const std::conditional_t<LV, TcLevelMaps, TcNoLevelMaps>& lm) {
     static bool attr_set = false;
     if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(conv2d_tcp_kernel<BN, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        const cudaError_t e = cudaFuncSetAttribute(conv2d_tcp_kernel<BN, F16, LV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    return cudaLaunchKernelEx(&cfg, conv2d_tcp_kernel<BN, F16>, mA, mAlo, mWhi, mWlo, p);
+    return cudaLaunchKernelEx(&cfg, conv2d_tcp_kernel<BN, F16, LV>, mA, mAlo, mWhi, mWlo, p, lm);
 }
 
-// launch of the persistent kernel: p.BN (<= TC_MAX_BN) / p.chunk / tile counts are set by the caller, the weight maps have BN rows per box
-static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi, const CUtensorMap& mWlo, void* stream) {
+// launch of the persistent kernel: p.BN (<= TC_MAX_BN) / p.chunk / tile counts are set by the caller, the weight maps have BN rows per box;
+// `lm`: the per-level activation maps of a multi-level launch (p.n_levels > 0, fp16 operands only)
+static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi, const CUtensorMap& mWlo, void* stream,
+                      const TcLevelMaps* lm = nullptr) {
     const int BN = p.BN;
     { const char* e = getenv("VD3D_TC_DEBUG"); p.dbg = e ? atoi(e) : 0; }
     p.trace = g_trace; p.trace_n = g_trace_n;
@@ -553,7 +560,10 @@ static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAl
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
     cudaError_t le = cudaErrorInvalidValue;
-#define VD3D_TCP_CASE(N) case N: le = p.f16 ? tcp_launch_kernel<N, true>(cfg, mA, mAlo, mWhi, mWlo, p) : tcp_launch_kernel<N, false>(cfg, mA, mAlo, mWhi, mWlo, p); break
+    VD3D_REQUIRE(!lm || (p.f16 && p.n_levels > 0), "conv2d_tc: multi-level launches take fp16 operands");
+    const TcNoLevelMaps nolm{0};
+#define VD3D_TCP_CASE(N) case N: le = lm ? tcp_launch_kernel<N, true, true>(cfg, mA, mAlo, mWhi, mWlo, p, *lm) : p.f16 ? \
+        tcp_launch_kernel<N, true, false>(cfg, mA, mAlo, mWhi, mWlo, p, nolm) : tcp_launch_kernel<N, false, false>(cfg, mA, mAlo, mWhi, mWlo, p, nolm); break
     switch (BN) {
         VD3D_TCP_CASE(16); VD3D_TCP_CASE(32); VD3D_TCP_CASE(48); VD3D_TCP_CASE(64);
         VD3D_TCP_CASE(80); VD3D_TCP_CASE(96); VD3D_TCP_CASE(112); VD3D_TCP_CASE(128);
@@ -570,11 +580,20 @@ static int fit_bn(int bn) {
     return bn;
 }
 
+// levels of a multi-level launch (vd3d_conv2d_tc16_levels): activation pointers and sizes per level, output / residual pixel offsets
+struct LevelSpec {
+    int L;
+    const void* in_hi[TC_MAX_LEVELS]; const void* in_lo[TC_MAX_LEVELS];
+    int H[TC_MAX_LEVELS], W[TC_MAX_LEVELS], res_H[TC_MAX_LEVELS], res_W[TC_MAX_LEVELS];
+    long long out_off[TC_MAX_LEVELS], res_off[TC_MAX_LEVELS];
+};
+
 static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
                             const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil, int stride,
                             const float* res, int res_cs, int res_co, float* out, float* out_lo, void* out_h16_hi, void* out_h16_lo,
                             int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream,
-                            const void* res_h16_hi = nullptr, const void* res_h16_lo = nullptr) {
+                            const void* res_h16_hi = nullptr, const void* res_h16_lo = nullptr, int res_up_H = 0, int res_up_W = 0,
+                            const LevelSpec* ls = nullptr) {
     VD3D_REQUIRE(in && w_hi && (out || out_h16_hi), "conv2d_tc: null pointer");
     VD3D_REQUIRE(!(res && res_h16_hi) && (!res_h16_hi == !res_h16_lo), "conv2d_tc: the residual is either an fp32 tensor or an fp16 (hi, lo) plane pair");
     const int two_pass = (f16 && passes == 2) ? 1 : 0;        // error-budget experiments: 3-pass machinery with the A_lo * W_hi product dropped
@@ -591,8 +610,13 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     int BN = bn;
     if (BN <= 0) {
         if (f16 && passes == 3) {
-            const int Ho_ = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1, Wo_ = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
-            BN = pick_bn_cost(Cout, cdiv(Wo_, TC_TW) * cdiv(Ho_, TC_TH) * B);
+            int mt_all = 0;
+            for (int l = 0; l < (ls ? ls->L : 1); ++l) {
+                const int h = ls ? ls->H[l] : H, w = ls ? ls->W[l] : W;
+                const int Ho_ = (h + 2 * pad - dil * (KH - 1) - 1) / stride + 1, Wo_ = (w + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+                mt_all += cdiv(Wo_, TC_TW) * cdiv(Ho_, TC_TH) * B;
+            }
+            BN = pick_bn_cost(Cout, mt_all);
             // short-K layers (the 1x1 expansion convs of the ResNet bottlenecks: 4 k-blocks, wide output, residual): a tile's MMAs are over
             // before its epilogue has fetched the first residual columns; 64-column tiles put twice as many CTAs on the output
             const char* esk = getenv("VD3D_TC_SHORTK");
@@ -617,6 +641,25 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     p.cout_pad = (Cout + 15) / 16 * 16;
     p.m_tiles = p.tiles_w * p.tiles_h * B; p.n_tiles = cdiv(p.cout_pad, BN);
     p.rowb = 128;
+    if (ls) {
+        // concatenated M tiles of the levels (tile_geom); the level's own maps give each its zero padding
+        VD3D_REQUIRE(ls->L >= 1 && ls->L <= TC_MAX_LEVELS && f16 && passes == 3 && !res_h16_hi && res_up_W == 0, "conv2d_tc16_levels: bad level set");
+        p.n_levels = ls->L;
+        int mt = 0;
+        for (int l = 0; l < ls->L; ++l) {
+            TcLevel& v = p.lv[l];
+            v.Ho = (ls->H[l] + 2 * pad - dil * (KH - 1) - 1) / stride + 1; v.Wo = (ls->W[l] + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+            VD3D_REQUIRE(v.Ho > 0 && v.Wo > 0, "conv2d_tc16_levels: level %d has an empty output", l);
+            v.tiles_w = cdiv(v.Wo, TC_TW); v.tiles_h = cdiv(v.Ho, TC_TH);
+            v.m_begin = mt;
+            mt += v.tiles_w * v.tiles_h * B;
+            v.pix_off = ls->out_off[l]; v.res_off = ls->res_off[l];
+            v.res_H = ls->res_H[l]; v.res_W = ls->res_W[l];
+            VD3D_REQUIRE(v.res_W == 0 || (res && v.Ho == 2 * v.res_H && v.Wo == 2 * v.res_W),
+                         "conv2d_tc16_levels: level %d: an upsampled residual needs exactly half the output size", l);
+        }
+        p.m_tiles = mt;
+    }
     {
         // L2-aware tile order (unit_tile): M blocks whose activation slab (the block's input pixels, all channels, both planes) is about
         // VD3D_TC_L2MB megabytes (default 20: well inside the 50 MB L2), only when there is more than one N tile (otherwise A is read once
@@ -641,6 +684,11 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     p.out_cs = out_cs; p.out_co = out_co; p.res_cs = res_cs; p.res_co = res_co; p.relu = relu;
     p.bias = bias; p.res = res; p.out = out; p.out_lo = out_lo; p.out_h16_hi = out_h16_hi; p.out_h16_lo = out_h16_lo;
     p.res_h16_hi = res_h16_hi; p.res_h16_lo = res_h16_lo;
+    if (res_up_W > 0) {
+        VD3D_REQUIRE(res && !res_h16_hi && p.Ho == 2 * res_up_H && p.Wo == 2 * res_up_W,
+                     "conv2d_tc: an upsampled residual is an fp32 tensor of exactly half the output size (%dx%d vs %dx%d)", res_up_H, res_up_W, p.Ho, p.Wo);
+        p.res_up_H = res_up_H; p.res_up_W = res_up_W;
+    }
     p.two_pass = two_pass;
     p.range_flag = out_h16_hi ? fp16_range_flag() : nullptr;
     {
@@ -655,7 +703,54 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     if ((rc = make_map_act(&mAlo, in_lo ? in_lo : in, B, H, W, Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
     if ((rc = make_map_wgt(&mWhi, w_hi, Cout, K, BN, esize))) return rc;
     if ((rc = make_map_wgt(&mWlo, w_lo ? w_lo : w_hi, Cout, K, BN, esize))) return rc;
-    return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
+    if (!ls) return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
+    TcLevelMaps lm;
+    for (int l = 0; l < ls->L; ++l) {
+        if ((rc = make_map_act(&lm.a[l], ls->in_hi[l], B, ls->H[l], ls->W[l], Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
+        if ((rc = make_map_act(&lm.alo[l], ls->in_lo[l], B, ls->H[l], ls->W[l], Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
+    }
+    return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream, &lm);
+}
+
+// pixel offset of level l's tensor relative to level 0's, from the two base pointers (bytes / (esize * cs)); -1 LL << 62 if not a whole pixel
+static long long level_pix_off(const void* base0, const void* base, int esize, int cs) {
+    const long long d = (long long)((const char*)base - (const char*)base0);
+    return d % ((long long)esize * cs) ? (-1LL << 62) : d / ((long long)esize * cs);
+}
+
+extern "C" int vd3d_conv2d_tc16_levels(int L, const void* const* in_hi, const void* const* in_lo, const int* H, const int* W, int B, int Cin, int in_cs,
+                                       int in_co, const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad,
+                                       int dil, int stride, const void* const* res, const int* res_H, const int* res_W, int res_cs, int res_co,
+                                       const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
+                                       int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
+    VD3D_REQUIRE(L >= 1 && L <= TC_MAX_LEVELS && in_hi && in_lo && H && W && (out || out_hi16) && (!out_hi16 == !out_lo16),
+                 "conv2d_tc16_levels: 1..%d levels, inputs, sizes and an output are required", TC_MAX_LEVELS);
+    LevelSpec ls;
+    memset(&ls, 0, sizeof(ls));
+    ls.L = L;
+    for (int l = 0; l < L; ++l) {
+        VD3D_REQUIRE(in_hi[l] && in_lo[l] && H[l] > 0 && W[l] > 0 && ((((uintptr_t)in_hi[l] | (uintptr_t)in_lo[l]) & 15) == 0),
+                     "conv2d_tc16_levels: level %d: 16-byte aligned input planes and a non-empty size are required", l);
+        ls.in_hi[l] = in_hi[l]; ls.in_lo[l] = in_lo[l]; ls.H[l] = H[l]; ls.W[l] = W[l];
+        ls.res_H[l] = res_H ? res_H[l] : 0; ls.res_W[l] = res_W ? res_W[l] : 0;
+        // every output form of level l sits at the same pixel offset from level 0's (one allocation per form, levels concatenated)
+        const long long o32 = out ? level_pix_off(out[0], out[l], 4, out_cs) : 0;
+        const long long oh = out_hi16 ? level_pix_off(out_hi16[0], out_hi16[l], 2, out_cs) : o32;
+        const long long ol = out_lo16 ? level_pix_off(out_lo16[0], out_lo16[l], 2, out_cs) : o32;
+        VD3D_REQUIRE(o32 == oh && oh == ol && (out ? out[l] != nullptr : true) && o32 > (-1LL << 62),
+                     "conv2d_tc16_levels: level %d: the output forms must lie at one common pixel offset from level 0's", l);
+        ls.out_off[l] = out ? o32 : oh;
+        ls.res_off[l] = 0;
+        if (res) {
+            VD3D_REQUIRE(res[l], "conv2d_tc16_levels: level %d has no residual", l);
+            ls.res_off[l] = level_pix_off(res[0], res[l], 4, res_cs);
+            VD3D_REQUIRE(ls.res_off[l] > (-1LL << 62), "conv2d_tc16_levels: level %d: residual not at a whole-pixel offset from level 0's", l);
+        }
+    }
+    return conv2d_tc_launch(1, in_hi[0], in_lo[0], B, H[0], W[0], Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride,
+                            res ? (const float*)res[0] : nullptr, res_cs, res_co, out ? (float*)out[0] : nullptr, nullptr,
+                            out_hi16 ? (void*)out_hi16[0] : nullptr, out_lo16 ? (void*)out_lo16[0] : nullptr, Cout, out_cs, out_co, relu, 3, bn, stream,
+                            nullptr, nullptr, 0, 0, &ls);
 }
 
 extern "C" int vd3d_conv2d_tc(const float* in, const float* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
@@ -681,6 +776,17 @@ extern "C" int vd3d_conv2d_tc16_planes(const void* in_hi, const void* in_lo, int
                                        float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
     return conv2d_tc_launch(1, in_hi, in_lo, B, H, W, Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride, res, res_cs, res_co,
                             out, nullptr, out_hi16, out_lo16, Cout, out_cs, out_co, relu, 3, bn, stream, res_hi16, res_lo16);
+}
+
+// FPN lateral conv with the top-down add fused (R/detectors/retinanet_2d.py:49-52): out = conv(in) + nearest_up2(res), the residual being
+// [B][Ho / 2][Wo / 2] (res_H, res_W); everything else as vd3d_conv2d_tc16 (3 passes, library tile policy when bn <= 0)
+extern "C" int vd3d_conv2d_tc16_res_up2(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                                        const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
+                                        int stride, const float* res, int res_cs, int res_co, int res_H, int res_W,
+                                        float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
+    VD3D_REQUIRE(res && res_H > 0 && res_W > 0, "conv2d_tc16_res_up2: needs the half-resolution residual");
+    return conv2d_tc_launch(1, in_hi, in_lo, B, H, W, Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride, res, res_cs, res_co,
+                            out, nullptr, out_hi16, out_lo16, Cout, out_cs, out_co, relu, 3, bn, stream, nullptr, nullptr, res_H, res_W);
 }
 
 // ----------------------------------------------------------------------------------------------------------------

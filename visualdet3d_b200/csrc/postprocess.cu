@@ -7,6 +7,7 @@
 // FMA contraction disabled (explicit __fmul_rn/__fadd_rn/__fdiv_rn), so they only differ where the CUDA libm
 // (expf/atan2f) differs from the host libm by an ulp on a knife edge.
 #include "common.cuh"
+#include <cstring>
 
 namespace vd3d {
 
@@ -227,6 +228,164 @@ __global__ void __launch_bounds__(NMS_THREADS) sort_nms_kernel(DecodeWs ws, int 
     if (t == 0) out_count[b] = nkeep;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// RetinaNet 2-D decode (RetinanetHead.get_bboxes, R/heads/retinanet_head.py:257-307), batched, no host sync:
+//   (1) retina_score_kernel: per anchor, max over classes of sigmoid(cls) (first maximum wins) -> 32-bit key ~bits(score) (ascending =
+//       better) and the label;
+//   (2) retina_select_kernel (one CTA per image): the k = min(nms_pre, N) smallest keys by an 8-bit radix select (4 histogram passes),
+//       ties at the k-th key resolved by anchor index (ascending, an ordered block scan), then the _decode of the selected rows (:227-255,
+//       no ClipBoxes) into the sort_nms_kernel workspace with box columns 4..10 zero;
+//   (3) sort_nms_kernel: sort by (score desc, index asc) + greedy class-agnostic NMS;
+//   (4) retina_thresh_kernel: the post-NMS score threshold, a prefix of the score-ordered kept rows, as a count.
+// Head outputs are per pyramid level (NHWC [B][pix_l][cs]): anchor n of level l at local index j = n - off_l is pixel j / A, channel
+// (j % A) * C + c.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int RETINA_MAX_LEVELS = 8;
+struct RetinaLevels {
+    const float* cls[RETINA_MAX_LEVELS];
+    const float* reg[RETINA_MAX_LEVELS];
+    int pix[RETINA_MAX_LEVELS];
+    int off[RETINA_MAX_LEVELS + 1];          // first anchor of level l (off[L] = N)
+    int L, A, cls_cs, reg_cs;
+};
+
+__device__ __forceinline__ long long retina_elem(const RetinaLevels& lv, int b, int n, int cs, int per, int& l_out) {
+    int l = 0;
+    while (l + 1 < lv.L && n >= lv.off[l + 1]) ++l;
+    const int j = n - lv.off[l];
+    const int px = j / lv.A, a = j - px * lv.A;
+    l_out = l;
+    return ((long long)b * lv.pix[l] + px) * cs + (long long)a * per;
+}
+
+__global__ void retina_score_kernel(RetinaLevels lv, int B, int N, int ncls, unsigned int* __restrict__ keys, uint8_t* __restrict__ labels) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)B * N) return;
+    const int n = (int)(idx % N), b = (int)(idx / N);
+    int l;
+    const long long e = retina_elem(lv, b, n, lv.cls_cs, ncls, l);
+    const float* cp = lv.cls[l] + e;
+    float best = -1.f; int label = 0;
+    for (int c = 0; c < ncls; ++c) {
+        const float p = sigmoidf_ref(__ldg(cp + c));
+        if (p > best) { best = p; label = c; }
+    }
+    keys[idx] = ~__float_as_uint(best);                 // sigmoid >= +0: the bit pattern is monotone
+    labels[idx] = (uint8_t)label;
+}
+
+constexpr int SEL_THREADS = 1024;
+
+// exclusive prefix of `flag` over the block (thread order) and the block total
+__device__ __forceinline__ int block_excl_scan(bool flag, int* s_warp, int& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned int bal = __ballot_sync(0xffffffffu, flag);
+    const int in_warp = __popc(bal & ((1u << lane) - 1u));
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    if (warp == 0) {
+        const int v = s_warp[lane];
+        int x = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+        s_warp[32 + lane] = x - v;
+        if (lane == 31) s_warp[64] = x;
+    }
+    __syncthreads();
+    const int r = s_warp[32 + warp] + in_warp;
+    total = s_warp[64];
+    __syncthreads();
+    return r;
+}
+
+__global__ void __launch_bounds__(SEL_THREADS) retina_select_kernel(RetinaLevels lv, const unsigned int* __restrict__ keys, const uint8_t* __restrict__ labels,
+                                                                    const float* __restrict__ anchors, int N, int k, float4 mean, float4 std, int cap, DecodeWs ws) {
+    __shared__ int hist[256];
+    __shared__ int s_warp[65];
+    __shared__ unsigned int s_prefix;
+    __shared__ int s_need;
+    const int b = blockIdx.x, t = threadIdx.x;
+    const unsigned int* kp = keys + (long long)b * N;
+    // ---- radix select: T = the k-th smallest key, `need` = how many keys equal to T are taken ----
+    unsigned int T = 0xffffffffu;
+    int need = 0;
+    if (k < N) {
+        if (t == 0) { s_prefix = 0; s_need = k; }
+        __syncthreads();
+        for (int shift = 24; shift >= 0; shift -= 8) {
+            for (int i = t; i < 256; i += SEL_THREADS) hist[i] = 0;
+            __syncthreads();
+            const unsigned int prefix = s_prefix;
+            const unsigned int hmask = shift == 24 ? 0u : (0xffffffffu << (shift + 8));
+            for (int i = t; i < N; i += SEL_THREADS) {
+                const unsigned int key = __ldg(kp + i);
+                if ((key & hmask) == prefix) atomicAdd(&hist[(key >> shift) & 255], 1);
+            }
+            __syncthreads();
+            if (t == 0) {
+                int rem = s_need, d = 0;
+                while (hist[d] < rem) { rem -= hist[d]; ++d; }
+                s_prefix = prefix | ((unsigned int)d << shift);
+                s_need = rem;
+            }
+            __syncthreads();
+        }
+        T = s_prefix;
+        need = s_need;
+    }
+    // ---- ordered compaction: every key < T, and the first `need` keys == T in anchor order; decode into the NMS workspace ----
+    int taken_ties = 0, slot0 = 0;
+    for (int base = 0; base < N; base += SEL_THREADS) {
+        const int n = base + t;
+        const unsigned int key = n < N ? __ldg(kp + n) : 0xffffffffu;
+        const bool tie = n < N && k < N && key == T;
+        int ntie;
+        const int tie_rank = block_excl_scan(tie, s_warp, ntie);
+        const bool sel = n < N && (k >= N || key < T || (tie && taken_ties + tie_rank < need));
+        int nsel;
+        const int pos = slot0 + block_excl_scan(sel, s_warp, nsel);
+        taken_ties += ntie;
+        slot0 += nsel;
+        if (!sel || pos >= cap) continue;
+        int l;
+        const float* rp = lv.reg[0];
+        {
+            const long long e = retina_elem(lv, b, n, lv.reg_cs, 4, l);
+            rp = lv.reg[l] + e;
+        }
+        const float4 a = ldg4(anchors + 4 * (long long)n);
+        const float dx = add(mul(__ldg(rp + 0), std.x), mean.x), dy = add(mul(__ldg(rp + 1), std.y), mean.y);
+        const float dw = add(mul(__ldg(rp + 2), std.z), mean.z), dh = add(mul(__ldg(rp + 3), std.w), mean.w);
+        const float px = mul(add(a.x, a.z), 0.5f), py = mul(add(a.y, a.w), 0.5f);
+        const float pw = sub(a.z, a.x), ph = sub(a.w, a.y);
+        const float gw = mul(pw, expf(dw)), gh = mul(ph, expf(dh));
+        const float gx = add(px, mul(pw, dx)), gy = add(py, mul(ph, dy));
+        const long long o = (long long)b * cap + pos;
+        ws.keys[o] = ((unsigned long long)key << 32) | (unsigned int)n;
+        float* bp = ws.boxes + o * 11;
+        bp[0] = sub(gx, mul(gw, 0.5f)); bp[1] = sub(gy, mul(gh, 0.5f)); bp[2] = add(gx, mul(gw, 0.5f)); bp[3] = add(gy, mul(gh, 0.5f));
+#pragma unroll
+        for (int q = 4; q < 11; ++q) bp[q] = 0.f;
+        ws.labels[o] = (int)labels[(long long)b * N + n];
+    }
+    if (t == 0) ws.ncand[b] = slot0;
+}
+
+// post-NMS `max_score > score_thr` (retinanet_head.py:295-304): the kept rows are in descending score order, so the survivors are a prefix
+__global__ void retina_thresh_kernel(const float* __restrict__ scores, int cap, float score_thr, int32_t* __restrict__ count) {
+    __shared__ int s_n;
+    const int b = blockIdx.x;
+    const int n = count[b];
+    if (n < 0) return;
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    int c = 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) c += scores[(long long)b * cap + i] > score_thr;
+    atomicAdd(&s_n, c);
+    __syncthreads();
+    if (threadIdx.x == 0) count[b] = s_n;
+}
+
 // fixed-capacity detection record block for the multi-GPU all-gather: rec[b] = [count | kmax x (11 box floats, score, class)]
 __global__ void pack_records_kernel(const float* __restrict__ scores, const float* __restrict__ boxes, const int64_t* __restrict__ cls,
                                     const int32_t* __restrict__ count, int cap, int kmax, float* __restrict__ rec, const int* __restrict__ range_flag) {
@@ -298,5 +457,58 @@ extern "C" int vd3d_decode_nms(const float* cls, const float* reg, const float* 
     VD3D_CUDA(cudaFuncSetAttribute(sort_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     sort_nms_kernel<<<B, NMS_THREADS, smem, st>>>(ws, cap, cp2, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand);
     VD3D_CHECK_LAUNCH("sort_nms");
+    return VD3D_OK;
+}
+
+extern "C" long long vd3d_retina_decode_workspace(int B, int N, int cap) {
+    // the vd3d_decode_nms workspace, then keys u32 [B][N] and labels u8 [B][N]
+    const long long nms = vd3d_decode_nms_workspace(B, cap);
+    return nms + ((long long)B * N * 4 + 15) / 16 * 16 + (long long)B * N + 64;
+}
+
+extern "C" int vd3d_retina_decode(int L, const void* const* cls_levels, const void* const* reg_levels, const int* level_pix, int cls_cs, int reg_cs,
+                                  const float* anchors, int B, int N, int A, int ncls, int nms_pre, const float* means4, const float* stds4,
+                                  float score_thr, double iou_thr, int cap, void* wsp,
+                                  float* out_scores, float* out_boxes, int64_t* out_cls, int32_t* out_anchor,
+                                  int32_t* out_count, int32_t* out_ncand, void* stream) {
+    VD3D_REQUIRE(cls_levels && reg_levels && level_pix && anchors && means4 && stds4 && wsp && out_scores && out_boxes && out_cls && out_anchor &&
+                 out_count && out_ncand, "retina_decode: null pointer");
+    VD3D_REQUIRE(L >= 1 && L <= RETINA_MAX_LEVELS && B > 0 && N > 0 && A > 0 && ncls > 0 && ncls <= 255 && cls_cs >= A * ncls && reg_cs >= A * 4,
+                 "retina_decode: bad shape (L=%d A=%d ncls=%d cls_cs=%d reg_cs=%d)", L, A, ncls, cls_cs, reg_cs);
+    const int k = (nms_pre > 0 && N > nms_pre) ? nms_pre : N;
+    VD3D_REQUIRE(cap > 0 && cap <= 4096 && k <= cap, "retina_decode: %d candidates exceed the NMS capacity %d (<= 4096)", k, cap);
+    RetinaLevels lv;
+    memset(&lv, 0, sizeof(lv));
+    lv.L = L; lv.A = A; lv.cls_cs = cls_cs; lv.reg_cs = reg_cs;
+    lv.off[0] = 0;
+    for (int l = 0; l < L; ++l) {
+        VD3D_REQUIRE(cls_levels[l] && reg_levels[l] && level_pix[l] > 0, "retina_decode: level %d is empty", l);
+        lv.cls[l] = (const float*)cls_levels[l]; lv.reg[l] = (const float*)reg_levels[l]; lv.pix[l] = level_pix[l];
+        lv.off[l + 1] = lv.off[l] + level_pix[l] * A;
+    }
+    VD3D_REQUIRE(lv.off[L] == N, "retina_decode: the levels hold %d anchors, N = %d", lv.off[L], N);
+    cudaStream_t st = (cudaStream_t)stream;
+    DecodeWs ws;
+    unsigned char* p = (unsigned char*)wsp;
+    ws.keys = (unsigned long long*)p; p += (long long)B * cap * 8;
+    ws.boxes = (float*)p; p += (long long)B * cap * 44;
+    ws.labels = (int*)p; p += (long long)B * cap * 4;
+    ws.ncand = (int*)p;
+    unsigned char* q = (unsigned char*)wsp + vd3d_decode_nms_workspace(B, cap);
+    unsigned int* keys = (unsigned int*)q;
+    uint8_t* labels = q + ((long long)B * N * 4 + 15) / 16 * 16;
+    retina_score_kernel<<<cdiv((long long)B * N, 256), 256, 0, st>>>(lv, B, N, ncls, keys, labels);
+    VD3D_CHECK_LAUNCH("retina_score");
+    retina_select_kernel<<<B, SEL_THREADS, 0, st>>>(lv, keys, labels, anchors, N, k, make_float4(means4[0], means4[1], means4[2], means4[3]),
+                                                    make_float4(stds4[0], stds4[1], stds4[2], stds4[3]), cap, ws);
+    VD3D_CHECK_LAUNCH("retina_select");
+    int cp2 = next_pow2(cap);
+    if (cp2 < 64) cp2 = 64;
+    const size_t smem = (size_t)cp2 * (8 + 8 + 16 + 4 + 4 + 4) + 16;
+    VD3D_CUDA(cudaFuncSetAttribute(sort_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sort_nms_kernel<<<B, NMS_THREADS, smem, st>>>(ws, cap, cp2, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand);
+    VD3D_CHECK_LAUNCH("sort_nms");
+    retina_thresh_kernel<<<B, 256, 0, st>>>(out_scores, cap, score_thr, out_count);
+    VD3D_CHECK_LAUNCH("retina_thresh");
     return VD3D_OK;
 }

@@ -14,6 +14,12 @@ constexpr int TC_MAX_BN = 128;                // widest tile: the chunk accumula
 // promotes the chunks and runs the epilogue), the warps after them produce the operands.
 constexpr int TC_CONSUMERS = 256;
 
+constexpr int TC_MAX_LEVELS = 5;
+struct TcLevel {
+    int Ho, Wo, tiles_w, tiles_h, m_begin, res_H, res_W;
+    long long pix_off, res_off;
+};
+
 struct TcParams {
     int B, H, W, Cin, KH, KW, pad, dil, stride;
     int Ho, Wo, Cout, BN, stages, passes, chunk;
@@ -43,6 +49,12 @@ struct TcParams {
     int out_cs, out_co, res_cs, res_co, relu;
     const float* bias; const float* res; float* out; float* out_lo;
     const void* res_h16_hi; const void* res_h16_lo;   // residual given as fp16 (hi, lo) planes (value = hi + lo) instead of an fp32 tensor (`res`)
+    int res_up_H, res_up_W;  // > 0: the residual is [B][res_up_H][res_up_W] at half the output resolution, read nearest-upsampled (tcp_res_pix)
+    // Multi-level launch (vd3d_conv2d_tc16_levels; n_levels = 0: one tensor).  The M tiles of the levels are concatenated: level l owns tiles
+    // [m_begin, m_begin + B * tiles_h * tiles_w) and reads its own activation maps; its output (residual) pixel p sits at pixel pix_off + p
+    // (res_off + p, or of the [B][res_H][res_W] half-resolution residual when res_W > 0) of the `out` (`res`) pointers.
+    int n_levels;
+    TcLevel lv[TC_MAX_LEVELS];
 };
 
 // 8 consecutive channels (16-byte aligned)
@@ -182,6 +194,36 @@ template <int V> using tc_int = std::integral_constant<int, V>;
 // Epilogue arithmetic of the persistent kernels, per 8 output channels n .. n + 7 of one output pixel `pix` (n + 4 <= Cout; when n + 8 > Cout,
 // the Cout % 8 == 4 tail, only the first four are read and written).  Split in two so that an epilogue can have the residual loads of
 // several groups in flight before it computes the first.
+// Output geometry of M tile mu: tile column / row, image, the output size, and the pixel offsets of the output and the residual (the level's,
+// in a multi-level launch; zero otherwise).  The level table is indexed with compile-time indices only, so it stays in parameter space.
+struct TcGeom { int tw, th, b, Ho, Wo, lvl, res_H, res_W; long long pix_off, res_off; };
+__device__ __forceinline__ TcGeom tile_geom(const TcParams& p, int mu) {
+    TcGeom g;
+    g.lvl = 0; g.Ho = p.Ho; g.Wo = p.Wo; g.res_H = p.res_up_H; g.res_W = p.res_up_W; g.pix_off = 0; g.res_off = 0;
+    int tiles_w = p.tiles_w, tiles_h = p.tiles_h;
+    if (p.n_levels > 0) {
+#pragma unroll
+        for (int i = 0; i < TC_MAX_LEVELS; ++i)
+            if (i < p.n_levels && mu >= p.lv[i].m_begin) {
+                g.lvl = i; g.Ho = p.lv[i].Ho; g.Wo = p.lv[i].Wo; g.res_H = p.lv[i].res_H; g.res_W = p.lv[i].res_W;
+                g.pix_off = p.lv[i].pix_off; g.res_off = p.lv[i].res_off; tiles_w = p.lv[i].tiles_w; tiles_h = p.lv[i].tiles_h;
+            }
+#pragma unroll
+        for (int i = 0; i < TC_MAX_LEVELS; ++i)
+            if (i == g.lvl) mu -= p.lv[i].m_begin;
+    }
+    g.tw = mu % tiles_w; mu /= tiles_w;
+    g.th = mu % tiles_h; g.b = mu / tiles_h;
+    return g;
+}
+// Output pixel of (b, ho, wo), and its residual pixel: the same pixel, or (res_W > 0) pixel (ho >> 1, wo >> 1) of the half-resolution
+// residual, i.e. the nearest-neighbour x2 upsampling of the FPN top-down path fused into the residual read.
+__device__ __forceinline__ long long tcp_out_pix(const TcGeom& g, int ho, int wo) {
+    return g.pix_off + ((long long)g.b * g.Ho + ho) * g.Wo + wo;
+}
+__device__ __forceinline__ long long tcp_res_pix(const TcGeom& g, int ho, int wo) {
+    return g.res_off + (g.res_W > 0 ? ((long long)g.b * g.res_H + (ho >> 1)) * g.res_W + (wo >> 1) : ((long long)g.b * g.Ho + ho) * g.Wo + wo);
+}
 // (1) the residual (zeros without one)
 __device__ __forceinline__ void tcp_epi_res(const TcParams& p, long long pix, int n, float (&rr)[8]) {
 #pragma unroll
@@ -271,14 +313,13 @@ __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* 
     int mu, nt;
     unit_tile(p, u, mt_units, mu, nt);
     const int ncols = min(HALF, min(p.BN, p.cout_pad - nt * p.BN) - cb);      // valid columns of this thread in this tile (<= 0: none)
-    int mt = mu;
-    const int tw = mt % p.tiles_w; mt /= p.tiles_w;
-    const int th = mt % p.tiles_h; const int b = mt / p.tiles_h;
+    const TcGeom g = tile_geom(p, mu);
     const int r = q * 32 + lane;
-    const int ho = th * TC_TH + r / TC_TW, wo = tw * TC_TW + r % TC_TW;
+    const int ho = g.th * TC_TH + r / TC_TW, wo = g.tw * TC_TW + r % TC_TW;
     float amax = 0.f;
-    if (!(ho < p.Ho && wo < p.Wo) || ncols <= 0 || (p.dbg & 16)) return amax;
-    const long long pix = ((long long)b * p.Ho + ho) * p.Wo + wo;
+    if (!(ho < g.Ho && wo < g.Wo) || ncols <= 0 || (p.dbg & 16)) return amax;
+    const long long pix = tcp_out_pix(g, ho, wo);
+    const long long rpix = tcp_res_pix(g, ho, wo);
     const float* acc = tile + r * ld;
     int sw = r & swz;
     if (swz) asm volatile("" : "+r"(sw));                           // (as in wg_stage)
@@ -288,7 +329,7 @@ __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* 
         const int n = nbase + col;
         if (col < ncols && n + 4 <= p.Cout) {
             float rr[8];
-            tcp_epi_res(p, pix, n, rr);
+            tcp_epi_res(p, rpix, n, rr);
             const int j = (cb + col) >> 2;                       // 16-byte chunk of the staged row
             const float4 a0 = *reinterpret_cast<const float4*>(acc + ((j ^ sw) << 2)), a1 = *reinterpret_cast<const float4*>(acc + (((j + 1) ^ sw) << 2));
             amax = fmaxf(amax, tcp_epi_out(p, pix, n, a0, a1, rr));

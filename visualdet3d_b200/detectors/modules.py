@@ -275,3 +275,48 @@ class YoloMono3DCoreP(Holder):
     def __init__(self, backbone_arguments):
         super().__init__()
         self.backbone = ResNetP(**backbone_arguments)
+
+
+class FPNP(Holder):
+    """keys of FPN (R/detectors/retinanet_2d.py:15-40): lateral_convs.i (1x1, bias), fpn_convs.i (3x3, bias; the extra levels stride 2)."""
+
+    def __init__(self, in_channels, out_channels, num_outs):
+        super().__init__()
+        self.in_channels, self.out_channels, self.num_outs = list(in_channels), int(out_channels), int(num_outs)
+        self.lateral_convs = nn.ModuleList([nn.Conv2d(c, out_channels, 1) for c in in_channels])
+        self.fpn_convs = nn.ModuleList([nn.Conv2d(out_channels, out_channels, 3, padding=1) for _ in in_channels])
+        for i in range(num_outs - len(in_channels)):
+            self.fpn_convs.append(nn.Conv2d(in_channels[-1] if i == 0 else out_channels, out_channels, 3, padding=1, stride=2))
+
+
+class RetinaNetCoreP(Holder):
+    """keys of RetinaNetCore (R/detectors/retinanet_2d.py:69-73)."""
+
+    def __init__(self, backbone_cfg, neck_cfg):
+        super().__init__()
+        self.backbone = ResNetP(**backbone_cfg)
+        self.neck = FPNP(**neck_cfg)
+
+
+class ConvReLUP(Holder):
+    """keys of ConvReLU (R/lib/blocks.py:46-60): `sequence.0` conv with bias, `sequence.1` ReLU."""
+
+    def __init__(self, cin, cout, k=3):
+        super().__init__()
+        self.sequence = seq(nn.Conv2d(cin, cout, k, 1, (k - 1) // 2), nn.ReLU())
+
+
+class RetinaHeadP(Holder):
+    """keys of RetinanetHead (R/heads/retinanet_head.py:13-80): cls_conv / reg_conv towers, retina_cls / retina_reg (AnchorFlatten has no
+    parameters), the focal-loss balance_weights buffers."""
+
+    def __init__(self, num_anchors, stacked_convs=4, in_channels=256, feat_channels=256, num_classes=3, reg_output=4, loss_cfg=None):
+        super().__init__()
+        cins = [in_channels] + [feat_channels] * (stacked_convs - 1) if stacked_convs > 0 else []
+        self.cls_conv = seq(*[ConvReLUP(c, feat_channels) for c in cins])
+        self.reg_conv = seq(*[ConvReLUP(c, feat_channels) for c in cins])
+        self.retina_cls = seq(nn.Conv2d(feat_channels, num_anchors * num_classes, 3, padding=1))
+        self.retina_reg = seq(nn.Conv2d(feat_channels, num_anchors * reg_output, 3, padding=1))
+        bw = torch.tensor((loss_cfg or {}).get("balance_weights", 0), dtype=torch.float32)
+        self.register_buffer("balance_weights", bw)
+        self.loss_cls = LossClsP(bw)

@@ -6,6 +6,7 @@ is how every torch.cat of the reference is fused away (producers write straight 
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Dict, Optional, Sequence, Tuple
 
 import numpy as np
@@ -132,6 +133,20 @@ class Arena:
             return Act(t, 0, None, self.get(name + "#h16", (2,) + tuple(shape), device, dtype=torch.float16, zero=True))
         return Act(t, 0, None, self.get(name + "#lo", shape, device, zero=True))
 
+    def level_acts(self, name: str, B: int, hws: Sequence[Tuple[int, int]], C: int, device, lo: bool = False) -> list:
+        """One NHWC activation per (H, W) in `hws`, as views of ONE allocation per form with the levels concatenated ([B, H, W, C] blocks in
+        order; the fp16 planes likewise): the layout `ConvLayer.run_levels` writes and reads."""
+        sizes = [B * h * w * C for h, w in hws]
+        t = self.get(name, (sum(sizes),), device)
+        p = self.get(name + "#h16", (2, sum(sizes)), device, dtype=torch.float16, zero=True) if lo and self.lo_form == "h16" else None
+        if lo and p is None:
+            raise _lib.Vd3dError("Arena.level_acts: the concatenated form needs the fp16 (hi, lo) planes (engine tc16)")
+        out, o = [], 0
+        for (h, w), n in zip(hws, sizes):
+            out.append(Act(t[o:o + n].view(B, h, w, C), 0, None, p[:, o:o + n].view(2, B, h, w, C) if p is not None else None))
+            o += n
+        return out
+
     def nbytes(self) -> int:
         return sum(t.numel() * t.element_size() for t in self._bufs.values())
 
@@ -236,15 +251,65 @@ class ConvLayer:
         Wo = (W + 2 * self.pad - self.dil * (self.KW - 1) - 1) // self.stride + 1
         return Ho, Wo
 
-    def __call__(self, x: Act, out: Act, res: Optional[Act] = None, relu: Optional[bool] = None, f32_out: bool = True):
+    def _check_tc16_input(self, x: Act, what: str):
+        if self.engine != "tc16" or getattr(self, "passes", 3) != 3:
+            raise _lib.Vd3dError(f"{what}: only the fp16-split tensor-core engine (VD3D_CONV_ENGINE=tc16) runs it")
+        if not x.h16:
+            raise _lib.Vd3dError(f"{what}: input activation has no fp16 (hi, lo) planes (plan bug: missing split_lo)")
+        if CHECK_LO:
+            check_lo(x)
+
+    def run_levels(self, xs: Sequence[Act], outs: Sequence[Act], res: Optional[Sequence[Act]] = None, res_up: bool = False):
+        """The conv on several tensors of different sizes in ONE persistent launch (vd3d_conv2d_tc16_levels): outs[l] = conv(xs[l]) [+ res[l],
+        nearest-upsampled when res_up].  Each form of `outs` (fp32, fp16 planes) and `res` must be views of one allocation with the levels
+        concatenated (`Arena.level_acts`).  Bit-identical to calling the layer on every level."""
+        L = len(xs)
+        assert 1 <= L == len(outs) and (res is None or len(res) == L)
+        for x, o in zip(xs, outs):
+            self._check_tc16_input(x, "multi-level conv")
+            assert x.C == self.Cin and o.C == self.Cout and o.B == x.B and (o.H, o.W) == self.out_hw(x.H, x.W) and o.h16 == outs[0].h16
+            assert (x.cs, x.co, o.cs, o.co) == (xs[0].cs, xs[0].co, outs[0].cs, outs[0].co)
+        if res is not None:
+            for r in res:
+                need_f32(r, "multi-level conv residual")
+        arr = lambda T, vals: (T * L)(*vals)
+        P = ctypes.c_void_p
+        call("vd3d_conv2d_tc16_levels", L, arr(P, [x.h16_ptrs[0] for x in xs]), arr(P, [x.h16_ptrs[1] for x in xs]),
+             arr(ctypes.c_int, [x.H for x in xs]), arr(ctypes.c_int, [x.W for x in xs]), xs[0].B, self.Cin, xs[0].cs, xs[0].co,
+             self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale, self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride,
+             arr(P, [r.ptr for r in res]) if res is not None else None,
+             arr(ctypes.c_int, [r.H if res_up else 0 for r in res]) if res is not None else None,
+             arr(ctypes.c_int, [r.W if res_up else 0 for r in res]) if res is not None else None,
+             res[0].cs if res is not None else 0, res[0].co if res is not None else 0,
+             arr(P, [o.ptr for o in outs]), arr(P, [o.h16_ptrs[0] for o in outs]) if outs[0].h16 else None,
+             arr(P, [o.h16_ptrs[1] for o in outs]) if outs[0].h16 else None,
+             self.Cout, outs[0].cs, outs[0].co, 1 if self.relu else 0, self.bn_tile, _stream())
+        for o in outs:
+            o.f32, o.lo_fresh = True, o.h16
+        return outs
+
+    def __call__(self, x: Act, out: Act, res: Optional[Act] = None, relu: Optional[bool] = None, f32_out: bool = True, res_up: bool = False):
         """f32_out=False (fp16-split engine only): write ONLY the fp16 (hi, lo) planes of the output; legal when every consumer is a
         tensor-core conv, a plane residual or the tensor-core PSMCosine kernel.  A residual whose fp32 tensor is not valid is read
-        from its planes."""
+        from its planes.  res_up=True (fp16-split engine, fp32 residual): `res` has half the output size and is added nearest-upsampled
+        (the FPN top-down add)."""
         assert x.C == self.Cin, (x.C, self.Cin)
         assert out.C == self.Cout and out.B == x.B
         Ho, Wo = self.out_hw(x.H, x.W)
         assert (out.H, out.W) == (Ho, Wo), ((out.H, out.W), (Ho, Wo))
         r = self.relu if relu is None else relu
+        if res_up:
+            self._check_tc16_input(x, "conv with an upsampled residual")
+            if not out.h16 or res is None:
+                raise _lib.Vd3dError("conv with an upsampled residual: needs a residual and an output with fp16 (hi, lo) planes")
+            need_f32(res, "upsampled conv residual")
+            xh, xl = x.h16_ptrs
+            oh, ol = out.h16_ptrs
+            call("vd3d_conv2d_tc16_res_up2", xh, xl, x.B, x.H, x.W, x.C, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale,
+                 self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride, res.ptr, res.cs, res.co, res.H, res.W,
+                 out.ptr, oh, ol, self.Cout, out.cs, out.co, 1 if r else 0, self.bn_tile, _stream())
+            out.f32, out.lo_fresh = True, True
+            return out
         if self.engine != "tc16" or not out.h16 or getattr(self, "passes", 3) != 3:
             f32_out = True
         out.f32 = f32_out

@@ -67,12 +67,18 @@ DATASET_DICT, BACKBONE_DICT, DETECTOR_DICT = Registry("datasets"), Registry("bac
 PIPELINE_DICT, AUGMENTATION_DICT, SAMPLER_DICT = Registry("pipelines"), Registry("augmentation"), Registry("sampler")
 
 
+# detectors that replace the reference's class only on request (install_retinanet_into_reference)
+OPT_IN_DETECTORS = ("RetinaNet",)
+
+
 def install_into_reference(force: bool = True):
-    """Put every B200 detector / pipeline into the REFERENCE's registries (when `visualDet3D` is importable) so the
-    reference's own scripts/eval.py and scripts/train.py pick them up by `cfg.detector.name` with no edit."""
+    """Put every B200 3-D detector / pipeline into the REFERENCE's registries (when `visualDet3D` is importable) so the
+    reference's own scripts/eval.py and scripts/train.py pick them up by `cfg.detector.name` with no edit.  The 2-D RetinaNet is
+    opt-in: `install_retinanet_into_reference()`."""
     from visualDet3D.networks.utils import registry as ref   # ImportError if the reference is not on sys.path
-    for cls in DETECTOR_DICT.module_dict.values():
-        ref.DETECTOR_DICT._register_module(cls, force=force)
+    for name, cls in DETECTOR_DICT.module_dict.items():
+        if name not in OPT_IN_DETECTORS:
+            ref.DETECTOR_DICT._register_module(cls, force=force)
     for fn in PIPELINE_DICT.module_dict.values():
         ref.PIPELINE_DICT._register_module(fn, force=force)
     return ref
@@ -88,3 +94,12 @@ def install_evaluator_into_reference():
     ref_evaluate.evaluate = evaluate
     ref_evaluators.evaluate = evaluate
     return evaluate
+
+
+def install_retinanet_into_reference():
+    """Make the REFERENCE's `DETECTOR_DICT['RetinaNet']` the native 2-D RetinaNet, so the unmodified scripts/eval.py (test_mono_detection,
+    test_one's 2-D branch) run the RetinaNet config on the GPU path.  Returns the installed class."""
+    from visualDet3D.networks.utils import registry as ref   # ImportError if the reference is not on sys.path
+    from .detectors.retinanet import RetinaNet
+    ref.DETECTOR_DICT._register_module(RetinaNet, force=True)
+    return RetinaNet

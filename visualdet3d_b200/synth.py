@@ -34,6 +34,7 @@ def _gen(key: str, seed: int) -> torch.Generator:
 
 
 CLS_GAIN = {"GroundAwareYolo3D": 3.2}     # final cls conv gain per detector kind (default 1.6): keeps ~1 % of anchors above score_thr
+RETINA_CLS_BIAS = 5.0     # subtracted from the seeded retina_cls bias: tens of boxes above score_thr = 0.2 after NMS at 288x1280
 
 
 def synth_state_dict(shapes: Mapping[str, Sequence[int]], seed: int = 0, gain: float = 0.8, cls_gain: float = 1.6) -> "OrderedDict[str, torch.Tensor]":
@@ -85,6 +86,8 @@ def synth_state_dict(shapes: Mapping[str, Sequence[int]], seed: int = 0, gain: f
                 b = b - 3.3
             elif k.endswith("head_layers.hm.2.bias") or k.endswith("head_layers.hm_hp.2.bias"):   # heat-map prior (km3d_head.py:146-148: -2.19)
                 b = b - 3.5
+            elif k.endswith("retina_cls.0.bias"):                    # RetinaNet cls prior (retinanet_head.py:66-68: log(0.01 / 0.99))
+                b = b - RETINA_CLS_BIAS
             out[k] = b
         elif leaf == "alpha" and shp == (1,):            # LookGround.alpha
             out[k] = torch.full(shp, 0.5)
@@ -258,4 +261,21 @@ def mono3d_cfg(preprocessed_path: str, kind: str = "Yolo3D", obj_types=("Car",),
                           regression_weight=[1, 1, 1, 1, 1, 1, 3, 1, 1, 0.5, 0.5, 0.5, 1]),
         test_cfg=AttrDict(score_thr=0.75, cls_agnostic=False, nms_iou_thr=0.5, post_optimization=False))
     det.anchors = anchors
+    return det
+
+
+def retinanet_cfg(obj_types=("Car", "Pedestrian", "Cyclist"), depth: int = 50, nms_pre: int = 1000) -> AttrDict:
+    """cfg.detector of R/config/RetinaNet_example (with pretrained=False: there is no network for the ImageNet weights)."""
+    obj_types = list(obj_types)
+    det = AttrDict(obj_types=obj_types, name="RetinaNet")
+    det.backbone = AttrDict(depth=depth, pretrained=False, frozen_stages=1, num_stages=4, out_indices=(1, 2, 3), norm_eval=True)
+    c = 4 if depth > 34 else 1
+    det.neck = AttrDict(in_channels=[128 * c, 256 * c, 512 * c], out_channels=256, num_outs=5)
+    anchors = AttrDict(pyramid_levels=[i for i in range(3, 8)], strides=[2 ** i for i in range(3, 8)], sizes=[4 * 2 ** i for i in range(3, 8)],
+                       ratios=np.array([0.5, 1, 2.0]), scales=np.array([2 ** (i / 3.0) for i in range(3)]))
+    det.head = AttrDict(stacked_convs=4, in_channels=256, feat_channels=256, num_classes=len(obj_types),
+                        target_stds=[1.0, 1.0, 1.0, 1.0], target_means=[0.0, 0.0, 0.0, 0.0], anchors_cfg=anchors,
+                        loss_cfg=AttrDict(fg_iou_threshold=0.5, bg_iou_threshold=0.4, min_iou_threshold=0, gamma=2.0, balance_weights=[1],
+                                          pos_weight=-1),
+                        test_cfg=AttrDict(nms_pre=nms_pre, score_thr=0.2, cls_agnostic=False, nms_iou_thr=0.4))
     return det
