@@ -415,6 +415,27 @@ int vd3d_kitti_eval(const double* gt, const double* dt, const long long* offs, i
                     double* overlaps, double* precision, double* orientation, double* thresholds, int* n_thresh,
                     void* workspace, long long workspace_bytes, void* stream);
 
+/* ---- training loss of the 3-D anchor head (AnchorBasedDetection3DHead.loss, R/networks/heads/detection_3d_head.py:402-498) -----------
+ * cls [B][N][C+1] f32 (last column: alpha logit), reg [B][N][12] f32, anchors [N][4] f32 (16-byte aligned), mask [B][N] bool (u8),
+ * mean_std [N][C][6][2] f32, ann [B][M][12] f32 (compound_annotation; class -1 rows are padding, anywhere).  C <= 8, M <= 512.
+ * params (host) [7 + C + 13] f32 = fg_iou_threshold, bg_iou_threshold, min_iou_threshold, focal gamma, then float32 of 1/alpha,
+ *   0.5*alpha and 0.5/alpha of ModifiedSmoothL1Loss, the balance weight of each class, the 13 regression weights.
+ * vd3d_anchor_loss_forward: assign [B][N] i32 = the reference's assigned_gt_inds (1-based among the image's valid rows in their order,
+ *   0 negative, -1 ignored; -1 for every anchor of an image without ground truth, -2 outside the mask); counts [B][3] i32 =
+ *   positives assigned, positives kept by the prior's z_mean > 0, negatives; factors [B][2] f32 (read by the backward);
+ *   cls_loss [1], reg_loss [1] f32.  Four launches, no host synchronisation, no float atomics (bit-reproducible).
+ *   workspace: vd3d_anchor_loss_workspace_bytes(B, N, M) bytes of device memory (a negative return is an error code).
+ * vd3d_anchor_loss_backward: grad_out [2] f32 (device) = d/d cls_loss, d/d reg_loss; writes grad_cls [B][N][C+1] and grad_reg [B][N][12]
+ *   in full (zeros where no term depends on the element), from the forward's assign and factors.  One launch. */
+long long vd3d_anchor_loss_workspace_bytes(int B, int N, int M);
+int vd3d_anchor_loss_forward(const float* cls, const float* reg, const float* anchors, const unsigned char* mask, const float* mean_std,
+                             const float* ann, int B, int N, int C, int M, const float* params, int match_low_quality, int gt_max_assign_all,
+                             void* workspace, long long workspace_bytes, int* assign, int* counts, float* factors, float* cls_loss, float* reg_loss,
+                             void* stream);
+int vd3d_anchor_loss_backward(const float* cls, const float* reg, const float* anchors, const float* mean_std, const float* ann,
+                              int B, int N, int C, int M, const float* params, const int* assign, const float* factors, const float* grad_out,
+                              float* grad_cls, float* grad_reg, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,6 +101,9 @@ _SIGS = {
     "vd3d_kitti_rotate_iou": (I, [P, I, P, I, I, P, P]),
     "vd3d_kitti_eval_workspace_bytes": (c_longlong, [I, c_longlong, c_longlong, c_longlong, I]),
     "vd3d_kitti_eval": (I, [P, P, P, I, c_longlong, c_longlong, c_longlong, c_longlong, P, I, P, I, P, P, P, P, P, P, c_longlong, P]),
+    "vd3d_anchor_loss_workspace_bytes": (c_longlong, [I, I, I]),
+    "vd3d_anchor_loss_forward": (I, [P, P, P, P, P, P, I, I, I, I, P, I, I, P, c_longlong, P, P, P, P, P, P]),
+    "vd3d_anchor_loss_backward": (I, [P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P]),
 }
 
 

@@ -103,3 +103,15 @@ def install_retinanet_into_reference():
     from .detectors.retinanet import RetinaNet
     ref.DETECTOR_DICT._register_module(RetinaNet, force=True)
     return RetinaNet
+
+
+def install_loss_into_reference():
+    """Make the REFERENCE's 3-D anchor head train with the native loss (`anchor_loss.head_loss`): rebinds
+    `AnchorBasedDetection3DHead.loss` in `visualDet3D.networks.heads.detection_3d_head`, which StereoHead (Stereo3D) and GroundAwareHead
+    (Yolo3D, GroundAwareYolo3D) inherit, so the unmodified scripts/train.py computes their head loss on the GPU path.  Each call reads the
+    head's own settings (num_classes, loss_cfg, focal_loss_gamma, balance_weights, regression_weight, loss_bbox.alpha).  Returns the
+    installed function."""
+    from visualDet3D.networks.heads import detection_3d_head as ref_head    # ImportError if the reference is not on sys.path
+    from .anchor_loss import head_loss
+    ref_head.AnchorBasedDetection3DHead.loss = head_loss
+    return head_loss

@@ -149,6 +149,16 @@ def write_priors(dirpath: str, mean: np.ndarray, std: np.ndarray, obj_types: Seq
     return dirpath
 
 
+def synth_head_outputs(B: int, N: int, C: int, seed: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Stand-ins for a 3-D anchor head's outputs, for the loss tests: cls [B, N, C+1] logits on a 1/8 grid over [-6, 2] and
+    reg [B, N, 12] on a 1/16 grid over [-2, 2], float32 from a seeded numpy RandomState (the same values on every machine).  On that
+    grid no focal-loss element lies near the reference's 1e-5 cut, so the cut decides the same way on the host and the device."""
+    rng = np.random.RandomState(seed)
+    cls = rng.randint(-48, 17, size=(B, N, C + 1)).astype(np.float32) / 8
+    reg = rng.randint(-32, 33, size=(B, N, 12)).astype(np.float32) / 16
+    return torch.from_numpy(cls), torch.from_numpy(reg)
+
+
 def synth_P2(B: int, H: int, W: int, seed: int = 1, jitter: float = 0.02) -> Tuple[torch.Tensor, torch.Tensor]:
     """KITTI P2 pushed through CropTop(100) + Resize((H, W)) like stereo_augmentator.py:213-258 does, with a
     per-image +-jitter on fx/fy/cy so the [B, N] useful-mask path is exercised.  P3 = P2 with Tx -= 0.54 fx."""
