@@ -436,6 +436,29 @@ int vd3d_anchor_loss_backward(const float* cls, const float* reg, const float* a
                               int B, int N, int C, int M, const float* params, const int* assign, const float* factors, const float* grad_out,
                               float* grad_cls, float* grad_reg, void* stream);
 
+/* ---- training loss of the MonoFlex head (MonoFlexHead.loss, R/networks/heads/monoflex_head.py:181-236) ------------------------------
+ * Replaces _neg_loss, _RegWeightedL1Loss and _RotLoss (km3d_head.py:61-130, compute_rot_loss rtm3d_utils.py:9-49), _gather_output and
+ * the six gathered terms (monoflex_head.py:26-104, 194-219, decode_depth_from_keypoints rtm3d_utils.py:141-182, IoULoss losses.py:93-120).
+ * maps (host array of 9 device pointers, f32 NCHW): hm [B][C][H][W] logits, bbox2d 4, hps 20, rot 8, dim 3, reg 2, depth 1,
+ *   depth_uncertainty 1, corner_uncertainty 3 channels.
+ * targets (host array of 13 device pointers): hm [B][C][H][W] f32, ind [B][K] i64, reg_mask [B][K] u8, hps [B][K][20] f32,
+ *   hps_mask [B][K][20] u8, dep [B][K] f32, rotbin [B][K][2] i64, rotres [B][K][2] f32, bboxes2d_target [B][K][4] f32, dim [B][K][3] f32,
+ *   reg [B][K][2] f32, kp_detph_mask [B][K][3] f32, P2 [B][3][4] f32.  K <= 128.
+ * unc_lo / unc_hi / unc_w: the head's uncertainty_range and uncertainty_weight.
+ * vd3d_monoflex_loss_forward: terms [9] f32 = hm, hp, box2d, off, dim, depth, kpd, rot, soft_depth (unweighted, as in loss_stats) and
+ *   total [1] f32 = their sum weighted 1, 1, 1, 0.5, 1, 1, 0.2, 1, 0.2.  Three launches, no host synchronisation, no float atomics.
+ *   With no reg_mask row in the batch the six gathered terms are 0.  An ind outside [0, H*W) in any row makes every loss NaN (the map is
+ *   not read there).  workspace: vd3d_monoflex_loss_workspace_bytes(B, C, H, W, K) bytes of device memory (negative: error code); the
+ *   backward reads the factors the forward leaves in it.
+ * vd3d_monoflex_loss_backward: grad_terms [9] and grad_total [1] f32 (device; either may be null = zero) = d/d terms, d/d total; writes
+ *   grads (host array of 9 device pointers, shaped like maps) in full.  One launch. */
+long long vd3d_monoflex_loss_workspace_bytes(int B, int C, int H, int W, int K);
+int vd3d_monoflex_loss_forward(const void* const* maps, const void* const* targets, int B, int C, int H, int W, int K, float unc_lo,
+                               float unc_hi, float unc_w, void* workspace, long long workspace_bytes, float* terms, float* total, void* stream);
+int vd3d_monoflex_loss_backward(const void* const* maps, const void* const* targets, int B, int C, int H, int W, int K, float unc_lo,
+                                float unc_hi, float unc_w, const void* workspace, const float* grad_terms, const float* grad_total,
+                                float* const* grads, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

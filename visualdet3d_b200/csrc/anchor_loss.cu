@@ -15,8 +15,11 @@
 // Compiled with -fmad=false: calc_iou then rounds every product and sum separately, like torch's fp32 elementwise ops, so the
 // IoU -- and with it the assignment -- is bit-identical to the reference's.
 #include "common.cuh"
+#include "loss_common.cuh"
 
 using vd3d::cdiv;
+using vd3d::log_sigmoid;
+using vd3d::sigmoid;
 
 namespace {
 
@@ -130,8 +133,6 @@ __device__ __forceinline__ int assign_anchor(const float* a, int n, int ng, cons
     return r;
 }
 
-__device__ __forceinline__ float log_sigmoid(float x) { return fminf(x, 0.f) - log1pf(expf(-fabsf(x))); }
-__device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 __device__ __forceinline__ float powg(float x, float g) { return g == 2.f ? x * x : powf(x, g); }
 
 // SigmoidFocalLoss element for target t in {0, 1} (t = -1 is zero and handled by the caller), before the < 1e-5 clamp

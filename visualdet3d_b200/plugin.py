@@ -115,3 +115,14 @@ def install_loss_into_reference():
     from .anchor_loss import head_loss
     ref_head.AnchorBasedDetection3DHead.loss = head_loss
     return head_loss
+
+
+def install_monoflex_loss_into_reference():
+    """Make the REFERENCE's MonoFlex head train with the native loss (`monoflex_loss.head_loss`): rebinds `MonoFlexHead.loss` in
+    `visualDet3D.networks.heads.monoflex_head`, so the unmodified scripts/train.py (train_rtm3d) computes MonoFlex's head loss on the GPU
+    path.  KM3DHead keeps its own loss.  Each call reads the head's uncertainty_range and uncertainty_weight.  Returns the installed
+    function."""
+    from visualDet3D.networks.heads import monoflex_head as ref_head         # ImportError if the reference is not on sys.path
+    from .monoflex_loss import head_loss
+    ref_head.MonoFlexHead.loss = head_loss
+    return head_loss

@@ -159,6 +159,22 @@ def synth_head_outputs(B: int, N: int, C: int, seed: int = 0) -> Tuple[torch.Ten
     return torch.from_numpy(cls), torch.from_numpy(reg)
 
 
+def monoflex_head_outputs(B: int, C: int, H: int, W: int, seed: int = 0) -> dict:
+    """Stand-ins for the MonoFlex head's nine output maps (fp32 NCHW), for the loss tests, from a seeded numpy RandomState (the same
+    values on every machine).  hm logits lie on a 1/8 grid over [-6, 6], which keeps sigmoid well away from the focal loss's 0.99 / 0.01
+    cuts; the keypoint y channels put keypoints 2, 3, 6, 7 and 8 below 0, 1, 4, 5 and 9, so the keypoint heights are mostly positive and
+    the keypoint depths land inside [0.1, 100]; depth decodes (exp(-depth)) to 4..55 m."""
+    rng = np.random.RandomState(seed)
+    u = lambda lo, hi, ch: rng.uniform(lo, hi, size=(B, ch, H, W)).astype(np.float32)  # noqa: E731
+    out = dict(hm=(rng.randint(-48, 49, size=(B, C, H, W)) / 8).astype(np.float32), bbox2d=u(0.5, 12.0, 4))
+    hps = u(-10.0, 10.0, 20)
+    below = np.array([-1, -1, 1, 1, -1, -1, 1, 1, 1, -1], dtype=np.float32)
+    hps[:, 1::2] = below[None, :, None, None] * u(1.5, 8.0, 10)
+    out.update(hps=hps, rot=u(-2.0, 2.0, 8), dim=u(1.0, 4.0, 3), reg=u(0.0, 1.0, 2), depth=u(-4.0, -1.4, 1),
+               depth_uncertainty=u(-1.0, 3.0, 1), corner_uncertainty=u(-1.0, 3.0, 3))
+    return {k: torch.from_numpy(np.ascontiguousarray(v)) for k, v in out.items()}
+
+
 def synth_P2(B: int, H: int, W: int, seed: int = 1, jitter: float = 0.02) -> Tuple[torch.Tensor, torch.Tensor]:
     """KITTI P2 pushed through CropTop(100) + Resize((H, W)) like stereo_augmentator.py:213-258 does, with a
     per-image +-jitter on fx/fy/cy so the [B, N] useful-mask path is exercised.  P3 = P2 with Tx -= 0.54 fx."""
