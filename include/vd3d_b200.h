@@ -459,6 +459,31 @@ int vd3d_monoflex_loss_backward(const void* const* maps, const void* const* targ
                                 float unc_hi, float unc_w, const void* workspace, const float* grad_terms, const float* grad_total,
                                 float* const* grads, void* stream);
 
+/* ---- training loss of the KM3D head (KM3DHead.loss, R/networks/heads/km3d_head.py:316-351) ----------------------------------------
+ * Replaces _neg_loss (hm and hm_hp), _RegWeightedL1Loss, _RegL1Loss (wh, dim, reg, hp_offset), _RotLoss (km3d_head.py:61-130,
+ * compute_rot_loss rtm3d_utils.py:9-49) and Position_loss with gen_position (rtm3d_utils.py:230-455).
+ * maps (host array of 9 device pointers, f32 NCHW): hm [B][C][H][W] logits, wh 2, hps 18, rot 8, dim 3, prob 1, reg 2, hm_hp 9 (logits),
+ *   hp_offset 2 channels.
+ * targets (host array of 18 device pointers): hm [B][C][H][W] f32, hm_hp [B][9][H][W] f32, ind [B][K] i64, reg_mask [B][K] u8,
+ *   hps [B][K][18] f32, hps_mask [B][K][18] u8, dep [B][K] f32, rotbin [B][K][2] i64, rotres [B][K][2] f32, wh [B][K][2] f32,
+ *   dim [B][K][3] f32, reg [B][K][2] f32, hp_ind [B][K*9] i64, hp_mask [B][K*9] u8, hp_offset [B][K*9][2] f32, location [B][K][3] f32,
+ *   ori [B][K] f32, P2 [B][3][4] f32.  K <= 128; 9 keypoints per object.  Inputs are never written (the reference rewrites dep in place).
+ * output_w: the loss config's output_w (the keypoint centre is (ind mod output_w, trunc(ind / output_w))); rampup: exp_rampup(epoch),
+ *   the weight of prob_loss and coor_loss (a captured graph holds one epoch's value).
+ * vd3d_km3d_loss_forward: terms [11] f32 = hm, hp, hm_hp, hp_offset, wh, off, dim, rot, prob, coor, box_score (unweighted, as in
+ *   loss_stats) and total [1] f32 = the first ten weighted 1, 1, 1, 1, 0.1, 1, 2, 0.2, rampup, rampup.  Three launches, no host
+ *   synchronisation, no float atomics.  An ind or hp_ind outside [0, H*W) in any row makes every loss NaN (the map is not read there).
+ *   workspace: vd3d_km3d_loss_workspace_bytes(B, C, H, W, K) bytes of device memory (negative: error code); the backward reads the factors
+ *   the forward leaves in it.
+ * vd3d_km3d_loss_backward: grad_terms [11] and grad_total [1] f32 (device; either may be null = zero) = d/d terms, d/d total (box_score
+ *   has no gradient); writes grads (host array of 9 device pointers, shaped like maps) in full.  One launch. */
+long long vd3d_km3d_loss_workspace_bytes(int B, int C, int H, int W, int K);
+int vd3d_km3d_loss_forward(const void* const* maps, const void* const* targets, int B, int C, int H, int W, int K, float output_w,
+                           float rampup, void* workspace, long long workspace_bytes, float* terms, float* total, void* stream);
+int vd3d_km3d_loss_backward(const void* const* maps, const void* const* targets, int B, int C, int H, int W, int K, float output_w,
+                            float rampup, const void* workspace, const float* grad_terms, const float* grad_total, float* const* grads,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif

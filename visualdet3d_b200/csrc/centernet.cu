@@ -8,6 +8,7 @@
 // Order equivalence: the reference keeps the K best peaks, then drops scores <= score_thr; selecting peaks > score_thr first
 // and keeping the best K of those yields the same set and order (scores are sorted descending, ties by flat index).
 #include "common.cuh"
+#include "km3d_position.cuh"
 
 namespace vd3d {
 
@@ -287,57 +288,11 @@ __global__ void __launch_bounds__(CN_THREADS) km3d_decode_nms_kernel(
         l *= 4.f; tp *= 4.f; rr *= 4.f; bt *= 4.f;
         // gen_position
         const float* P = P2 + 12 * b;
-        const float f = P[0], pcx = P[2], pcy = P[6];
-        const float* rot = px + L.rot;
-        float a1 = atanf(rot[2] / rot[3]) + (-0.5f * 3.14159265358979323846f);
-        float a2 = atanf(rot[6] / rot[7]) + (0.5f * 3.14159265358979323846f);
-        float sel = (rot[1] > rot[5]) ? 1.f : 0.f;
-        float alpha = a1 * sel + a2 * (1.f - sel);
-        float rot_y = alpha + atan2f(kx[8] - pcx, f);
-        const float PI = 3.14159265358979323846f;
-        if (rot_y > PI) rot_y = rot_y - 2.f * PI;
-        if (rot_y < -PI) rot_y = rot_y + 2.f * PI;
-        float dw = px[L.dim + 0], dh = px[L.dim + 1], dl = px[L.dim + 2];
-        float co = cosf(rot_y), si = sinf(rot_y);
-        float lc = dl * 0.5f * co, ls = dl * 0.5f * si, wc = dw * 0.5f * co, wsn = dw * 0.5f * si, hh = dh * 0.5f;
-        // rows 2j (x of corner j) and 2j+1 (y of corner j), corners 0..7
-        const float Bx[8] = {-lc - wsn, -lc + wsn, -lc + wsn, lc + wsn, lc + wsn, lc - wsn, lc - wsn, -lc - wsn};
-        const float By[8] = {-hh, -hh, hh, hh, -hh, -hh, hh, hh};
-        const float Cc[8] = {ls - wc, ls + wc, ls + wc, -ls + wc, -ls + wc, -ls - wc, -ls - wc, ls - wc};
-        double ata[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
-        float A2[16], Bv[16];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            float nx = (kx[j] - pcx) / f, ny = (ky[j] - pcy) / f;
-            A2[2 * j] = nx; A2[2 * j + 1] = ny;
-            Bv[2 * j] = Bx[j] - nx * Cc[j];
-            Bv[2 * j + 1] = By[j] - ny * Cc[j];
-        }
-        // A row 2j = [-1, 0, nx], row 2j+1 = [0, -1, ny]
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            double a0 = (q & 1) ? 0.0 : -1.0, a1d = (q & 1) ? -1.0 : 0.0, a2d = (double)A2[q];
-            ata[0][0] += a0 * a0; ata[0][1] += a0 * a1d; ata[0][2] += a0 * a2d;
-            ata[1][1] += a1d * a1d; ata[1][2] += a1d * a2d; ata[2][2] += a2d * a2d;
-        }
-        ata[1][0] = ata[0][1]; ata[2][0] = ata[0][2]; ata[2][1] = ata[1][2];
-        // 3x3 inverse (double)
-        double c00 = ata[1][1] * ata[2][2] - ata[1][2] * ata[2][1], c01 = ata[0][2] * ata[2][1] - ata[0][1] * ata[2][2], c02 = ata[0][1] * ata[1][2] - ata[0][2] * ata[1][1];
-        double c10 = ata[1][2] * ata[2][0] - ata[1][0] * ata[2][2], c11 = ata[0][0] * ata[2][2] - ata[0][2] * ata[2][0], c12 = ata[0][2] * ata[1][0] - ata[0][0] * ata[1][2];
-        double c20 = ata[1][0] * ata[2][1] - ata[1][1] * ata[2][0], c21 = ata[0][1] * ata[2][0] - ata[0][0] * ata[2][1], c22 = ata[0][0] * ata[1][1] - ata[0][1] * ata[1][0];
-        double det = ata[0][0] * c00 + ata[0][1] * c10 + ata[0][2] * c20;
-        double inv[3][3] = {{c00 / det, c01 / det, c02 / det}, {c10 / det, c11 / det, c12 / det}, {c20 / det, c21 / det, c22 / det}};
-        float pos[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            double a0 = (q & 1) ? 0.0 : -1.0, a1d = (q & 1) ? -1.0 : 0.0, a2d = (double)A2[q];
-#pragma unroll
-            for (int rI = 0; rI < 3; ++rI) {
-                float pq = (float)(inv[rI][0] * a0 + inv[rI][1] * a1d + inv[rI][2] * a2d);     // (pinv @ A^T).float()
-                pos[rI] = fmaf(pq, Bv[q], pos[rI]);
-            }
-        }
-        pos[0] -= P[3] / P[0];
+        vd3d::Km3dPosition gp;
+        const float dw = px[L.dim + 0], dh = px[L.dim + 1], dl = px[L.dim + 2];
+        vd3d::km3d_gen_position(kx, ky, dw, dh, dl, px + L.rot, P, gp);
+        const float alpha = gp.alpha;
+        const float* pos = gp.pos;
         float z3 = pos[2];
         float cx3 = (pos[0] * P[0] + P[3] + P[2] * z3) / z3;
         float cy3 = (pos[1] * P[5] + P[7] + P[6] * z3) / z3;

@@ -1,4 +1,4 @@
-// Device helpers shared by the training-loss kernels (anchor_loss.cu, monoflex_loss.cu).
+// Device helpers shared by the training-loss kernels (anchor_loss.cu, monoflex_loss.cu, km3d_loss.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -7,5 +7,118 @@ namespace vd3d {
 // torch.nn.functional.logsigmoid, in its overflow-free form
 __device__ __forceinline__ float log_sigmoid(float x) { return fminf(x, 0.f) - log1pf(expf(-fabsf(x))); }
 __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
+// torch.sign: 0 at 0
+__device__ __forceinline__ float sign0(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); }
+
+// ---- the heatmap focal terms of CenterNet-style heads (KM3DHead._neg_loss, km3d_head.py:61-98) -----------------------------------------
+constexpr int kHmRec = 3;              // per-block partial: positive sum, negative sum, positive count
+
+__device__ __forceinline__ void hm_terms(float x, float g, float& pos, float& neg) {
+    const float p = sigmoid(x);
+    pos = neg = 0.f;
+    if (g == 1.f && !(p > 0.99f)) pos = log_sigmoid(x) * ((1.f - p) * (1.f - p));
+    if (g < 1.f && !(p < 0.01f)) {
+        const float w = (1.f - g) * (1.f - g);
+        neg = log_sigmoid(-x) * (p * p) * (w * w);
+    }
+}
+
+// d (pos + neg) / dx, the powers of p not detached
+__device__ __forceinline__ float hm_grad(float x, float g) {
+    const float p = sigmoid(x), q = 1.f - p;
+    if (g == 1.f) return p > 0.99f ? 0.f : q * q * q - 2.f * p * q * q * log_sigmoid(x);
+    if (g < 1.f && !(p < 0.01f)) {
+        const float w = (1.f - g) * (1.f - g);
+        return (w * w) * (-p * p * p + 2.f * p * p * q * log_sigmoid(-x));
+    }
+    return 0.f;
+}
+
+// One block's partials of the focal terms over hm / gt [n]: the block is number `block` of `nblocks` striding over the elements by
+// kThreads; the partial (kHmRec doubles) goes to partial[block].  Reduced in a fixed order (warp shuffle tree, then warps in order).
+template <int kThreads>
+__device__ __forceinline__ void hm_block_partial(const float* __restrict__ hm, const float* __restrict__ gt, long long n, int block,
+                                                 int nblocks, double* __restrict__ partial) {
+    __shared__ double s_red[kThreads / 32][kHmRec];
+    double acc[kHmRec] = {0.0, 0.0, 0.0};
+    for (long long i = (long long)block * kThreads + threadIdx.x; i < n; i += (long long)nblocks * kThreads) {
+        const float g = gt[i];
+        float pos, neg;
+        hm_terms(hm[i], g, pos, neg);
+        acc[0] += pos;
+        acc[1] += neg;
+        acc[2] += g == 1.f ? 1.0 : 0.0;
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < kHmRec; ++k) {
+        double v = acc[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+        if (lane == 0) s_red[warp][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < kHmRec) {
+        double v = 0.0;
+        for (int w = 0; w < kThreads / 32; ++w) v += s_red[w][threadIdx.x];
+        partial[(size_t)block * kHmRec + threadIdx.x] = v;
+    }
+}
+
+// ---- one object row of KM3DHead._RegWeightedL1Loss (km3d_head.py:100-115) -------------------------------------------------------------
+// at(c): the keypoint map's channel c at the row's pixel; mask / target: the row's kKp entries of hps_mask / hps; dep: the row's depth,
+// transformed on a copy (0.01 dep below 5, log10(dep - 4) + 0.1 from 5).  Returns the row's weighted L1 in l and its mask sum in ms; with
+// kGrad, adds d l / d at(c) times scale to g[c].
+template <int kKp, bool kGrad, class At>
+__device__ __forceinline__ void weighted_l1_row(At at, const unsigned char* mask, const float* target, float dep, float scale, float* g,
+                                                float& l_out, float& ms_out) {
+    const float dep_t = dep < 5.f ? dep * 0.01f : log10f(dep - 4.f) + 0.1f;
+    float l = 0.f, ms = 0.f;
+    for (int c = 0; c < kKp; ++c) {
+        const float m = (float)mask[c];
+        const float d = at(c) * m - target[c] * m;
+        if (kGrad) g[c] += sign0(d) * m * dep_t * scale;
+        l += fabsf(d);
+        ms += m;
+    }
+    l_out = l * dep_t;
+    ms_out = ms;
+}
+
+// ---- one object row of compute_rot_loss (rtm3d_utils.py:9-49) -------------------------------------------------------------------------
+// at(c): the rotation map's channel c (8) at the row's pixel; valid: the row's reg_mask; bin / res: its rotbin / rotres (2 each).  The two
+// cross-entropies use the logits times reg_mask (every row counts); the sin / cos smooth-L1 of bin j counts where bin j is set.  Returns
+// the cross-entropy sum in ce and, for each set bin j, its residual loss in res[j] and 1 in n[j] (untouched otherwise); with kGrad, adds
+// the gradient (cross-entropy scaled by s_ce, residual j by s_res[j]) to g[0..7].
+template <bool kGrad, class At>
+__device__ __forceinline__ void rot_row(At at, bool valid, const long long* bin2, const float* res2, float s_ce, float s_res1, float s_res2,
+                                        float* g, float& ce_out, float* res, float* n) {
+    const float m = valid ? 1.f : 0.f;
+    float ce = 0.f;
+    for (int j = 0; j < 2; ++j) {
+        const long long bin = bin2[j];
+        const float z0 = at(4 * j) * m, z1 = at(4 * j + 1) * m;
+        const float mx = fmaxf(z0, z1);
+        const float lse = mx + logf(expf(z0 - mx) + expf(z1 - mx));
+        ce += lse - (bin != 0 ? z1 : z0);
+        if (kGrad) {
+            g[4 * j] += (expf(z0 - lse) - (bin != 0 ? 0.f : 1.f)) * m * s_ce;
+            g[4 * j + 1] += (expf(z1 - lse) - (bin != 0 ? 1.f : 0.f)) * m * s_ce;
+        }
+        if (bin != 0) {
+            const float r = res2[j];
+            const float ds = at(4 * j + 2) - sinf(r), dc = at(4 * j + 3) - cosf(r);
+            if (kGrad) {
+                const float f = j == 0 ? s_res1 : s_res2;
+                g[4 * j + 2] += (fabsf(ds) < 1.f ? ds : sign0(ds)) * f;
+                g[4 * j + 3] += (fabsf(dc) < 1.f ? dc : sign0(dc)) * f;
+            } else {
+                const float ads = fabsf(ds), adc = fabsf(dc);
+                res[j] = (ads < 1.f ? 0.5f * ds * ds : ads - 0.5f) + (adc < 1.f ? 0.5f * dc * dc : adc - 0.5f);
+                n[j] = 1.f;
+            }
+        }
+    }
+    ce_out = ce;
+}
 
 }  // namespace vd3d

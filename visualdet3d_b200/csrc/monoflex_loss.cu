@@ -19,6 +19,8 @@
 #include "loss_common.cuh"
 
 using vd3d::cdiv;
+using vd3d::hm_grad;
+using vd3d::kHmRec;
 using vd3d::log_sigmoid;
 using vd3d::sigmoid;
 
@@ -43,7 +45,6 @@ enum { T_HM, T_IND, T_REG_MASK, T_HPS, T_HPS_MASK, T_DEP, T_ROTBIN, T_ROTRES, T_
 
 // per-image partial record of the rows pass
 enum { R_HP, R_HPM, R_CE, R_RES1, R_N1, R_RES2, R_N2, R_N, R_BOX, R_DIM, R_OFF, R_DEPTH, R_KPD, R_SOFT, R_BAD, kRec };
-constexpr int kHmRec = 3;              // positive sum, negative sum, positive count
 // factors [kFac] f32 written by combine: d term / d (summed element) of each denominator
 enum { F_HM, F_HP, F_CE, F_RES1, F_RES2, F_GATH, kFac };
 
@@ -72,61 +73,15 @@ struct Scales {
 };
 
 __device__ __forceinline__ float sgn(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); }
-__device__ __forceinline__ float smooth_l1(float d) { const float a = fabsf(d); return a < 1.f ? 0.5f * d * d : a - 0.5f; }
-__device__ __forceinline__ float smooth_l1_grad(float d) { return fabsf(d) < 1.f ? d : sgn(d); }
 // d max(a, b) / d a and d min(a, b) / d a: a tie splits the gradient
 __device__ __forceinline__ float dmax(float a, float b) { return a > b ? 1.f : (a == b ? 0.5f : 0.f); }
 __device__ __forceinline__ float dmin(float a, float b) { return a < b ? 1.f : (a == b ? 0.5f : 0.f); }
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
 __device__ __forceinline__ float clamp_pass(float x, float lo, float hi) { return (x >= lo && x <= hi) ? 1.f : 0.f; }
 
-// ---- the heatmap focal terms (_neg_loss) -------------------------------------------------------------------------------------------
-__device__ __forceinline__ void hm_terms(float x, float g, float& pos, float& neg) {
-    const float p = sigmoid(x);
-    pos = neg = 0.f;
-    if (g == 1.f && !(p > 0.99f)) pos = log_sigmoid(x) * ((1.f - p) * (1.f - p));
-    if (g < 1.f && !(p < 0.01f)) {
-        const float w = (1.f - g) * (1.f - g);
-        neg = log_sigmoid(-x) * (p * p) * (w * w);
-    }
-}
-
-// d (pos + neg) / dx, the powers of p not detached
-__device__ __forceinline__ float hm_grad(float x, float g) {
-    const float p = sigmoid(x), q = 1.f - p;
-    if (g == 1.f) return p > 0.99f ? 0.f : q * q * q - 2.f * p * q * q * log_sigmoid(x);
-    if (g < 1.f && !(p < 0.01f)) {
-        const float w = (1.f - g) * (1.f - g);
-        return (w * w) * (-p * p * p + 2.f * p * p * q * log_sigmoid(-x));
-    }
-    return 0.f;
-}
-
 __global__ void __launch_bounds__(kThreads) hm_kernel(const float* __restrict__ hm, const float* __restrict__ gt, long long n,
                                                       double* __restrict__ partial) {
-    __shared__ double s_red[kThreads / 32][kHmRec];
-    double acc[kHmRec] = {0.0, 0.0, 0.0};
-    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads) {
-        const float g = gt[i];
-        float pos, neg;
-        hm_terms(hm[i], g, pos, neg);
-        acc[0] += pos;
-        acc[1] += neg;
-        acc[2] += g == 1.f ? 1.0 : 0.0;
-    }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kHmRec; ++k) {
-        double v = acc[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kHmRec) {
-        double v = 0.0;
-        for (int w = 0; w < kThreads / 32; ++w) v += s_red[w][threadIdx.x];
-        partial[(size_t)blockIdx.x * kHmRec + threadIdx.x] = v;
-    }
+    vd3d::hm_block_partial<kThreads>(hm, gt, n, blockIdx.x, gridDim.x, partial);
 }
 
 // ---- one object row: its loss terms (rec, forward) or its gradient at the gathered pixel (g[kGathCh], backward) ----------------------
@@ -146,48 +101,24 @@ __device__ bool row_eval(const Args& a, int b, int k, const Scales* s, float* re
 
     // hp_loss: every row, under hps_mask; dep transformed on a copy
     const float dep = a.dep[r];
-    const float dep_t = dep < 5.f ? dep * 0.01f : log10f(dep - 4.f) + 0.1f;
     {
-        float l = 0.f, ms = 0.f;
-        for (int c = 0; c < 20; ++c) {
-            const float m = (float)a.hps_mask[r * 20 + c];
-            const float d = at(M_HPS, c) * m - a.hps_t[r * 20 + c] * m;
-            if (kGrad) g[kGOff[M_HPS] + c] += sgn(d) * m * dep_t * s->hp;
-            l += fabsf(d);
-            ms += m;
-        }
-        if (!kGrad) { rec[R_HP] = l * dep_t; rec[R_HPM] = ms; }
+        float l, ms;
+        vd3d::weighted_l1_row<20, kGrad>([&](int c) { return at(M_HPS, c); }, a.hps_mask + r * 20, a.hps_t + r * 20, dep,
+                                         kGrad ? s->hp : 0.f, g + kGOff[M_HPS], l, ms);
+        if (!kGrad) { rec[R_HP] = l; rec[R_HPM] = ms; }
     }
 
     // rot_loss: two cross-entropies of every row (logits times reg_mask), smooth-L1 of the rows whose bin is set
     const bool valid = a.reg_mask[r] != 0;
     {
-        const float m = valid ? 1.f : 0.f;
-        float ce = 0.f;
-        for (int j = 0; j < 2; ++j) {
-            const long long bin = a.rotbin[r * 2 + j];
-            const float z0 = at(M_ROT, 4 * j) * m, z1 = at(M_ROT, 4 * j + 1) * m;
-            const float mx = fmaxf(z0, z1);
-            const float lse = mx + logf(expf(z0 - mx) + expf(z1 - mx));
-            ce += lse - (bin != 0 ? z1 : z0);
-            if (kGrad) {
-                g[kGOff[M_ROT] + 4 * j] += (expf(z0 - lse) - (bin != 0 ? 0.f : 1.f)) * m * s->ce;
-                g[kGOff[M_ROT] + 4 * j + 1] += (expf(z1 - lse) - (bin != 0 ? 1.f : 0.f)) * m * s->ce;
-            }
-            if (bin != 0) {
-                const float res = a.rotres[r * 2 + j];
-                const float ds = at(M_ROT, 4 * j + 2) - sinf(res), dc = at(M_ROT, 4 * j + 3) - cosf(res);
-                if (kGrad) {
-                    const float f = j == 0 ? s->res1 : s->res2;
-                    g[kGOff[M_ROT] + 4 * j + 2] += smooth_l1_grad(ds) * f;
-                    g[kGOff[M_ROT] + 4 * j + 3] += smooth_l1_grad(dc) * f;
-                } else {
-                    rec[j == 0 ? R_RES1 : R_RES2] = smooth_l1(ds) + smooth_l1(dc);
-                    rec[j == 0 ? R_N1 : R_N2] = 1.f;
-                }
-            }
+        float ce, res[2] = {0.f, 0.f}, n[2] = {0.f, 0.f};
+        vd3d::rot_row<kGrad>([&](int c) { return at(M_ROT, c); }, valid, a.rotbin + r * 2, a.rotres + r * 2, kGrad ? s->ce : 0.f,
+                             kGrad ? s->res1 : 0.f, kGrad ? s->res2 : 0.f, g + kGOff[M_ROT], ce, res, n);
+        if (!kGrad) {
+            rec[R_CE] = ce;
+            rec[R_RES1] = res[0]; rec[R_N1] = n[0];
+            rec[R_RES2] = res[1]; rec[R_N2] = n[1];
         }
-        if (!kGrad) rec[R_CE] = ce;
     }
     if (!valid) return true;
 

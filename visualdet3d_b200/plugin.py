@@ -126,3 +126,14 @@ def install_monoflex_loss_into_reference():
     from .monoflex_loss import head_loss
     ref_head.MonoFlexHead.loss = head_loss
     return head_loss
+
+
+def install_km3d_loss_into_reference():
+    """Make the REFERENCE's KM3D head train with the native loss (`km3d_loss.head_loss`): rebinds `KM3DHead.loss` in
+    `visualDet3D.networks.heads.km3d_head`, so the unmodified scripts/train.py (train_rtm3d) computes KM3D's head loss on the GPU path.
+    MonoFlexHead subclasses KM3DHead but defines its own loss, which stays as it is.  Each call reads the head's position_loss.output_w
+    and rampup_length.  Returns the installed function."""
+    from visualDet3D.networks.heads import km3d_head as ref_head             # ImportError if the reference is not on sys.path
+    from .km3d_loss import head_loss
+    ref_head.KM3DHead.loss = head_loss
+    return head_loss
