@@ -484,6 +484,24 @@ int vd3d_km3d_loss_backward(const void* const* maps, const void* const* targets,
                             float rampup, const void* workspace, const float* grad_terms, const float* grad_total, float* const* grads,
                             void* stream);
 
+/* ---- disparity loss of Stereo3D (DisparityLoss(max_disp), R/networks/heads/losses.py:122-135) -----------------------------------------
+ * Replaces StereoFocalLoss.loss_per_level with LaplaceDisp2Prob (R/networks/lib/disparity_loss/*.py) at the shipped settings: start_disp 0,
+ * dilation 1, one level, focal_coefficient 0, variance 0.5, the label at the cost volume's H, W, and max_disp = D.
+ * cost [B][D][H][W] f32 (logits), disp [B][H][W] f32 (the disparity label; 0 = no label).  2 <= D <= 1024, H*W < 2^31 - 256, offsets are
+ *   64-bit.  Masks: outer = 0 < disp < D (the loss), inner = 0 < disp < D - 1 (the target); target p_c = softmax_c(-|c - disp*inner| / 0.5)
+ *   * inner + 1e-40.  Inputs are never written.
+ * vd3d_disparity_loss_forward: loss [1] f32 = -(1/(B*H*W)) sum_pixels outer * sum_c p_c log_softmax(cost)_c, and lse [B][H][W] f32 = each
+ *   pixel's log-sum-exp over D (0 outside outer), which the backward reads.  Two launches, no host synchronisation, no float atomics; one
+ *   read of the volume (none at pixels outside outer).  With no outer pixel the loss is 0; a non-finite disp value makes it NaN.
+ *   workspace: vd3d_disparity_loss_workspace_bytes(B, D, H, W) bytes of device memory (negative: error code), one float64 per block.
+ * vd3d_disparity_loss_backward: grad_loss [1] f32 (device) = d/d loss; writes grad_cost [B][D][H][W] in full (exact zeros outside outer).
+ *   One launch. */
+long long vd3d_disparity_loss_workspace_bytes(int B, int D, int H, int W);
+int vd3d_disparity_loss_forward(const float* cost, const float* disp, int B, int D, int H, int W, void* workspace, long long workspace_bytes,
+                                float* lse, float* loss, void* stream);
+int vd3d_disparity_loss_backward(const float* cost, const float* disp, const float* lse, int B, int D, int H, int W, const float* grad_loss,
+                                 float* grad_cost, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -110,6 +110,9 @@ _SIGS = {
     "vd3d_km3d_loss_workspace_bytes": (c_longlong, [I, I, I, I, I]),
     "vd3d_km3d_loss_forward": (I, [P, P, I, I, I, I, I, F, F, P, c_longlong, P, P, P]),
     "vd3d_km3d_loss_backward": (I, [P, P, I, I, I, I, I, F, F, P, P, P, P, P]),
+    "vd3d_disparity_loss_workspace_bytes": (c_longlong, [I, I, I, I]),
+    "vd3d_disparity_loss_forward": (I, [P, P, I, I, I, I, P, c_longlong, P, P, P]),
+    "vd3d_disparity_loss_backward": (I, [P, P, P, I, I, I, I, P, P, P]),
 }
 
 

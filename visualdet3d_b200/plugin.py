@@ -137,3 +137,15 @@ def install_km3d_loss_into_reference():
     from .km3d_loss import head_loss
     ref_head.KM3DHead.loss = head_loss
     return head_loss
+
+
+def install_disparity_loss_into_reference():
+    """Make the REFERENCE's Stereo3D train its disparity branch with the native loss (`disparity_loss.forward`): rebinds
+    `DisparityLoss.forward` in `visualDet3D.networks.heads.losses`, so the unmodified `Stereo3D.train_forward` (scripts/train.py,
+    train_stereo_detection) computes the stereo focal loss on the GPU path.  With `install_loss_into_reference()` the whole Stereo3D
+    training loss is native.  Each call reads the criterion's max_disp and refuses settings other than the shipped ones.  Returns the
+    installed function."""
+    from visualDet3D.networks.heads import losses as ref_losses               # ImportError if the reference is not on sys.path
+    from .disparity_loss import forward
+    ref_losses.DisparityLoss.forward = forward
+    return forward
