@@ -696,6 +696,14 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
         p.chunk = e ? atoi(e) : 4;
         if (p.chunk < 1) p.chunk = 1;
     }
+    {
+        // 64-channel 3x3 convs: the row-strip kernel (conv2d_row64.cu, same bits).  VD3D_ROW64=0 keeps them on conv2d_tcp_kernel, as do the
+        // MMA-mode timing experiments (VD3D_TC_DEBUG bits 0 and 1), which only conv2d_tcp_kernel implements.
+        const char* e = getenv("VD3D_ROW64");
+        const char* d = getenv("VD3D_TC_DEBUG");
+        if (!ls && conv2d_row64_eligible(p) && !(e && atoi(e) == 0) && !(d && (atoi(d) & 3)))
+            return conv2d_row64_launch(p, in, in_lo, in_cs, in_co, w_hi, w_lo, stream);
+    }
     const int K = KH * KW * p.cin_pad;
     CUtensorMap mA, mAlo, mWhi, mWlo;
     int rc;

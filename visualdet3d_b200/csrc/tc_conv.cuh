@@ -118,25 +118,27 @@ __device__ __forceinline__ int unit_nt(const TcParams& p, int u, int mt_units) {
 // step (A_lo W_hi, A_hi W_lo, A_hi W_hi: small terms first, then the main product), one (A W) or two (A W_lo, A W) in the experiment modes.
 // `first`: the first k-block of a promotion chunk (the accumulator restarts from zero).  MODE and KSTEPS are template arguments so that the
 // MMA chain is straight-line code: wgmma instructions under a run-time branch make ptxas serialise them (warpgroup.arrive / wait injection).
+// AK: step of the A descriptor per K step in 16-byte units (2: 32 bytes along a swizzled 128-byte row; conv2d_row64.cu's core-matrix rows
+// keep each 8-channel group in a plane of its own, so a K step there moves two planes).
 template <int N, bool F16>
 __device__ __forceinline__ void wg_mma(float (&c)[N / 2], uint64_t da, uint64_t db, uint32_t acc) {
     if constexpr (F16) wgmma_f16<N>(c, da, db, acc); else wgmma_tf32<N>(c, da, db, acc);
 }
-template <int N, bool F16, int MODE, int KSTEPS>
+template <int N, bool F16, int MODE, int KSTEPS, int AK = 2>
 __device__ __forceinline__ void wg_kblock(float (&c)[N / 2], uint64_t dA, uint64_t dAlo, uint64_t dB, uint64_t dBlo, bool first) {
 #pragma unroll
     for (int k = 0; k < KSTEPS; ++k) {
-        const uint64_t off = (uint64_t)((k * 32) >> 4);
+        const uint64_t off = (uint64_t)((k * 32) >> 4), aoff = (uint64_t)(k * AK);
         const uint32_t acc0 = (first && k == 0) ? 0u : 1u;
         if constexpr (MODE == 0) {
-            wg_mma<N, F16>(c, dAlo + off, dB + off, acc0);
-            wg_mma<N, F16>(c, dA + off, dBlo + off, 1u);
-            wg_mma<N, F16>(c, dA + off, dB + off, 1u);
+            wg_mma<N, F16>(c, dAlo + aoff, dB + off, acc0);
+            wg_mma<N, F16>(c, dA + aoff, dBlo + off, 1u);
+            wg_mma<N, F16>(c, dA + aoff, dB + off, 1u);
         } else if constexpr (MODE == 2) {
-            wg_mma<N, F16>(c, dA + off, dBlo + off, acc0);
-            wg_mma<N, F16>(c, dA + off, dB + off, 1u);
+            wg_mma<N, F16>(c, dA + aoff, dBlo + off, acc0);
+            wg_mma<N, F16>(c, dA + aoff, dB + off, 1u);
         } else {
-            wg_mma<N, F16>(c, dA + off, dB + off, acc0);
+            wg_mma<N, F16>(c, dA + aoff, dB + off, acc0);
         }
     }
 }
@@ -156,11 +158,11 @@ struct KbOperands { uint64_t dA, dAlo, dB, dBlo; int slot; };
 
 // One k-block: wait for its operands (acquire), issue its MMAs as one commit group, then wait until at most this group is outstanding and
 // release the slot of the previous k-block.  `pend`: slot of the k-block whose MMAs may still be running (-1: none).
-template <int N, bool F16, int MODE, int KSTEPS, class Acquire, class Release, class Issued>
+template <int N, bool F16, int MODE, int KSTEPS, int AK = 2, class Acquire, class Release, class Issued>
 __device__ __forceinline__ void wg_kblock_step(float (&c)[N / 2], bool first, int& pend, Acquire& acquire, Release& release, Issued& issued) {
     const KbOperands o = acquire();
     wg_fence();
-    wg_kblock<N, F16, MODE, KSTEPS>(c, o.dA, o.dAlo, o.dB, o.dBlo, first);
+    wg_kblock<N, F16, MODE, KSTEPS, AK>(c, o.dA, o.dAlo, o.dB, o.dBlo, first);
     wg_commit();
     wg_wait<1>();                                       // every earlier k-block's MMAs are done
     if (pend >= 0) release(pend);
@@ -174,15 +176,15 @@ __device__ __forceinline__ void wg_kblock_step(float (&c)[N / 2], bool first, in
 // asynchronous (with a conditional promotion inside the k-block loop it injects a warpgroup.wait that drains the pipe after every k-block).
 // `keep_last`: the slot of the tile's last k-block is not released but returned (the caller stages the accumulator there and releases it after
 // the epilogue); otherwise every slot is released and the result is -1.
-template <int N, bool F16, int MODE, int KSTEPS, class Acquire, class Release, class Issued>
+template <int N, bool F16, int MODE, int KSTEPS, int AK = 2, class Acquire, class Release, class Issued>
 __device__ __forceinline__ int wg_tile_kloop(float (&tot)[N / 2], float (&c)[N / 2], int KB, int chunk, Acquire& acquire, Release& release, Issued& issued,
                                              bool keep_last = false) {
     int pend = -1;
     for (int kb0 = 0; kb0 < KB; kb0 += chunk) {
         const int kb1 = min(KB, kb0 + chunk);
         pend = -1;
-        wg_kblock_step<N, F16, MODE, KSTEPS>(c, true, pend, acquire, release, issued);
-        for (int kb = kb0 + 1; kb < kb1; ++kb) wg_kblock_step<N, F16, MODE, KSTEPS>(c, false, pend, acquire, release, issued);
+        wg_kblock_step<N, F16, MODE, KSTEPS, AK>(c, true, pend, acquire, release, issued);
+        for (int kb = kb0 + 1; kb < kb1; ++kb) wg_kblock_step<N, F16, MODE, KSTEPS, AK>(c, false, pend, acquire, release, issued);
         wg_wait<0>();
         if (!keep_last || kb1 < KB) { release(pend); pend = -1; }
         wg_promote(tot, c);
@@ -357,6 +359,14 @@ inline int make_map_wgt(CUtensorMap* m, const void* base, int Cout, int K, int B
     if (r != CUDA_SUCCESS) { set_error("conv2d_tc: cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return VD3D_ECUDA; }
     return VD3D_OK;
 }
+
+// The row-strip kernel (conv2d_row64.cu) runs a conv of the fp16-split engine bit-identically to conv2d_tcp_kernel when it is a 3x3 / stride-1 /
+// pad-1 conv over at most 64 input channels into one output tile of at most 64 columns, with a plain (fp32 or plane) residual or none.
+inline bool conv2d_row64_eligible(const TcParams& p) {
+    return p.f16 && p.passes == 3 && !p.two_pass && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.pad == 1 && p.dil == 1 && p.stride_w == 1 &&
+           p.pad_w == 1 && p.cin_pad == 64 && p.BN <= 64 && p.n_tiles == 1 && p.n_levels == 0 && p.res_up_W == 0 && !p.pool_out && !p.out_lo;
+}
+int conv2d_row64_launch(TcParams& p, const void* in_hi, const void* in_lo, int in_cs, int in_co, const void* w_hi, const void* w_lo, void* stream);
 
 
 }  // namespace vd3d
