@@ -436,6 +436,28 @@ int vd3d_anchor_loss_backward(const float* cls, const float* reg, const float* a
                               int B, int N, int C, int M, const float* params, const int* assign, const float* factors, const float* grad_out,
                               float* grad_cls, float* grad_reg, void* stream);
 
+/* ---- training loss of the RetinaNet head (RetinanetHead.loss, R/networks/heads/retinanet_head.py:309-362) ----------------------------
+ * Replaces _assign / _sample / _encode / _decode (retinanet_head.py:99-255), SigmoidFocalLoss and IoULoss (losses.py:11-46, 93-120) and
+ * calc_iou (R/networks/utils/utils.py:83-100).
+ * cls [B][N][C] f32 logits, reg [B][N][4] f32 deltas, anchors [N][4] f32 (16-byte aligned), ann [B][M][K] f32 (x1 y1 x2 y2 class in the
+ *   first five columns; class -1 rows are padding, anywhere).  C <= 64, M <= 512, K >= 5.
+ * params (host) [12 + C] f32 = fg_iou_threshold, bg_iou_threshold, min_iou_threshold, focal gamma, target_means[4], target_stds[4], the
+ *   balance weight of each class.
+ * vd3d_retina_loss_forward: assign [B][N] i32 = the reference's assigned_gt_inds (1-based among the image's valid rows in their order,
+ *   0 negative, -1 ignored; 0 for every anchor of an image without a valid row); counts [B][3] i32 = positives, negatives, ignored;
+ *   scale [1] f32 = 1 / (positives of the batch + 1e-4) (read by the backward); cls_loss, reg_loss 0-d f32.  A positive whose class.long() lies
+ *   outside [0, C) makes both losses and the scale NaN.  Four launches, no host synchronisation, no float atomics (bit-reproducible).
+ *   workspace: vd3d_retina_loss_workspace_bytes(B, N, M) bytes of device memory (a negative return is an error code).
+ * vd3d_retina_loss_backward: grad_out [2] f32 (device) = d/d cls_loss, d/d reg_loss; writes grad_cls [B][N][C] and grad_reg [B][N][4]
+ *   (16-byte aligned) in full (zeros where no term depends on the element), from the forward's assign and scale.  One launch. */
+long long vd3d_retina_loss_workspace_bytes(int B, int N, int M);
+int vd3d_retina_loss_forward(const float* cls, const float* reg, const float* anchors, const float* ann, int B, int N, int C, int M, int K,
+                             const float* params, int match_low_quality, int gt_max_assign_all, void* workspace, long long workspace_bytes,
+                             int* assign, int* counts, float* scale, float* cls_loss, float* reg_loss, void* stream);
+int vd3d_retina_loss_backward(const float* cls, const float* reg, const float* anchors, const float* ann, int B, int N, int C, int M, int K,
+                              const float* params, const int* assign, const float* scale, const float* grad_out, float* grad_cls,
+                              float* grad_reg, void* stream);
+
 /* ---- training loss of the MonoFlex head (MonoFlexHead.loss, R/networks/heads/monoflex_head.py:181-236) ------------------------------
  * Replaces _neg_loss, _RegWeightedL1Loss and _RotLoss (km3d_head.py:61-130, compute_rot_loss rtm3d_utils.py:9-49), _gather_output and
  * the six gathered terms (monoflex_head.py:26-104, 194-219, decode_depth_from_keypoints rtm3d_utils.py:141-182, IoULoss losses.py:93-120).

@@ -104,6 +104,9 @@ _SIGS = {
     "vd3d_anchor_loss_workspace_bytes": (c_longlong, [I, I, I]),
     "vd3d_anchor_loss_forward": (I, [P, P, P, P, P, P, I, I, I, I, P, I, I, P, c_longlong, P, P, P, P, P, P]),
     "vd3d_anchor_loss_backward": (I, [P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P]),
+    "vd3d_retina_loss_workspace_bytes": (c_longlong, [I, I, I]),
+    "vd3d_retina_loss_forward": (I, [P, P, P, P, I, I, I, I, I, P, I, I, P, c_longlong, P, P, P, P, P, P]),
+    "vd3d_retina_loss_backward": (I, [P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P]),
     "vd3d_monoflex_loss_workspace_bytes": (c_longlong, [I, I, I, I, I]),
     "vd3d_monoflex_loss_forward": (I, [P, P, I, I, I, I, I, F, F, F, P, c_longlong, P, P, P]),
     "vd3d_monoflex_loss_backward": (I, [P, P, I, I, I, I, I, F, F, F, P, P, P, P, P]),

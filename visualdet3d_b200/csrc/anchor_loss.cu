@@ -17,7 +17,12 @@
 #include "common.cuh"
 #include "loss_common.cuh"
 
+using vd3d::assign_anchor;
 using vd3d::cdiv;
+using vd3d::focal;
+using vd3d::focal_grad;
+using vd3d::fold_gt_keys;
+using vd3d::load_gts;
 using vd3d::log_sigmoid;
 using vd3d::sigmoid;
 
@@ -46,39 +51,6 @@ struct Cfg {
 
 __constant__ float kStds[kReg] = {0.1f, 0.1f, 0.2f, 0.2f, 0.1f, 0.1f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f};
 
-// calc_iou(a, b), one pair, the reference's expression order
-__device__ __forceinline__ float calc_iou(const float* a, const float* b) {
-    const float area = (b[2] - b[0]) * (b[3] - b[1]);
-    float iw = fminf(a[2], b[2]) - fmaxf(a[0], b[0]);
-    float ih = fminf(a[3], b[3]) - fmaxf(a[1], b[1]);
-    iw = fmaxf(iw, 0.f);
-    ih = fmaxf(ih, 0.f);
-    float ua = ((a[2] - a[0]) * (a[3] - a[1]) + area) - iw * ih;
-    ua = fmaxf(ua, 1e-8f);
-    const float inter = iw * ih;
-    return inter / ua;
-}
-
-// The image's valid ground-truth rows (class != -1), compacted in their original order into s_gt[ng][12].  Returns ng.
-__device__ int load_gts(const float* ann_b, int M, float* s_gt, int* s_idx, int* s_ng) {
-    if (threadIdx.x < 32) {
-        int base = 0;
-        for (int m0 = 0; m0 < M; m0 += 32) {
-            const int m = m0 + (int)threadIdx.x;
-            const bool valid = m < M && ann_b[(size_t)m * kGtCols + 4] != -1.f;
-            const unsigned bal = __ballot_sync(0xffffffffu, valid);
-            if (valid) s_idx[base + __popc(bal & ((1u << threadIdx.x) - 1u))] = m;
-            base += __popc(bal);
-        }
-        if (threadIdx.x == 0) *s_ng = base;
-    }
-    __syncthreads();
-    const int ng = *s_ng;
-    for (int k = threadIdx.x; k < ng * kGtCols; k += blockDim.x) s_gt[k] = ann_b[(size_t)s_idx[k / kGtCols] * kGtCols + k % kGtCols];
-    __syncthreads();
-    return ng;
-}
-
 // ---- pass 1: per-ground-truth max IoU over the masked anchors, and the lowest anchor index reaching it ---------------------------
 __global__ void __launch_bounds__(kThreads) iou_max_kernel(const float* __restrict__ anchors, const unsigned char* __restrict__ mask,
                                                            const float* __restrict__ ann, Cfg cfg, unsigned long long* __restrict__ gt_key) {
@@ -88,10 +60,8 @@ __global__ void __launch_bounds__(kThreads) iou_max_kernel(const float* __restri
     unsigned long long* s_key = reinterpret_cast<unsigned long long*>(s_idx + ((cfg.M + 1) & ~1));
     __shared__ int s_ng;
     const int b = blockIdx.y;
-    const int ng = load_gts(ann + (size_t)b * cfg.M * kGtCols, cfg.M, s_gt, s_idx, &s_ng);
+    const int ng = load_gts<kGtCols>(ann + (size_t)b * cfg.M * kGtCols, cfg.M, kGtCols, s_gt, s_idx, &s_ng);
     if (ng == 0) return;
-    for (int i = threadIdx.x; i < ng; i += blockDim.x) s_key[i] = 0ull;
-    __syncthreads();
     const int n = blockIdx.x * kThreads + threadIdx.x;
     const bool m = n < cfg.N && mask[(size_t)b * cfg.N + n];
     float a[4] = {0.f, 0.f, 0.f, 0.f};
@@ -99,63 +69,10 @@ __global__ void __launch_bounds__(kThreads) iou_max_kernel(const float* __restri
         const float4 v = *reinterpret_cast<const float4*>(anchors + (size_t)n * 4);
         a[0] = v.x; a[1] = v.y; a[2] = v.z; a[3] = v.w;
     }
-    const int lane = threadIdx.x & 31;
-    for (int i = 0; i < ng; ++i) {
-        const unsigned bits = m ? __float_as_uint(calc_iou(a, s_gt + i * kGtCols)) : 0u;     // IoU >= 0: bit order is value order
-        const unsigned mx = __reduce_max_sync(0xffffffffu, bits);
-        const unsigned idx = __reduce_min_sync(0xffffffffu, (m && bits == mx) ? (unsigned)n : 0xffffffffu);
-        if (lane == 0 && idx != 0xffffffffu) atomicMax(s_key + i, ((unsigned long long)mx << 32) | (unsigned long long)(~idx));
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < ng; i += blockDim.x)
-        if (s_key[i]) atomicMax(gt_key + (size_t)b * cfg.M + i, s_key[i]);
+    fold_gt_keys<kGtCols>(a, m, n, ng, s_gt, s_key, gt_key + (size_t)b * cfg.M);
 }
 
 // ---- shared by the assignment pass and the backward -----------------------------------------------------------------------------
-// _assign for one masked anchor: the 1-based compacted ground-truth index, 0 negative, -1 ignored
-__device__ __forceinline__ int assign_anchor(const float* a, int n, int ng, const float* s_gt, const float* s_gmax, const int* s_garg,
-                                             const Cfg& cfg) {
-    float best = calc_iou(a, s_gt);
-    int arg = 0;
-    for (int i = 1; i < ng; ++i) {
-        const float v = calc_iou(a, s_gt + i * kGtCols);
-        if (v > best) { best = v; arg = i; }                          // first maximum, like max(dim=1)
-    }
-    int r = -1;
-    if (best >= 0.f && best < cfg.bg) r = 0;
-    if (best >= cfg.fg) r = arg + 1;
-    if (cfg.match_low_quality) {
-        for (int i = 0; i < ng; ++i) {                                // ground-truth order: the last match wins
-            if (!(s_gmax[i] >= cfg.min_iou)) continue;
-            if (cfg.gt_max_assign_all ? calc_iou(a, s_gt + i * kGtCols) == s_gmax[i] : n == s_garg[i]) r = i + 1;
-        }
-    }
-    return r;
-}
-
-__device__ __forceinline__ float powg(float x, float g) { return g == 2.f ? x * x : powf(x, g); }
-
-// SigmoidFocalLoss element for target t in {0, 1} (t = -1 is zero and handled by the caller), before the < 1e-5 clamp
-__device__ __forceinline__ float focal(float x, float t, float bw, float gamma) {
-    const float p = sigmoid(x);
-    const float fw = powg(t == 1.f ? 1.f - p : p, gamma);
-    const float bce = -(t * log_sigmoid(x)) * bw - ((1.f - t) * log_sigmoid(-x));
-    return fw * bce;
-}
-
-// its derivative in x, focal weight not detached (autograd on the reference expression)
-__device__ __forceinline__ float focal_grad(float x, float t, float bw, float gamma) {
-    const float p = sigmoid(x), q = 1.f - p;
-    if (t == 1.f) {
-        const float bce = -log_sigmoid(x) * bw;
-        const float dfw = gamma == 0.f ? 0.f : gamma * powg(q, gamma - 1.f) * (-p * q);
-        return dfw * bce + powg(q, gamma) * (-bw * q);
-    }
-    const float bce = -log_sigmoid(-x);
-    const float dfw = gamma == 0.f ? 0.f : gamma * powg(p, gamma - 1.f) * (p * q);
-    return dfw * bce + powg(p, gamma) * p;
-}
-
 // _encode: the 12 regression targets and the alpha class of one (anchor, ground truth) pair; ms = anchor_mean_std_3d[n][label]
 __device__ __forceinline__ float encode(const float* a, const float* g, const float* ms, float* t) {
     const float px = (a[0] + a[2]) * 0.5f, py = (a[1] + a[3]) * 0.5f, pw = a[2] - a[0], ph = a[3] - a[1];
@@ -193,7 +110,7 @@ __device__ GtShared load_image(const float* ann, const unsigned long long* gt_ke
     s.gmax = s.gt + cfg.M * kGtCols;
     s.garg = reinterpret_cast<int*>(s.gmax + cfg.M);
     int* s_idx = s.garg + cfg.M;
-    s.ng = load_gts(ann + (size_t)b * cfg.M * kGtCols, cfg.M, s.gt, s_idx, &s_ng);
+    s.ng = load_gts<kGtCols>(ann + (size_t)b * cfg.M * kGtCols, cfg.M, kGtCols, s.gt, s_idx, &s_ng);
     for (int i = threadIdx.x; gt_key && i < s.ng; i += blockDim.x) {
         const unsigned long long k = gt_key[(size_t)b * cfg.M + i];
         s.gmax[i] = __uint_as_float((unsigned)(k >> 32));
@@ -224,7 +141,7 @@ __global__ void __launch_bounds__(kThreads) assign_loss_kernel(const float* __re
             if (s.ng > 0) {
                 const float4 av = *reinterpret_cast<const float4*>(anchors + (size_t)n * 4);
                 const float a[4] = {av.x, av.y, av.z, av.w};
-                r = assign_anchor(a, n, s.ng, s.gt, s.gmax, s.garg, cfg);
+                r = assign_anchor<kGtCols>(a, n, s.ng, s.gt, s.gmax, s.garg, cfg);
                 const float* g = s.gt + (r > 0 ? r - 1 : 0) * kGtCols;
                 const int label = r > 0 ? (int)g[4] : 0;
                 const float* ms = mean_std + ((size_t)n * cfg.C + label) * 12;

@@ -1,4 +1,4 @@
-// Device helpers shared by the training-loss kernels (anchor_loss.cu, monoflex_loss.cu, km3d_loss.cu).
+// Device helpers shared by the training-loss kernels (anchor_loss.cu, retina_loss.cu, monoflex_loss.cu, km3d_loss.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -9,6 +9,111 @@ __device__ __forceinline__ float log_sigmoid(float x) { return fminf(x, 0.f) - l
 __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 // torch.sign: 0 at 0
 __device__ __forceinline__ float sign0(float x) { return x > 0.f ? 1.f : (x < 0.f ? -1.f : 0.f); }
+
+// ---- anchor assignment of the anchor heads (_assign, detection_3d_head.py:101-171 and retinanet_head.py:99-171, textually identical) --
+// Both callers compile with -fmad=false, so calc_iou rounds like torch's fp32 elementwise ops and the assignment is the reference's.
+
+// calc_iou(a, b) (R/networks/utils/utils.py:83-100), one pair, the reference's expression order
+__device__ __forceinline__ float calc_iou(const float* a, const float* b) {
+    const float area = (b[2] - b[0]) * (b[3] - b[1]);
+    float iw = fminf(a[2], b[2]) - fmaxf(a[0], b[0]);
+    float ih = fminf(a[3], b[3]) - fmaxf(a[1], b[1]);
+    iw = fmaxf(iw, 0.f);
+    ih = fmaxf(ih, 0.f);
+    float ua = ((a[2] - a[0]) * (a[3] - a[1]) + area) - iw * ih;
+    ua = fmaxf(ua, 1e-8f);
+    const float inter = iw * ih;
+    return inter / ua;
+}
+
+// The image's valid ground-truth rows (column 4, the class, != -1) of ann_b [M][pitch], compacted in their original order into
+// s_gt[ng][kCols] (each row's first kCols columns).  s_idx: M ints of shared scratch.  Called by the whole block; returns ng.
+template <int kCols>
+__device__ int load_gts(const float* ann_b, int M, int pitch, float* s_gt, int* s_idx, int* s_ng) {
+    if (threadIdx.x < 32) {
+        int base = 0;
+        for (int m0 = 0; m0 < M; m0 += 32) {
+            const int m = m0 + (int)threadIdx.x;
+            const bool valid = m < M && ann_b[(size_t)m * pitch + 4] != -1.f;
+            const unsigned bal = __ballot_sync(0xffffffffu, valid);
+            if (valid) s_idx[base + __popc(bal & ((1u << threadIdx.x) - 1u))] = m;
+            base += __popc(bal);
+        }
+        if (threadIdx.x == 0) *s_ng = base;
+    }
+    __syncthreads();
+    const int ng = *s_ng;
+    for (int k = threadIdx.x; k < ng * kCols; k += blockDim.x) s_gt[k] = ann_b[(size_t)s_idx[k / kCols] * pitch + k % kCols];
+    __syncthreads();
+    return ng;
+}
+
+// Each of the ng ground truths' max IoU over this block's taking-part anchors, and the lowest anchor index reaching it, folded into
+// gt_key[i] as one 64-bit key (iou_bits << 32 | ~anchor) with an integer atomicMax: order-independent, so deterministic.  a: the thread's
+// anchor n, m: whether it takes part.  s_key: ng slots of shared scratch.  Called by the whole block (ng > 0).
+template <int kCols>
+__device__ __forceinline__ void fold_gt_keys(const float* a, bool m, int n, int ng, const float* s_gt, unsigned long long* s_key,
+                                             unsigned long long* gt_key) {
+    for (int i = threadIdx.x; i < ng; i += blockDim.x) s_key[i] = 0ull;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    for (int i = 0; i < ng; ++i) {
+        const unsigned bits = m ? __float_as_uint(calc_iou(a, s_gt + i * kCols)) : 0u;       // IoU >= 0: bit order is value order
+        const unsigned mx = __reduce_max_sync(0xffffffffu, bits);
+        const unsigned idx = __reduce_min_sync(0xffffffffu, (m && bits == mx) ? (unsigned)n : 0xffffffffu);
+        if (lane == 0 && idx != 0xffffffffu) atomicMax(s_key + i, ((unsigned long long)mx << 32) | (unsigned long long)(~idx));
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < ng; i += blockDim.x)
+        if (s_key[i]) atomicMax(gt_key + i, s_key[i]);
+}
+
+// _assign for one taking-part anchor: the 1-based compacted ground-truth index, 0 negative, -1 ignored.  s_gmax / s_garg: each ground
+// truth's max IoU and first arg anchor (from fold_gt_keys).  Cfg: fg, bg, min_iou, match_low_quality, gt_max_assign_all.
+template <int kCols, class Cfg>
+__device__ __forceinline__ int assign_anchor(const float* a, int n, int ng, const float* s_gt, const float* s_gmax, const int* s_garg,
+                                             const Cfg& cfg) {
+    float best = calc_iou(a, s_gt);
+    int arg = 0;
+    for (int i = 1; i < ng; ++i) {
+        const float v = calc_iou(a, s_gt + i * kCols);
+        if (v > best) { best = v; arg = i; }                          // first maximum, like max(dim=1)
+    }
+    int r = -1;
+    if (best >= 0.f && best < cfg.bg) r = 0;
+    if (best >= cfg.fg) r = arg + 1;
+    if (cfg.match_low_quality) {
+        for (int i = 0; i < ng; ++i) {                                // ground-truth order: the last match wins
+            if (!(s_gmax[i] >= cfg.min_iou)) continue;
+            if (cfg.gt_max_assign_all ? calc_iou(a, s_gt + i * kCols) == s_gmax[i] : n == s_garg[i]) r = i + 1;
+        }
+    }
+    return r;
+}
+
+// ---- SigmoidFocalLoss (losses.py:11-46) ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ float powg(float x, float g) { return g == 2.f ? x * x : powf(x, g); }
+
+// one element for target t in {0, 1} (t = -1 is zero and handled by the caller), before the < 1e-5 clamp
+__device__ __forceinline__ float focal(float x, float t, float bw, float gamma) {
+    const float p = sigmoid(x);
+    const float fw = powg(t == 1.f ? 1.f - p : p, gamma);
+    const float bce = -(t * log_sigmoid(x)) * bw - ((1.f - t) * log_sigmoid(-x));
+    return fw * bce;
+}
+
+// its derivative in x, focal weight not detached (autograd on the reference expression)
+__device__ __forceinline__ float focal_grad(float x, float t, float bw, float gamma) {
+    const float p = sigmoid(x), q = 1.f - p;
+    if (t == 1.f) {
+        const float bce = -log_sigmoid(x) * bw;
+        const float dfw = gamma == 0.f ? 0.f : gamma * powg(q, gamma - 1.f) * (-p * q);
+        return dfw * bce + powg(q, gamma) * (-bw * q);
+    }
+    const float bce = -log_sigmoid(-x);
+    const float dfw = gamma == 0.f ? 0.f : gamma * powg(p, gamma - 1.f) * (p * q);
+    return dfw * bce + powg(p, gamma) * p;
+}
 
 // ---- the heatmap focal terms of CenterNet-style heads (KM3DHead._neg_loss, km3d_head.py:61-98) -----------------------------------------
 constexpr int kHmRec = 3;              // per-block partial: positive sum, negative sum, positive count

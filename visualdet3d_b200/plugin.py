@@ -117,6 +117,18 @@ def install_loss_into_reference():
     return head_loss
 
 
+def install_retinanet_loss_into_reference():
+    """Make the REFERENCE's RetinaNet head train with the native loss (`retina_loss.head_loss`): rebinds `RetinanetHead.loss` in
+    `visualDet3D.networks.heads.retinanet_head`, so the unmodified scripts/train.py (train_mono_detection) computes the 2-D detector's head
+    loss on the GPU path while the reference's own RetinaNet modules compute the features.  DETECTOR_DICT is left alone:
+    `install_retinanet_into_reference()` stays the inference swap.  Each call reads the head's num_clasess, loss_cfg, target_means /
+    target_stds and its focal loss's gamma and balance_weights.  Returns the installed function."""
+    from visualDet3D.networks.heads import retinanet_head as ref_head        # ImportError if the reference is not on sys.path
+    from .retina_loss import head_loss
+    ref_head.RetinanetHead.loss = head_loss
+    return head_loss
+
+
 def install_monoflex_loss_into_reference():
     """Make the REFERENCE's MonoFlex head train with the native loss (`monoflex_loss.head_loss`): rebinds `MonoFlexHead.loss` in
     `visualDet3D.networks.heads.monoflex_head`, so the unmodified scripts/train.py (train_rtm3d) computes MonoFlex's head loss on the GPU

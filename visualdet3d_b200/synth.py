@@ -159,6 +159,16 @@ def synth_head_outputs(B: int, N: int, C: int, seed: int = 0) -> Tuple[torch.Ten
     return torch.from_numpy(cls), torch.from_numpy(reg)
 
 
+def retina_head_outputs(B: int, N: int, C: int, seed: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Stand-ins for the RetinaNet head's outputs, for the loss tests: cls [B, N, C] logits on a 1/8 grid over [-6, 2] and reg [B, N, 4]
+    deltas on a 1/32 grid over [-1, 1] (decoded boxes mostly overlap their targets), float32 from a seeded numpy RandomState (the same
+    values on every machine)."""
+    rng = np.random.RandomState(seed)
+    cls = rng.randint(-48, 17, size=(B, N, C)).astype(np.float32) / 8
+    reg = rng.randint(-32, 33, size=(B, N, 4)).astype(np.float32) / 32
+    return torch.from_numpy(cls), torch.from_numpy(reg)
+
+
 def monoflex_head_outputs(B: int, C: int, H: int, W: int, seed: int = 0) -> dict:
     """Stand-ins for the MonoFlex head's nine output maps (fp32 NCHW), for the loss tests, from a seeded numpy RandomState (the same
     values on every machine).  hm logits lie on a 1/8 grid over [-6, 6], which keeps sigmoid well away from the focal loss's 0.99 / 0.01
