@@ -2,16 +2,11 @@
 reference loss (tests/golden/make_golden_disparity_loss.py): the loss within 1e-5 relative, the gradient within 1e-5 of its max |.| at the
 stored positions (the band and edge pixels included) and exactly zero outside the loss mask, bit-identical reruns and CUDA-graph replays,
 the launch counts, no volume-sized allocation in the forward, and a reference Stereo3D training step with the native losses installed."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from loss_harness import graph_replay_matches_eager, run_seam_worker
 from test_disparity_loss_cpu import CASES, FX, GEN
 from visualdet3d_b200 import _lib, disparity_loss
 
@@ -115,32 +110,11 @@ def test_cuda_graph_replay_bit_identical():
         loss.backward()
         return loss, x.grad
 
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        eager = [t.clone() for t in step()]
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        outs = step()
-    for _ in range(2):
-        g.replay()
-        torch.cuda.synchronize()
-        for a, b in zip(outs, eager):
-            assert torch.equal(a, b)
+    graph_replay_matches_eager(step)
 
 
 def test_reference_stereo3d_training_step():
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import refload
-    if not refload.available():
-        pytest.skip("no reference package (neither the reference tree nor oracle/_ref/visualDet3D)")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "workers", "stereo3d_loss_step.py")], capture_output=True, text=True,
-                       timeout=1200)
-    lines = [ln for ln in r.stdout.splitlines() if ln.startswith("SEAM_JSON ")]
-    assert r.returncode == 0 and lines, f"worker failed (rc {r.returncode}):\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}"
-    out = json.loads(lines[-1][len("SEAM_JSON "):])
-    print(out)
+    out = run_seam_worker("stereo3d_loss_step.py", timeout=1200)
     assert out["native_bound"] and out["same_params"] and out["disp_loss_ran"]
     assert out["cls_rel"] <= LOSS_RTOL and out["reg_rel"] <= LOSS_RTOL and out["disp_rel"] <= LOSS_RTOL
     assert out["depth_grad_err"] <= GRAD_TOL, out["depth_grad_worst"]

@@ -4,16 +4,11 @@ wherever the reference's are -- coor_loss and the hps / dim gradients within 1e-
 from a float64 restatement, which they are also checked against, and prob within 1e-4 (float64 overlap in the fixture) -- bit-identical
 reruns and CUDA-graph replays, the fixed launch count, the backward of a single term, NaN losses for an index outside the map, and a
 reference KM3DHead training step on the GPU with the reference's own compiled iou3d, with and without the native loss."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from loss_harness import graph_replay_matches_eager, run_seam_worker
 from test_km3d_loss_cpu import CASES, FX, GEN, case_inputs
 from visualdet3d_b200 import _lib, km3d_loss
 from visualdet3d_b200.km3d_loss import MAPS, TERMS, LossConfig
@@ -142,19 +137,7 @@ def test_cuda_graph_replay_bit_identical():
         loss.backward()
         return [loss] + [stats[k] for k in TERMS] + [out[k].grad for k, _ in MAPS]
 
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        eager = [t.clone() for t in step()]
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        outs = step()
-    for _ in range(2):
-        g.replay()
-        torch.cuda.synchronize()
-        for x, y in zip(outs, eager):
-            assert torch.equal(x, y)
+    graph_replay_matches_eager(step)
 
 
 def test_backward_of_a_single_term():
@@ -191,16 +174,7 @@ def test_index_outside_the_map_gives_nan(key):
 
 
 def test_reference_head_training_step():
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import refload
-    if not refload.available():
-        pytest.skip("no reference package (neither the reference tree nor oracle/_ref/visualDet3D)")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "workers", "km3d_loss_step.py")], capture_output=True, text=True,
-                       timeout=900)
-    lines = [ln for ln in r.stdout.splitlines() if ln.startswith("SEAM_JSON ")]
-    assert r.returncode == 0 and lines, f"worker failed (rc {r.returncode}):\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}"
-    out = json.loads(lines[-1][len("SEAM_JSON "):])
-    print(out)
+    out = run_seam_worker("km3d_loss_step.py")
     assert out["native_bound"] and out["reference_iou3d_kernel"] and out["same_params"] and out["n_grads"] >= 36
     # within 1e-5, plus twice the reference's own scatter between two draws of its solve jitter
     for k, v in out["loss_rel"].items():

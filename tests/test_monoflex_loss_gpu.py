@@ -2,16 +2,11 @@
 reference loss (tests/golden/make_golden_monoflex_loss.py): terms and total within 1e-5 relative, gradients within 1e-5 of each map's max
 |.| and zero wherever the reference's are, bit-identical reruns and CUDA-graph replays, the fixed launch count, NaN losses for an ind
 outside the map, and a reference MonoFlexHead training step with the native loss installed."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from loss_harness import graph_replay_matches_eager, run_seam_worker
 from test_monoflex_loss_cpu import CASES, FX, case_inputs
 from visualdet3d_b200 import _lib, monoflex_loss
 from visualdet3d_b200.monoflex_loss import MAPS, TERMS
@@ -89,19 +84,7 @@ def test_cuda_graph_replay_bit_identical():
         loss.backward()
         return [loss] + [stats[k] for k in TERMS] + [out[k].grad for k, _ in MAPS]
 
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        eager = [t.clone() for t in step()]
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        outs = step()
-    for _ in range(2):
-        g.replay()
-        torch.cuda.synchronize()
-        for x, y in zip(outs, eager):
-            assert torch.equal(x, y)
+    graph_replay_matches_eager(step)
 
 
 def test_backward_of_a_single_term():
@@ -129,16 +112,7 @@ def test_ind_outside_the_map_gives_nan():
 
 
 def test_reference_head_training_step():
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import refload
-    if not refload.available():
-        pytest.skip("no reference package (neither the reference tree nor oracle/_ref/visualDet3D)")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "workers", "monoflex_loss_step.py")], capture_output=True, text=True,
-                       timeout=900)
-    lines = [ln for ln in r.stdout.splitlines() if ln.startswith("SEAM_JSON ")]
-    assert r.returncode == 0 and lines, f"worker failed (rc {r.returncode}):\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}"
-    out = json.loads(lines[-1][len("SEAM_JSON "):])
-    print(out)
+    out = run_seam_worker("monoflex_loss_step.py")
     assert out["native_bound"] and out["same_params"] and out["n_grads"] >= 36
     assert out["loss_rel_max"] <= LOSS_RTOL, out["loss_rel"]
     assert out["grad_err_max"] <= GRAD_TOL, out["grad_err_worst"]

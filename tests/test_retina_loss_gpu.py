@@ -3,16 +3,11 @@ reference loss (tests/golden/make_golden_retina_loss.py): assignment and counts 
 within 1e-5 of each tensor's max |.| (plus the reference's own one-ulp spread where decoded boxes barely overlap) with the
 reference's exact zeros, the same bits at an odd annotation row count, bit-identical reruns and CUDA-graph replays, a fixed launch count,
 NaN for an out-of-range class, and reference training steps (head, and the whole detector) with the native loss installed."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from loss_harness import graph_replay_matches_eager, run_seam_worker
 from test_retina_loss_cpu import CASES, FX, case_inputs
 from visualdet3d_b200 import _lib, retina_loss
 
@@ -140,19 +135,7 @@ def test_cuda_graph_replay_bit_identical():
         (c + r).backward()
         return d["total_loss"], cls.grad, reg.grad
 
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        eager = [t.clone() for t in step()]
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        outs = step()
-    for _ in range(2):
-        g.replay()
-        torch.cuda.synchronize()
-        for x, y in zip(outs, eager):
-            assert torch.equal(x, y)
+    graph_replay_matches_eager(step)
 
 
 def test_out_of_range_class_gives_nan():
@@ -177,15 +160,7 @@ def test_no_positive_reg_loss_is_zero_tensor():
 
 
 def _worker(name, *args):
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import refload
-    if not refload.available():
-        pytest.skip("no reference package (neither the reference tree nor oracle/_ref/visualDet3D)")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "workers", name), *args], capture_output=True, text=True, timeout=900)
-    lines = [ln for ln in r.stdout.splitlines() if ln.startswith("SEAM_JSON ")]
-    assert r.returncode == 0 and lines, f"worker failed (rc {r.returncode}):\n{r.stdout[-3000:]}\n{r.stderr[-3000:]}"
-    out = json.loads(lines[-1][len("SEAM_JSON "):])
-    print(out)
+    out = run_seam_worker(name, *args)
     assert out["native_bound"] and out["same_params"] and out["n_grads"] > 1
     assert out["cls_rel"] <= LOSS_RTOL and out["reg_rel"] <= LOSS_RTOL and out["total_rel"] <= LOSS_RTOL
     assert out["grad_err_max"] <= GRAD_TOL, out["grad_err_worst"]

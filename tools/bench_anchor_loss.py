@@ -9,29 +9,20 @@ The reference arm needs the reference package (the reference tree or oracle/_ref
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+from bench_common import card, timed  # noqa: E402
 
 SHAPES = {"Stereo3D": dict(B=4, kind="Stereo3D"), "GroundAwareYolo3D": dict(B=8, kind="GroundAwareYolo3D")}
 H, W, M = 288, 1280, 8
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception as e:                                   # noqa: BLE001
-        q = f"nvidia-smi unavailable ({e})"
-    return q
 
 
 def annotations(B, C, seed=0):
@@ -74,26 +65,6 @@ def setup(name, ref_head_cls):
     N = anchors["anchors"].shape[1]
     cls, reg = synth.synth_head_outputs(B, N, C, seed=1)
     return head, hc.loss_cfg, anchors, annotations(B, C), P2, cls.cuda().requires_grad_(True), reg.cuda().requires_grad_(True)
-
-
-def timed(step, steps, warmup):
-    for _ in range(warmup):
-        step()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        step()
-    torch.cuda.synchronize()
-    ms = (time.perf_counter() - t0) * 1e3 / steps
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        step()
-        torch.cuda.synchronize()
-    names = [e.name for e in prof.events()]
-    launches = sum(("LaunchKernel" in n) or n in ("cudaMemsetAsync",) for n in names)
-    d2h = sum(n.startswith("Memcpy DtoH") for n in names)
-    syncs = sum(n in ("cudaStreamSynchronize", "cudaDeviceSynchronize") for n in names)
-    return dict(ms_per_step=round(ms, 4), launches=launches, d2h_copies=d2h, host_syncs=syncs - 1)    # minus the profiler's own
 
 
 def main():

@@ -23,7 +23,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
-from bench_monoflex_loss import card, timed  # noqa: E402
+from bench_common import card, timed  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12        # H100 SXM5 80 GB HBM3
 

@@ -21,7 +21,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
-from bench_monoflex_loss import card, timed  # noqa: E402
+from bench_common import card, timed  # noqa: E402
 
 
 def main():

@@ -10,23 +10,14 @@ card's name and power limit come from the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import torch  # noqa: E402
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True,
-                            timeout=30).stdout.strip()
-    except Exception:
-        pl = "unknown"
-    return name, pl
+from bench_common import card  # noqa: E402
 
 
 def head_flops(det, hws, B):
@@ -63,7 +54,7 @@ def main():
     from visualdet3d_b200.detectors import build_synthetic_retinanet
     det, _, _ = build_synthetic_retinanet(seed=0)
     det = det.cuda().eval()
-    name, power = card()
+    gpu = card()
     for B in [int(v) for v in a.batches.split(",")]:
         img, _ = synth.synth_mono_inputs(B, a.H, a.W, seed=1)
         img = img.cuda()
@@ -96,7 +87,7 @@ def main():
         fl = head_flops(det, hws, B)
         print(json.dumps({"metric": "retinanet_images_per_sec", "H": a.H, "W": a.W, "batch": B, "value": B * 1000.0 / step_ms,
                           "ms_per_step": step_ms, "launches_per_step": launches, "stage_ms": st, "head_gflop": fl / 1e9,
-                          "head_tflops": fl / (st["head"] * 1e-3) / 1e12, "gpu": name, "power_limit": power, "steps": a.steps,
+                          "head_tflops": fl / (st["head"] * 1e-3) / 1e12, "card": gpu, "steps": a.steps,
                           "warmup": a.warmup}))
         # one head layer: one multi-level launch vs level-by-level launches of the same layer, alternating
         from visualdet3d_b200 import engine as E
@@ -138,7 +129,7 @@ def main():
         lf = 2 * 9 * layer.Cin * layer.Cout * B * sum(h * w for h, w in hws)
         print(json.dumps({"metric": "retinanet_head_layer_grouped_vs_per_level", "H": a.H, "W": a.W, "batch": B, "grouped_us": tg * 1e3,
                           "per_level_us": tp * 1e3, "grouped_tflops": lf / (tg * 1e-3) / 1e12, "per_level_tflops": lf / (tp * 1e-3) / 1e12,
-                          "levels": hws, "gpu": name, "power_limit": power, "reps": a.reps}))
+                          "levels": hws, "card": gpu, "reps": a.reps}))
 
 
 if __name__ == "__main__":

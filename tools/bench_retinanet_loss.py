@@ -18,7 +18,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
-from bench_anchor_loss import card, timed  # noqa: E402
+from bench_common import card, timed  # noqa: E402
 
 B, H, W, C, M = 8, 288, 1280, 3, 16
 

@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .loss_common import as_config, cached_on, check, grad_out_pair, stream, workspace
 
 N_REG = 12          # regression outputs per anchor
 N_TERMS = 13        # the 12 smooth-L1 terms and the alpha BCE: the length regression_weight must have
@@ -95,24 +96,17 @@ class LossConfig:
                                               1.0 / a, 0.5 * a, 0.5 / a, *bw, *self.regression_weight], dtype=np.float32))
 
 
-def _check_cuda(t: torch.Tensor, name: str, dtype=torch.float32) -> None:
-    if not t.is_cuda:
-        raise RuntimeError(f"anchor loss: {name} must be a CUDA tensor (there is no CPU path)")
-    if t.dtype != dtype:
-        raise RuntimeError(f"anchor loss: {name} must be {dtype}, got {t.dtype}")
-
-
 def _inputs(cls_scores, reg_preds, anchors: Mapping, annotations, cfg: LossConfig):
-    _check_cuda(cls_scores, "cls_scores")
-    _check_cuda(reg_preds, "reg_preds")
+    check(cls_scores, "anchor loss", "cls_scores", torch.float32)
+    check(reg_preds, "anchor loss", "reg_preds", torch.float32)
     anchor = anchors["anchors"][0].contiguous()
     mask = anchors["mask"].contiguous()
     mean_std = anchors["anchor_mean_std_3d"].contiguous()
     ann = annotations.contiguous()
-    _check_cuda(anchor, "anchors['anchors']")
-    _check_cuda(mask, "anchors['mask']", torch.bool)
-    _check_cuda(mean_std, "anchors['anchor_mean_std_3d']")
-    _check_cuda(ann, "annotations")
+    check(anchor, "anchor loss", "anchors['anchors']", torch.float32)
+    check(mask, "anchor loss", "anchors['mask']", torch.bool)
+    check(mean_std, "anchor loss", "anchors['anchor_mean_std_3d']", torch.float32)
+    check(ann, "anchor loss", "annotations", torch.float32)
     B, N, C1 = cls_scores.shape
     C = cfg.num_classes
     if C1 != C + 1:
@@ -131,11 +125,7 @@ def _forward(cls_scores, reg_preds, anchor, mask, mean_std, ann, cfg: LossConfig
     B, N, _ = cls_scores.shape
     M = ann.shape[1]
     dev = cls_scores.device
-    lib = _lib.load()
-    ws_bytes = int(lib.vd3d_anchor_loss_workspace_bytes(B, N, M))
-    if ws_bytes < 0:
-        raise _lib.Vd3dError(f"vd3d_anchor_loss_workspace_bytes failed ({ws_bytes}): {lib.vd3d_last_error().decode()}")
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    ws, ws_bytes = workspace("vd3d_anchor_loss_workspace_bytes", B, N, M, device=dev)
     assign = torch.empty(B, N, dtype=torch.int32, device=dev)
     counts = torch.empty(B, 3, dtype=torch.int32, device=dev)
     factors = torch.empty(B, 2, dtype=torch.float32, device=dev)
@@ -144,7 +134,7 @@ def _forward(cls_scores, reg_preds, anchor, mask, mean_std, ann, cfg: LossConfig
     _lib.call("vd3d_anchor_loss_forward", cls_scores.data_ptr(), reg_preds.data_ptr(), anchor.data_ptr(), mask.data_ptr(),
               mean_std.data_ptr(), ann.data_ptr(), B, N, cfg.num_classes, M, params.ctypes.data, int(cfg.match_low_quality),
               int(cfg.gt_max_assign_all), ws.data_ptr(), ws_bytes, assign.data_ptr(), counts.data_ptr(), factors.data_ptr(),
-              cls_loss.data_ptr(), reg_loss.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+              cls_loss.data_ptr(), reg_loss.data_ptr(), stream(cls_scores))
     return cls_loss, reg_loss, assign, counts, factors
 
 
@@ -162,20 +152,14 @@ class AnchorHeadLoss(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_cls, g_reg):
         cls_scores, reg_preds, anchor, mean_std, ann, assign, factors = ctx.saved_tensors
-        dev = cls_scores.device
-        zero = torch.zeros(1, dtype=torch.float32, device=dev)
-        grad_out = torch.cat([(zero if g_cls is None else g_cls.reshape(1)), (zero if g_reg is None else g_reg.reshape(1))]).float()
+        grad_out = grad_out_pair(g_cls, g_reg, cls_scores.device)
         B, N, C1 = cls_scores.shape
         grad_cls = torch.empty_like(cls_scores)
         grad_reg = torch.empty_like(reg_preds)
         _lib.call("vd3d_anchor_loss_backward", cls_scores.data_ptr(), reg_preds.data_ptr(), anchor.data_ptr(), mean_std.data_ptr(),
                   ann.data_ptr(), B, N, ctx.cfg.num_classes, ann.shape[1], ctx.params.ctypes.data, assign.data_ptr(), factors.data_ptr(),
-                  grad_out.data_ptr(), grad_cls.data_ptr(), grad_reg.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                  grad_out.data_ptr(), grad_cls.data_ptr(), grad_reg.data_ptr(), stream(cls_scores))
         return grad_cls, grad_reg, None, None, None, None, None
-
-
-def _config(cfg, num_classes: int) -> LossConfig:
-    return cfg if isinstance(cfg, LossConfig) else LossConfig.from_loss_cfg(cfg, num_classes)
 
 
 def anchor3d_head_loss(cls_scores: torch.Tensor, reg_preds: torch.Tensor, anchors: Mapping, annotations: torch.Tensor, cfg):
@@ -183,7 +167,7 @@ def anchor3d_head_loss(cls_scores: torch.Tensor, reg_preds: torch.Tensor, anchor
     anchor_mean_std_3d [N,C,6,2]); annotations [B,M,12] compound_annotation rows (class -1 = padding); cfg: the head's loss_cfg
     mapping (num_classes = cls_scores' last dimension - 1) or a LossConfig.  Returns (cls_loss [1], reg_loss [1],
     dict(cls_loss, reg_loss, total_loss)), differentiable in cls_scores and reg_preds."""
-    cfg = _config(cfg, cls_scores.shape[-1] - 1)
+    cfg = as_config(LossConfig, cfg, cls_scores.shape[-1] - 1)
     cls_scores, reg_preds, anchor, mask, mean_std, ann = _inputs(cls_scores, reg_preds, anchors, annotations, cfg)
     cls_loss, reg_loss = AnchorHeadLoss.apply(cls_scores, reg_preds, anchor, mask, mean_std, ann, cfg)
     return cls_loss, reg_loss, dict(cls_loss=cls_loss, reg_loss=reg_loss, total_loss=cls_loss + reg_loss)
@@ -193,7 +177,7 @@ def assignment(cls_scores, reg_preds, anchors: Mapping, annotations, cfg):
     """The forward's anchor assignment and counts (same arguments as anchor3d_head_loss): assigned_gt_inds [B, N] int32 (1-based among
     the image's valid annotation rows, 0 negative, -1 ignored or image without ground truth, -2 outside the mask) and counts [B, 3]
     int32 (positives assigned, positives kept by the prior's z_mean > 0 selection, negatives)."""
-    cfg = _config(cfg, cls_scores.shape[-1] - 1)
+    cfg = as_config(LossConfig, cfg, cls_scores.shape[-1] - 1)
     with torch.no_grad():
         _, _, assign, counts, _ = _forward(*_inputs(cls_scores, reg_preds, anchors, annotations, cfg), cfg, cfg.params())
     return assign, counts
@@ -204,11 +188,7 @@ def _head_config(head) -> LossConfig:
     is replaced or written in place (its storage or version counter changes)."""
     key = tuple((t.data_ptr(), t._version) for t in (head.balance_weights, head.regression_weight)) + (
         head.num_classes, head.focal_loss_gamma, head.decode_before_loss, id(head.loss_cfg), head.loss_bbox.alpha)
-    cached = head.__dict__.get("_vd3d_loss_config")
-    if cached is None or cached[0] != key:
-        cached = (key, LossConfig.from_head(head))
-        head.__dict__["_vd3d_loss_config"] = cached
-    return cached[1]
+    return cached_on(head, "_vd3d_loss_config", key, lambda: LossConfig.from_head(head))
 
 
 def head_loss(self, cls_scores, reg_preds, anchors, annotations, P2s):

@@ -29,7 +29,6 @@ using vd3d::sigmoid;
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
 constexpr int kGtCols = 12;           // compound_annotation: x1 y1 x2 y2, class, cx cy z, w h l, alpha
 constexpr int kReg = 12;              // regression outputs per anchor
 constexpr int kTerms = 13;            // 12 smooth-L1 terms + the alpha BCE
@@ -126,7 +125,7 @@ __global__ void __launch_bounds__(kThreads) assign_loss_kernel(const float* __re
                                                                const float* __restrict__ mean_std, const float* __restrict__ ann,
                                                                const unsigned long long* __restrict__ gt_key, Cfg cfg,
                                                                int* __restrict__ assign, double* __restrict__ partial) {
-    __shared__ double s_red[kWarps][kRec];
+    __shared__ double s_red[kThreads / 32][kRec];
     const int b = blockIdx.y;
     const GtShared s = load_image(ann, gt_key, cfg, b);
     const int n = blockIdx.x * kThreads + threadIdx.x;
@@ -175,18 +174,8 @@ __global__ void __launch_bounds__(kThreads) assign_loss_kernel(const float* __re
         }
         assign[bn] = r;
     }
-    // block sum in a fixed order: warp tree, then warps in index order
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kRec; ++k) {
-        double v = acc[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][k] = v;
-    }
-    __syncthreads();
+    double v = vd3d::block_partial<kThreads, kRec>(acc, s_red);
     if (threadIdx.x < kRec) {
-        double v = 0.0;
-        for (int w = 0; w < kWarps; ++w) v += s_red[w][threadIdx.x];
         if (threadIdx.x == R_NGT) v = s.ng;
         partial[((size_t)b * cfg.tiles + blockIdx.x) * kRec + threadIdx.x] = v;
     }
@@ -294,19 +283,6 @@ __global__ void __launch_bounds__(kThreads) backward_kernel(const float* __restr
 size_t gt_smem_bytes(int M) { return (size_t)M * (kGtCols + 3) * sizeof(float) + 16; }
 size_t iou_smem_bytes(int M) { return (size_t)M * kGtCols * sizeof(float) + ((M + 1) & ~1) * sizeof(int) + (size_t)M * 8; }
 
-struct Layout {
-    size_t keys, partial, total;
-};
-
-Layout layout(int B, int N, int M) {
-    Layout L;
-    const size_t tiles = (size_t)cdiv(N, kThreads);
-    L.keys = 0;
-    L.partial = ((size_t)B * M * 8 + 255) & ~(size_t)255;
-    L.total = L.partial + (size_t)B * tiles * kRec * sizeof(double);
-    return L;
-}
-
 int make_cfg(int B, int N, int C, int M, const float* params, int match_low_quality, int gt_max_assign_all, Cfg& cfg) {
     VD3D_REQUIRE(B > 0 && N > 0 && M >= 0 && M <= kMaxGt, "anchor_loss: bad sizes B=%d N=%d M=%d (M <= %d)", B, N, M, kMaxGt);
     VD3D_REQUIRE(C >= 1 && C <= kMaxClasses, "anchor_loss: %d classes, 1..%d supported", C, kMaxClasses);
@@ -324,11 +300,7 @@ int make_cfg(int B, int N, int C, int M, const float* params, int match_low_qual
 }  // namespace
 
 extern "C" long long vd3d_anchor_loss_workspace_bytes(int B, int N, int M) {
-    if (B <= 0 || N <= 0 || M < 0 || M > kMaxGt) {
-        vd3d::set_error("anchor_loss_workspace_bytes: bad sizes B=%d N=%d M=%d", B, N, M);
-        return VD3D_EINVAL;
-    }
-    return (long long)layout(B, N, M).total;
+    return vd3d::assign_workspace_bytes<kThreads, kRec>("anchor_loss", B, N, M, kMaxGt);
 }
 
 extern "C" int vd3d_anchor_loss_forward(const float* cls, const float* reg, const float* anchors, const unsigned char* mask,
@@ -341,7 +313,7 @@ extern "C" int vd3d_anchor_loss_forward(const float* cls, const float* reg, cons
     VD3D_REQUIRE(cls && reg && anchors && mask && mean_std && (M == 0 || ann) && workspace && assign && counts && factors && cls_loss && reg_loss,
                  "anchor_loss_forward: null pointer");
     VD3D_REQUIRE(((uintptr_t)anchors & 15) == 0, "anchor_loss_forward: anchors must be 16-byte aligned");
-    const Layout L = layout(B, N, M);
+    const vd3d::AssignLayout L = vd3d::assign_layout<kThreads, kRec>(B, N, M);
     VD3D_REQUIRE((size_t)workspace_bytes >= L.total, "anchor_loss_forward: workspace of %lld bytes, %zu needed", workspace_bytes, L.total);
     char* ws = static_cast<char*>(workspace);
     auto* keys = reinterpret_cast<unsigned long long*>(ws + L.keys);

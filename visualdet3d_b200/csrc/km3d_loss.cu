@@ -35,6 +35,7 @@ using vd3d::kHmRec;
 using vd3d::log_sigmoid;
 using vd3d::sigmoid;
 using vd3d::sign0;
+using vd3d::warp_sum;
 
 namespace {
 
@@ -334,28 +335,11 @@ __global__ void __launch_bounds__(kRowThreads) rows_kernel(Args a, double* __res
             rec[R_BAD] = 1.f;
         }
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int i = 0; i < kRec; ++i) {
-        double v = rec[i];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][i] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kRec) {
-        double v = 0.0;
-        for (int w = 0; w < kRowThreads / 32; ++w) v += s_red[w][threadIdx.x];
-        partial[(size_t)b * kRec + threadIdx.x] = v;
-    }
+    const double v = vd3d::block_partial<kRowThreads, kRec>(rec, s_red);
+    if (threadIdx.x < kRec) partial[(size_t)b * kRec + threadIdx.x] = v;
 }
 
-// ---- combine: one warp; sums in a fixed order (lane-strided, then a shuffle tree) ------------------------------------------------
-__device__ double warp_sum(const double* p, int n, int stride, int lane) {
-    double v = 0.0;
-    for (int i = lane; i < n; i += 32) v += p[(size_t)i * stride];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    return __shfl_sync(0xffffffffu, v, 0);
-}
+// ---- combine: one warp; sums in a fixed order (vd3d::warp_sum: lane-strided, then a shuffle tree) -----------------------------
 
 // _neg_loss from its summed partials: the term and its factor (the num_pos == 0 choice made here)
 __device__ __forceinline__ float focal_term(const double* hv, float& factor) {

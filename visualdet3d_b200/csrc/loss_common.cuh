@@ -2,7 +2,37 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "common.cuh"
+
 namespace vd3d {
+
+// ---- fixed-order reductions: no float atomics, so two runs give the same bits -------------------------------------------------------
+
+// One block's sums of the kRec per-thread accumulators (float or double, summed in double): a shuffle tree per warp, then the warps in
+// index order.  s_red: [kThreads / 32][kRec] of shared scratch.  Called by the whole block; thread k < kRec gets slot k's sum (the others 0).
+template <int kThreads, int kRec, class T>
+__device__ __forceinline__ double block_partial(const T (&acc)[kRec], double (*s_red)[kRec]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < kRec; ++k) {
+        double v = acc[k];
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+        if (lane == 0) s_red[warp][k] = v;
+    }
+    __syncthreads();
+    double v = 0.0;
+    if (threadIdx.x < kRec)
+        for (int w = 0; w < kThreads / 32; ++w) v += s_red[w][threadIdx.x];
+    return v;
+}
+
+// The sum of p[i * stride], i < n, over one warp: lane-strided, then a shuffle tree; every lane gets it.
+__device__ inline double warp_sum(const double* p, int n, int stride, int lane) {
+    double v = 0.0;
+    for (int i = lane; i < n; i += 32) v += p[(size_t)i * stride];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    return __shfl_sync(0xffffffffu, v, 0);
+}
 
 // torch.nn.functional.logsigmoid, in its overflow-free form
 __device__ __forceinline__ float log_sigmoid(float x) { return fminf(x, 0.f) - log1pf(expf(-fabsf(x))); }
@@ -91,6 +121,32 @@ __device__ __forceinline__ int assign_anchor(const float* a, int n, int ng, cons
     return r;
 }
 
+// Workspace of the assigning losses: each image's M best keys (fold_gt_keys; zeroed before the IoU pass), then the assignment pass's
+// [B][tiles][kRec] double partials at the next 256-byte boundary, tiles = ceil(N / kThreads).
+struct AssignLayout {
+    size_t keys, partial, total;
+};
+
+template <int kThreads, int kRec>
+AssignLayout assign_layout(int B, int N, int M) {
+    AssignLayout L;
+    const size_t tiles = (size_t)cdiv(N, kThreads);
+    L.keys = 0;
+    L.partial = ((size_t)B * M * 8 + 255) & ~(size_t)255;
+    L.total = L.partial + (size_t)B * tiles * kRec * sizeof(double);
+    return L;
+}
+
+// vd3d_<who>_workspace_bytes: the layout's size, or VD3D_EINVAL for sizes the kernels do not take (at most max_gt rows per image)
+template <int kThreads, int kRec>
+long long assign_workspace_bytes(const char* who, int B, int N, int M, int max_gt) {
+    if (B <= 0 || N <= 0 || M < 0 || M > max_gt) {
+        set_error("%s_workspace_bytes: bad sizes B=%d N=%d M=%d", who, B, N, M);
+        return VD3D_EINVAL;
+    }
+    return (long long)assign_layout<kThreads, kRec>(B, N, M).total;
+}
+
 // ---- SigmoidFocalLoss (losses.py:11-46) ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ float powg(float x, float g) { return g == 2.f ? x * x : powf(x, g); }
 
@@ -154,19 +210,8 @@ __device__ __forceinline__ void hm_block_partial(const float* __restrict__ hm, c
         acc[1] += neg;
         acc[2] += g == 1.f ? 1.0 : 0.0;
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kHmRec; ++k) {
-        double v = acc[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kHmRec) {
-        double v = 0.0;
-        for (int w = 0; w < kThreads / 32; ++w) v += s_red[w][threadIdx.x];
-        partial[(size_t)block * kHmRec + threadIdx.x] = v;
-    }
+    const double v = block_partial<kThreads, kHmRec>(acc, s_red);
+    if (threadIdx.x < kHmRec) partial[(size_t)block * kHmRec + threadIdx.x] = v;
 }
 
 // ---- one object row of KM3DHead._RegWeightedL1Loss (km3d_head.py:100-115) -------------------------------------------------------------

@@ -23,6 +23,7 @@ using vd3d::hm_grad;
 using vd3d::kHmRec;
 using vd3d::log_sigmoid;
 using vd3d::sigmoid;
+using vd3d::warp_sum;
 
 namespace {
 
@@ -273,28 +274,11 @@ __global__ void __launch_bounds__(kRowThreads) rows_kernel(Args a, double* __res
 #pragma unroll
     for (int i = 0; i < kRec; ++i) rec[i] = 0.f;
     if (k < a.K) row_eval<false>(a, b, k, nullptr, rec, nullptr);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int i = 0; i < kRec; ++i) {
-        double v = rec[i];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][i] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kRec) {
-        double v = 0.0;
-        for (int w = 0; w < kRowThreads / 32; ++w) v += s_red[w][threadIdx.x];
-        partial[(size_t)b * kRec + threadIdx.x] = v;
-    }
+    const double v = vd3d::block_partial<kRowThreads, kRec>(rec, s_red);
+    if (threadIdx.x < kRec) partial[(size_t)b * kRec + threadIdx.x] = v;
 }
 
-// ---- combine: one warp; sums in a fixed order (lane-strided, then a shuffle tree) ------------------------------------------------
-__device__ double warp_sum(const double* p, int n, int stride, int lane) {
-    double v = 0.0;
-    for (int i = lane; i < n; i += 32) v += p[(size_t)i * stride];
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    return __shfl_sync(0xffffffffu, v, 0);
-}
+// ---- combine: one warp; sums in a fixed order (vd3d::warp_sum: lane-strided, then a shuffle tree) -----------------------------
 
 __global__ void combine_kernel(const double* __restrict__ hm_part, const double* __restrict__ row_part, Args a, float* __restrict__ terms,
                                float* __restrict__ total, float* __restrict__ factors) {

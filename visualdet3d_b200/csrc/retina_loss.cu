@@ -28,7 +28,6 @@ using vd3d::load_gts;
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
 constexpr int kGtCols = 5;            // the annotation columns the loss reads: x1 y1 x2 y2, class
 constexpr int kMaxClasses = 64;
 constexpr int kMaxGt = 512;
@@ -161,7 +160,7 @@ __global__ void __launch_bounds__(kThreads) assign_loss_kernel(const float* __re
                                                                const float* __restrict__ anchors, const float* __restrict__ ann,
                                                                const unsigned long long* __restrict__ gt_key, Cfg cfg,
                                                                int* __restrict__ assign, double* __restrict__ partial) {
-    __shared__ double s_red[kWarps][kRec];
+    __shared__ double s_red[kThreads / 32][kRec];
     const int b = blockIdx.y;
     const GtShared s = load_image(ann, gt_key, cfg, b);
     const int n = blockIdx.x * kThreads + threadIdx.x;
@@ -195,18 +194,8 @@ __global__ void __launch_bounds__(kThreads) assign_loss_kernel(const float* __re
         }
         assign[bn] = r;
     }
-    // block sum in a fixed order: warp tree, then warps in index order
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kRec; ++k) {
-        double v = acc[k];
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][k] = v;
-    }
-    __syncthreads();
+    double v = vd3d::block_partial<kThreads, kRec>(acc, s_red);
     if (threadIdx.x < kRec) {
-        double v = 0.0;
-        for (int w = 0; w < kWarps; ++w) v += s_red[w][threadIdx.x];
         partial[((size_t)b * cfg.tiles + blockIdx.x) * kRec + threadIdx.x] = v;
     }
 }
@@ -292,19 +281,6 @@ __global__ void __launch_bounds__(kThreads) backward_kernel(const float* __restr
 size_t gt_smem_bytes(int M) { return (size_t)M * (kGtCols + 3) * sizeof(float) + 16; }
 size_t iou_smem_bytes(int M) { return (size_t)M * 8 + (size_t)M * kGtCols * sizeof(float) + (size_t)M * sizeof(int); }
 
-struct Layout {
-    size_t keys, partial, total;
-};
-
-Layout layout(int B, int N, int M) {
-    Layout L;
-    const size_t tiles = (size_t)cdiv(N, kThreads);
-    L.keys = 0;
-    L.partial = ((size_t)B * M * 8 + 255) & ~(size_t)255;
-    L.total = L.partial + (size_t)B * tiles * kRec * sizeof(double);
-    return L;
-}
-
 // params: fg, bg, min_iou, gamma, target_means[4], target_stds[4], the balance weight of each class
 int make_cfg(int B, int N, int C, int M, int K, const float* params, int match_low_quality, int gt_max_assign_all, Cfg& cfg) {
     VD3D_REQUIRE(B > 0 && N > 0 && M >= 0 && M <= kMaxGt && K >= kGtCols, "retina_loss: bad sizes B=%d N=%d M=%d K=%d (M <= %d, K >= %d)",
@@ -326,11 +302,7 @@ int make_cfg(int B, int N, int C, int M, int K, const float* params, int match_l
 }  // namespace
 
 extern "C" long long vd3d_retina_loss_workspace_bytes(int B, int N, int M) {
-    if (B <= 0 || N <= 0 || M < 0 || M > kMaxGt) {
-        vd3d::set_error("retina_loss_workspace_bytes: bad sizes B=%d N=%d M=%d", B, N, M);
-        return VD3D_EINVAL;
-    }
-    return (long long)layout(B, N, M).total;
+    return vd3d::assign_workspace_bytes<kThreads, kRec>("retina_loss", B, N, M, kMaxGt);
 }
 
 extern "C" int vd3d_retina_loss_forward(const float* cls, const float* reg, const float* anchors, const float* ann, int B, int N, int C,
@@ -343,7 +315,7 @@ extern "C" int vd3d_retina_loss_forward(const float* cls, const float* reg, cons
     VD3D_REQUIRE(cls && reg && anchors && (M == 0 || ann) && workspace && assign && counts && scale && cls_loss && reg_loss,
                  "retina_loss_forward: null pointer");
     VD3D_REQUIRE(((uintptr_t)anchors & 15) == 0, "retina_loss_forward: anchors must be 16-byte aligned");
-    const Layout L = layout(B, N, M);
+    const vd3d::AssignLayout L = vd3d::assign_layout<kThreads, kRec>(B, N, M);
     VD3D_REQUIRE((size_t)workspace_bytes >= L.total, "retina_loss_forward: workspace of %lld bytes, %zu needed", workspace_bytes, L.total);
     char* ws = static_cast<char*>(workspace);
     auto* keys = reinterpret_cast<unsigned long long*>(ws + L.keys);

@@ -19,6 +19,7 @@ from __future__ import annotations
 import torch
 
 from . import _lib
+from .loss_common import check, stream, workspace
 
 MAX_DISP_LIMIT = 1024       # csrc/disparity_loss.cu keeps a table of D + 1 floats per block
 
@@ -61,12 +62,11 @@ def _inputs(est_cost, gt_disp, max_disp):
     if tuple(label.shape) != (B, H, W):
         raise ValueError(f"disparity loss: gt_disp {tuple(gt_disp.shape)} does not match est_cost's B, H, W = {(B, H, W)} (no rescaled "
                          "label is supported)")
-    for name, t in (("est_cost", est_cost), ("gt_disp", gt_disp)):
+    for name, t in (("est_cost", est_cost), ("gt_disp", gt_disp)):             # both dtypes before either device
         if t.dtype != torch.float32:
             raise RuntimeError(f"disparity loss: {name} must be float32, got {t.dtype}")
     for name, t in (("est_cost", est_cost), ("gt_disp", gt_disp)):
-        if not t.is_cuda:
-            raise RuntimeError(f"disparity loss: {name} must be a CUDA tensor (there is no CPU path)")
+        check(t, "disparity loss", name, torch.float32)
     if est_cost.device != gt_disp.device:
         raise RuntimeError(f"disparity loss: est_cost on {est_cost.device}, gt_disp on {gt_disp.device}")
     return est_cost, label
@@ -79,15 +79,11 @@ class DisparityLossFn(torch.autograd.Function):
     def forward(ctx, cost, label):
         cost, label = cost.contiguous(), label.contiguous()
         B, D, H, W = cost.shape
-        lib = _lib.load()
-        ws_bytes = int(lib.vd3d_disparity_loss_workspace_bytes(B, D, H, W))
-        if ws_bytes < 0:
-            raise _lib.Vd3dError(f"vd3d_disparity_loss_workspace_bytes failed ({ws_bytes}): {lib.vd3d_last_error().decode()}")
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=cost.device)
+        ws, ws_bytes = workspace("vd3d_disparity_loss_workspace_bytes", B, D, H, W, device=cost.device)
         lse = torch.empty((B, H, W), dtype=torch.float32, device=cost.device)
         loss = torch.empty((), dtype=torch.float32, device=cost.device)
         _lib.call("vd3d_disparity_loss_forward", cost.data_ptr(), label.data_ptr(), B, D, H, W, ws.data_ptr(), ws_bytes, lse.data_ptr(),
-                  loss.data_ptr(), torch.cuda.current_stream(cost.device).cuda_stream)
+                  loss.data_ptr(), stream(cost))
         ctx.save_for_backward(cost, label, lse)
         return loss
 
@@ -98,7 +94,7 @@ class DisparityLossFn(torch.autograd.Function):
         g = g.float().contiguous()
         grad = torch.empty_like(cost)
         _lib.call("vd3d_disparity_loss_backward", cost.data_ptr(), label.data_ptr(), lse.data_ptr(), B, D, H, W, g.data_ptr(),
-                  grad.data_ptr(), torch.cuda.current_stream(cost.device).cuda_stream)
+                  grad.data_ptr(), stream(cost))
         return grad, None
 
 

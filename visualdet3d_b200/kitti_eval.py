@@ -16,6 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .loss_common import workspace
 
 # eval.py:35-38 / 730-739: CLASS_NAMES of clean_data (index 5 is 'car' again) and class_to_name of the printed header
 CLASS_TO_NAME = {0: 'Car', 1: 'Pedestrian', 2: 'Cyclist', 3: 'Van', 4: 'Person_sitting', 5: 'car', 6: 'tractor', 7: 'trailer'}
@@ -109,11 +110,9 @@ class DeviceEval:
         self.offs = np.stack([_offsets(self.ng), _offsets(self.nd), _offsets(self.ng * self.nd), _offsets((self.nd + 31) // 32)])
         self.sizes = (n_img,) + tuple(int(x) for x in self.offs[:, -1])          # n_img, n_gt, n_dt, n_pairs, n_words
         self.n_cls, self.compute_aos = n_cls, bool(compute_aos)
-        lib = _lib.load()
-        self.ws_bytes = int(lib.vd3d_kitti_eval_workspace_bytes(n_img, self.sizes[1], self.sizes[2], self.sizes[4], n_cls))
-        if self.ws_bytes < 0:
-            raise _lib.Vd3dError(f"vd3d_kitti_eval_workspace_bytes failed ({self.ws_bytes}): {lib.vd3d_last_error().decode()}")
         self.dev = dev = torch.device("cuda", torch.cuda.current_device())
+        self.ws, self.ws_bytes = workspace("vd3d_kitti_eval_workspace_bytes", n_img, self.sizes[1], self.sizes[2], self.sizes[4], n_cls,
+                                           device=dev)
         self.gt = torch.from_numpy(_pack(gt_annos, False)).to(dev)
         self.dt = torch.from_numpy(_pack(dt_annos, True)).to(dev)
         self.offs_d = torch.from_numpy(self.offs).to(dev)
@@ -126,7 +125,6 @@ class DeviceEval:
         self.orientation = torch.zeros(n_cls * 6 * N_SAMPLE_PTS, **f64)
         self.thresholds = torch.empty(n_cfg * N_SAMPLE_PTS, **f64)
         self.n_thresh = torch.empty(n_cfg, dtype=torch.int32, device=dev)
-        self.ws = torch.empty(max(self.ws_bytes, 1), dtype=torch.uint8, device=dev)
 
     def run(self) -> "DeviceEval":
         n_img, n_gt, n_dt, n_pairs, n_words = self.sizes

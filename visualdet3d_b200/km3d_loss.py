@@ -18,7 +18,6 @@ row's own pair instead of the diagonal of a (B*K) x (B*K) IoU matrix.
 """
 from __future__ import annotations
 
-import ctypes
 from dataclasses import dataclass
 from typing import Mapping
 
@@ -26,13 +25,15 @@ import numpy as np
 import torch
 
 from . import _lib
+from .loss_common import as_config, map_inputs, ptr_array, stream, workspace
 
 MAPS = (("hm", None), ("wh", 2), ("hps", 18), ("rot", 8), ("dim", 3), ("prob", 1), ("reg", 2), ("hm_hp", 9), ("hp_offset", 2))
 TERMS = ("hm_loss", "hp_loss", "hm_hp_loss", "hp_offset_loss", "wh_loss", "off_loss", "dim_loss", "rot_loss", "prob_loss", "coor_loss",
          "box_score")
 MAX_ROWS = 128
 NUM_JOINTS = 9
-# annotation key -> (dtypes accepted, trailing shape after [B, rows], rows: K or K*9); hm / hm_hp are [B, C, H, W] like the output
+_HM_TARGETS = (("hm", None), ("hm_hp", NUM_JOINTS))        # [B, channels (None: C), H, W] like the output
+# annotation key -> (dtypes accepted, trailing shape after [B, rows], rows per object: 1 or 9)
 _TARGETS = (("ind", (torch.int64,), (), 1), ("reg_mask", (torch.uint8, torch.bool), (), 1), ("hps", (torch.float32,), (18,), 1),
             ("hps_mask", (torch.uint8, torch.bool), (18,), 1), ("dep", (torch.float32,), (1,), 1), ("rotbin", (torch.int64,), (2,), 1),
             ("rotres", (torch.float32,), (2,), 1), ("wh", (torch.float32,), (2,), 1), ("dim", (torch.float32,), (3,), 1),
@@ -72,74 +73,17 @@ class LossConfig:
         return 1.0
 
 
-def _check(t: torch.Tensor, name: str, dtypes) -> None:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise RuntimeError(f"km3d loss: {name} must be a CUDA tensor (there is no CPU path)")
-    if t.dtype not in dtypes:
-        raise RuntimeError(f"km3d loss: {name} must be {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
-
-
-def _inputs(output: Mapping, annotations: Mapping, P2: torch.Tensor):
-    """Validated, contiguous (maps, targets, sizes); raises before any launch."""
-    maps = []
-    for name, ch in MAPS:
-        t = output[name]
-        _check(t, f"output['{name}']", (torch.float32,))
-        if t.dim() != 4:
-            raise ValueError(f"km3d loss: output['{name}'] must be [B, C, H, W], got {tuple(t.shape)}")
-        if ch is not None and t.shape[1] != ch:
-            raise ValueError(f"km3d loss: output['{name}'] has {t.shape[1]} channels, the KM3D head has {ch}")
-        maps.append(t.contiguous())
-    B, C, H, W = maps[0].shape
-    for (name, _), t in zip(MAPS, maps):
-        if (t.shape[0], t.shape[2], t.shape[3]) != (B, H, W):
-            raise ValueError(f"km3d loss: output['{name}'] {tuple(t.shape)} does not match hm's B, H, W = {(B, H, W)}")
-    targets = []
-    for name, ch in (("hm", C), ("hm_hp", NUM_JOINTS)):
-        t = annotations[name]
-        _check(t, f"annotations['{name}']", (torch.float32,))
-        if tuple(t.shape) != (B, ch, H, W):
-            raise ValueError(f"km3d loss: annotations['{name}'] {tuple(t.shape)}, expected {(B, ch, H, W)}")
-        targets.append(t.contiguous())
-    ind = annotations["ind"]
-    if ind.dim() != 2 or ind.shape[0] != B:
-        raise ValueError(f"km3d loss: annotations['ind'] {tuple(ind.shape)}, expected [{B}, K]")
-    K = ind.shape[1]
-    if not 1 <= K <= MAX_ROWS:
-        raise ValueError(f"km3d loss: {K} object rows per image, 1..{MAX_ROWS} supported")
-    for name, dtypes, trail, per in _TARGETS:
-        t = annotations[name]
-        _check(t, f"annotations['{name}']", dtypes)
-        if tuple(t.shape) != (B, K * per) + trail:
-            raise ValueError(f"km3d loss: annotations['{name}'] {tuple(t.shape)}, expected {(B, K * per) + trail}")
-        targets.append(t.contiguous())
-    _check(P2, "P2", (torch.float32,))
-    if tuple(P2.shape) != (B, 3, 4):
-        raise ValueError(f"km3d loss: P2 {tuple(P2.shape)}, expected {(B, 3, 4)}")
-    targets.append(P2.contiguous())
-    return maps, targets, (B, C, H, W, K)
-
-
-def _ptrs(ts):
-    """Host array of device pointers (the C ABI's maps / targets / grads)."""
-    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
-
-
 class KM3DLoss(torch.autograd.Function):
     """(output_w, rampup, targets tuple, sizes, *maps) -> (total 0-dim, terms [11]); differentiable in the nine maps."""
 
     @staticmethod
     def forward(ctx, output_w: float, rampup: float, targets, sizes, *maps):
         dev = maps[0].device
-        lib = _lib.load()
-        ws_bytes = int(lib.vd3d_km3d_loss_workspace_bytes(*sizes))
-        if ws_bytes < 0:
-            raise _lib.Vd3dError(f"vd3d_km3d_loss_workspace_bytes failed ({ws_bytes}): {lib.vd3d_last_error().decode()}")
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        ws, ws_bytes = workspace("vd3d_km3d_loss_workspace_bytes", *sizes, device=dev)
         terms = torch.empty(len(TERMS), dtype=torch.float32, device=dev)
         total = torch.empty((), dtype=torch.float32, device=dev)
-        _lib.call("vd3d_km3d_loss_forward", _ptrs(maps), _ptrs(targets), *sizes, output_w, rampup, ws.data_ptr(), ws_bytes,
-                  terms.data_ptr(), total.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        _lib.call("vd3d_km3d_loss_forward", ptr_array(maps), ptr_array(targets), *sizes, output_w, rampup, ws.data_ptr(), ws_bytes,
+                  terms.data_ptr(), total.data_ptr(), stream(maps[0]))
         ctx.save_for_backward(ws, *targets, *maps)
         ctx.args, ctx.sizes, ctx.n_targets = (output_w, rampup), sizes, len(targets)
         ctx.set_materialize_grads(False)
@@ -152,9 +96,9 @@ class KM3DLoss(torch.autograd.Function):
         grads = [torch.empty_like(m) for m in maps]
         g_total = None if g_total is None else g_total.float().contiguous()
         g_terms = None if g_terms is None else g_terms.float().contiguous()
-        _lib.call("vd3d_km3d_loss_backward", _ptrs(maps), _ptrs(targets), *ctx.sizes, *ctx.args, ws.data_ptr(),
-                  None if g_terms is None else g_terms.data_ptr(), None if g_total is None else g_total.data_ptr(), _ptrs(grads),
-                  torch.cuda.current_stream(maps[0].device).cuda_stream)
+        _lib.call("vd3d_km3d_loss_backward", ptr_array(maps), ptr_array(targets), *ctx.sizes, *ctx.args, ws.data_ptr(),
+                  None if g_terms is None else g_terms.data_ptr(), None if g_total is None else g_total.data_ptr(), ptr_array(grads),
+                  stream(maps[0]))
         return (None, None, None, None, *grads)
 
 
@@ -164,8 +108,8 @@ def km3d_head_loss(output: Mapping, annotations: Mapping, P2: torch.Tensor, epoc
     LossConfig or the head's loss_cfg mapping (None: the defaults).  Returns (loss, loss_stats) like the reference: 0-dim float32 device
     tensors, loss_stats with `loss` (= box_score), the ten unweighted terms, box_score and total_loss (= loss); box_score carries no
     gradient.  The annotations are not modified."""
-    cfg = cfg if isinstance(cfg, LossConfig) else LossConfig.from_loss_cfg(cfg or {})
-    maps, targets, sizes = _inputs(output, annotations, P2)
+    cfg = as_config(LossConfig, cfg or {})
+    maps, targets, sizes = map_inputs("km3d loss", "KM3D", MAPS, _HM_TARGETS, _TARGETS, MAX_ROWS, output, annotations, P2)
     total, terms = KM3DLoss.apply(float(cfg.output_w), cfg.exp_rampup(epoch), tuple(targets), sizes, *maps)
     stats = {name: terms[i] for i, name in enumerate(TERMS)}
     stats = dict(loss=stats["box_score"], **stats)

@@ -11,23 +11,23 @@ fixed order without float atomics, so two runs give the same bits and the pair c
 """
 from __future__ import annotations
 
-import ctypes
 from dataclasses import dataclass
 from typing import Mapping, Tuple
 
 import torch
 
 from . import _lib
+from .loss_common import as_config, map_inputs, ptr_array, stream, workspace
 
 MAPS = (("hm", None), ("bbox2d", 4), ("hps", 20), ("rot", 8), ("dim", 3), ("reg", 2), ("depth", 1), ("depth_uncertainty", 1),
         ("corner_uncertainty", 3))
 TERMS = ("hm_loss", "hp_loss", "box2d_loss", "off_loss", "dim_loss", "depth_loss", "kpd_loss", "rot_loss", "soft_depth_loss")
 MAX_ROWS = 128
-# annotation key -> (dtypes accepted, trailing shape after [B, K]); hm is [B, C, H, W] like the output
-_TARGETS = (("ind", (torch.int64,), ()), ("reg_mask", (torch.bool, torch.uint8), ()), ("hps", (torch.float32,), (20,)),
-            ("hps_mask", (torch.uint8, torch.bool), (20,)), ("dep", (torch.float32,), (1,)), ("rotbin", (torch.int64,), (2,)),
-            ("rotres", (torch.float32,), (2,)), ("bboxes2d_target", (torch.float32,), (4,)), ("dim", (torch.float32,), (3,)),
-            ("reg", (torch.float32,), (2,)), ("kp_detph_mask", (torch.float32,), (3,)))
+# annotation key -> (dtypes accepted, trailing shape after [B, K], rows per object); hm is [B, C, H, W] like the output
+_TARGETS = (("ind", (torch.int64,), (), 1), ("reg_mask", (torch.bool, torch.uint8), (), 1), ("hps", (torch.float32,), (20,), 1),
+            ("hps_mask", (torch.uint8, torch.bool), (20,), 1), ("dep", (torch.float32,), (1,), 1), ("rotbin", (torch.int64,), (2,), 1),
+            ("rotres", (torch.float32,), (2,), 1), ("bboxes2d_target", (torch.float32,), (4,), 1), ("dim", (torch.float32,), (3,), 1),
+            ("reg", (torch.float32,), (2,), 1), ("kp_detph_mask", (torch.float32,), (3,), 1))
 
 
 @dataclass(frozen=True)
@@ -53,73 +53,18 @@ class LossConfig:
         return cls(uncertainty_range=tuple(float(v) for v in head.uncertainty_range), uncertainty_weight=float(head.uncertainty_weight))
 
 
-def _check(t: torch.Tensor, name: str, dtypes) -> None:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise RuntimeError(f"monoflex loss: {name} must be a CUDA tensor (there is no CPU path)")
-    if t.dtype not in dtypes:
-        raise RuntimeError(f"monoflex loss: {name} must be {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
-
-
-def _inputs(output: Mapping, annotations: Mapping, P2: torch.Tensor):
-    """Validated, contiguous (maps, targets, sizes); raises before any launch."""
-    maps = []
-    for name, ch in MAPS:
-        t = output[name]
-        _check(t, f"output['{name}']", (torch.float32,))
-        if t.dim() != 4:
-            raise ValueError(f"monoflex loss: output['{name}'] must be [B, C, H, W], got {tuple(t.shape)}")
-        if ch is not None and t.shape[1] != ch:
-            raise ValueError(f"monoflex loss: output['{name}'] has {t.shape[1]} channels, the MonoFlex head has {ch}")
-        maps.append(t.contiguous())
-    B, C, H, W = maps[0].shape
-    for (name, _), t in zip(MAPS, maps):
-        if (t.shape[0], t.shape[2], t.shape[3]) != (B, H, W):
-            raise ValueError(f"monoflex loss: output['{name}'] {tuple(t.shape)} does not match hm's B, H, W = {(B, H, W)}")
-    hm_t = annotations["hm"]
-    _check(hm_t, "annotations['hm']", (torch.float32,))
-    if tuple(hm_t.shape) != (B, C, H, W):
-        raise ValueError(f"monoflex loss: annotations['hm'] {tuple(hm_t.shape)}, expected {(B, C, H, W)}")
-    ind = annotations["ind"]
-    if ind.dim() != 2 or ind.shape[0] != B:
-        raise ValueError(f"monoflex loss: annotations['ind'] {tuple(ind.shape)}, expected [{B}, K]")
-    K = ind.shape[1]
-    if not 1 <= K <= MAX_ROWS:
-        raise ValueError(f"monoflex loss: {K} object rows per image, 1..{MAX_ROWS} supported")
-    targets = [hm_t.contiguous()]
-    for name, dtypes, trail in _TARGETS:
-        t = annotations[name]
-        _check(t, f"annotations['{name}']", dtypes)
-        if tuple(t.shape) != (B, K) + trail:
-            raise ValueError(f"monoflex loss: annotations['{name}'] {tuple(t.shape)}, expected {(B, K) + trail}")
-        targets.append(t.contiguous())
-    _check(P2, "P2", (torch.float32,))
-    if tuple(P2.shape) != (B, 3, 4):
-        raise ValueError(f"monoflex loss: P2 {tuple(P2.shape)}, expected {(B, 3, 4)}")
-    targets.append(P2.contiguous())
-    return maps, targets, (B, C, H, W, K)
-
-
-def _ptrs(ts):
-    """Host array of device pointers (the C ABI's maps / targets / grads)."""
-    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
-
-
 class MonoFlexLoss(torch.autograd.Function):
     """(cfg, targets tuple, *maps) -> (total 0-dim, terms [9]); differentiable in the nine maps."""
 
     @staticmethod
     def forward(ctx, cfg: LossConfig, targets, sizes, *maps):
         dev = maps[0].device
-        lib = _lib.load()
-        ws_bytes = int(lib.vd3d_monoflex_loss_workspace_bytes(*sizes))
-        if ws_bytes < 0:
-            raise _lib.Vd3dError(f"vd3d_monoflex_loss_workspace_bytes failed ({ws_bytes}): {lib.vd3d_last_error().decode()}")
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        ws, ws_bytes = workspace("vd3d_monoflex_loss_workspace_bytes", *sizes, device=dev)
         terms = torch.empty(len(TERMS), dtype=torch.float32, device=dev)
         total = torch.empty((), dtype=torch.float32, device=dev)
         lo, hi = cfg.uncertainty_range
-        _lib.call("vd3d_monoflex_loss_forward", _ptrs(maps), _ptrs(targets), *sizes, lo, hi, cfg.uncertainty_weight, ws.data_ptr(),
-                  ws_bytes, terms.data_ptr(), total.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+        _lib.call("vd3d_monoflex_loss_forward", ptr_array(maps), ptr_array(targets), *sizes, lo, hi, cfg.uncertainty_weight,
+                  ws.data_ptr(), ws_bytes, terms.data_ptr(), total.data_ptr(), stream(maps[0]))
         ctx.save_for_backward(ws, *targets, *maps)
         ctx.cfg, ctx.sizes, ctx.n_targets = cfg, sizes, len(targets)
         ctx.set_materialize_grads(False)
@@ -133,9 +78,9 @@ class MonoFlexLoss(torch.autograd.Function):
         g_total = None if g_total is None else g_total.float().contiguous()
         g_terms = None if g_terms is None else g_terms.float().contiguous()
         lo, hi = ctx.cfg.uncertainty_range
-        _lib.call("vd3d_monoflex_loss_backward", _ptrs(maps), _ptrs(targets), *ctx.sizes, lo, hi, ctx.cfg.uncertainty_weight, ws.data_ptr(),
-                  None if g_terms is None else g_terms.data_ptr(), None if g_total is None else g_total.data_ptr(), _ptrs(grads),
-                  torch.cuda.current_stream(maps[0].device).cuda_stream)
+        _lib.call("vd3d_monoflex_loss_backward", ptr_array(maps), ptr_array(targets), *ctx.sizes, lo, hi, ctx.cfg.uncertainty_weight,
+                  ws.data_ptr(), None if g_terms is None else g_terms.data_ptr(), None if g_total is None else g_total.data_ptr(),
+                  ptr_array(grads), stream(maps[0]))
         return (None, None, None, *grads)
 
 
@@ -144,8 +89,8 @@ def monoflex_head_loss(output: Mapping, annotations: Mapping, P2: torch.Tensor, 
     the KittiMonoFlexDataset targets with `ind` int64 and `reg_mask` bool / uint8; P2 [B, 3, 4]; cfg: a LossConfig or the head's
     loss_cfg mapping (None: the defaults).  Returns (loss, loss_stats) like the reference: 0-dim float32 device tensors, loss_stats with
     the nine unweighted terms and total_loss (= loss), all differentiable in the nine maps."""
-    cfg = cfg if isinstance(cfg, LossConfig) else LossConfig.from_loss_cfg(cfg or {})
-    maps, targets, sizes = _inputs(output, annotations, P2)
+    cfg = as_config(LossConfig, cfg or {})
+    maps, targets, sizes = map_inputs("monoflex loss", "MonoFlex", MAPS, (("hm", None),), _TARGETS, MAX_ROWS, output, annotations, P2)
     total, terms = MonoFlexLoss.apply(cfg, tuple(targets), sizes, *maps)
     stats = {name: terms[i] for i, name in enumerate(TERMS)}
     stats["total_loss"] = total

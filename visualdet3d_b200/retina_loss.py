@@ -26,6 +26,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .loss_common import as_config, cached_on, check, grad_out_pair, stream, workspace
 
 MAX_CLASSES = 64
 MAX_ROWS = 512          # annotation rows per image the kernels hold in shared memory
@@ -112,10 +113,7 @@ def _inputs(cls_scores, reg_preds, anchors, annotations, cfg: LossConfig):
     if annotations.shape[1] > MAX_ROWS:
         raise ValueError(f"retina loss: {annotations.shape[1]} annotation rows per image, at most {MAX_ROWS} supported")
     for t, name in ((cls_scores, "cls_scores"), (reg_preds, "reg_preds"), (anchors, "anchors"), (annotations, "annotations")):
-        if t.dtype != torch.float32:
-            raise RuntimeError(f"retina loss: {name} must be torch.float32, got {t.dtype}")
-        if not t.is_cuda:
-            raise RuntimeError(f"retina loss: {name} must be a CUDA tensor (there is no CPU path)")
+        check(t, "retina loss", name, torch.float32)
     return cls_scores.contiguous(), reg_preds.contiguous(), anchor.contiguous(), annotations.contiguous()
 
 
@@ -123,11 +121,7 @@ def _forward(cls_scores, reg_preds, anchor, ann, cfg: LossConfig, params: np.nda
     B, N, C = cls_scores.shape
     M, K = ann.shape[1], ann.shape[2]
     dev = cls_scores.device
-    lib = _lib.load()
-    ws_bytes = int(lib.vd3d_retina_loss_workspace_bytes(B, N, M))
-    if ws_bytes < 0:
-        raise _lib.Vd3dError(f"vd3d_retina_loss_workspace_bytes failed ({ws_bytes}): {lib.vd3d_last_error().decode()}")
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    ws, ws_bytes = workspace("vd3d_retina_loss_workspace_bytes", B, N, M, device=dev)
     assign = torch.empty(B, N, dtype=torch.int32, device=dev)
     counts = torch.empty(B, 3, dtype=torch.int32, device=dev)
     scale = torch.empty(1, dtype=torch.float32, device=dev)
@@ -135,7 +129,7 @@ def _forward(cls_scores, reg_preds, anchor, ann, cfg: LossConfig, params: np.nda
     reg_loss = torch.empty((), dtype=torch.float32, device=dev)
     _lib.call("vd3d_retina_loss_forward", cls_scores.data_ptr(), reg_preds.data_ptr(), anchor.data_ptr(), ann.data_ptr(), B, N, C, M, K,
               params.ctypes.data, int(cfg.match_low_quality), int(cfg.gt_max_assign_all), ws.data_ptr(), ws_bytes, assign.data_ptr(),
-              counts.data_ptr(), scale.data_ptr(), cls_loss.data_ptr(), reg_loss.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+              counts.data_ptr(), scale.data_ptr(), cls_loss.data_ptr(), reg_loss.data_ptr(), stream(cls_scores))
     return cls_loss, reg_loss, assign, counts, scale
 
 
@@ -153,20 +147,14 @@ class RetinaHeadLoss(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_cls, g_reg):
         cls_scores, reg_preds, anchor, ann, assign, scale = ctx.saved_tensors
-        dev = cls_scores.device
-        zero = torch.zeros(1, dtype=torch.float32, device=dev)
-        grad_out = torch.cat([(zero if g_cls is None else g_cls.reshape(1)), (zero if g_reg is None else g_reg.reshape(1))]).float()
+        grad_out = grad_out_pair(g_cls, g_reg, cls_scores.device)
         B, N, C = cls_scores.shape
         grad_cls = torch.empty_like(cls_scores)
         grad_reg = torch.empty_like(reg_preds)
         _lib.call("vd3d_retina_loss_backward", cls_scores.data_ptr(), reg_preds.data_ptr(), anchor.data_ptr(), ann.data_ptr(), B, N, C,
                   ann.shape[1], ann.shape[2], ctx.params.ctypes.data, assign.data_ptr(), scale.data_ptr(), grad_out.data_ptr(),
-                  grad_cls.data_ptr(), grad_reg.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+                  grad_cls.data_ptr(), grad_reg.data_ptr(), stream(cls_scores))
         return grad_cls, grad_reg, None, None, None
-
-
-def _config(cfg, num_classes: int) -> LossConfig:
-    return cfg if isinstance(cfg, LossConfig) else LossConfig.from_loss_cfg(cfg, num_classes)
 
 
 def retinanet_head_loss(cls_scores: torch.Tensor, reg_preds: torch.Tensor, anchors: torch.Tensor, annotations: torch.Tensor, cfg):
@@ -175,7 +163,7 @@ def retinanet_head_loss(cls_scores: torch.Tensor, reg_preds: torch.Tensor, ancho
     compound_annotation's 12 columns); cfg: a LossConfig, or the head's loss_cfg mapping (num_classes = cls_scores' last dimension, default
     target_means / target_stds).  Returns (cls_loss, reg_loss, dict(cls_loss, reg_loss, total_loss)), 0-d float32 tensors differentiable
     in cls_scores and reg_preds."""
-    cfg = _config(cfg, cls_scores.shape[-1])
+    cfg = as_config(LossConfig, cfg, cls_scores.shape[-1])
     cls_scores, reg_preds, anchor, ann = _inputs(cls_scores, reg_preds, anchors, annotations, cfg)
     cls_loss, reg_loss = RetinaHeadLoss.apply(cls_scores, reg_preds, anchor, ann, cfg)
     return cls_loss, reg_loss, dict(cls_loss=cls_loss, reg_loss=reg_loss, total_loss=cls_loss + reg_loss)
@@ -185,7 +173,7 @@ def assignment(cls_scores, reg_preds, anchors, annotations, cfg):
     """The forward's anchor assignment and counts (same arguments as retinanet_head_loss): assigned_gt_inds [B, N] int32 (1-based among
     the image's valid annotation rows, 0 negative -- every anchor of an image without a valid row --, -1 ignored) and counts [B, 3] int32
     (positives, negatives, ignored)."""
-    cfg = _config(cfg, cls_scores.shape[-1])
+    cfg = as_config(LossConfig, cfg, cls_scores.shape[-1])
     with torch.no_grad():
         _, _, assign, counts, _ = _forward(*_inputs(cls_scores, reg_preds, anchors, annotations, cfg), cfg, cfg.params())
     return assign, counts
@@ -197,11 +185,7 @@ def _head_config(head) -> LossConfig:
     bw = head.loss_cls.balance_weights
     key = (bw.data_ptr(), bw._version, head.num_clasess, head.loss_cls.gamma, id(head.loss_cfg), tuple(head.target_means),
            tuple(head.target_stds))
-    cached = head.__dict__.get("_vd3d_retina_loss_config")
-    if cached is None or cached[0] != key:
-        cached = (key, LossConfig.from_head(head))
-        head.__dict__["_vd3d_retina_loss_config"] = cached
-    return cached[1]
+    return cached_on(head, "_vd3d_retina_loss_config", key, lambda: LossConfig.from_head(head))
 
 
 def head_loss(self, cls_scores, reg_preds, anchors, annotations):
