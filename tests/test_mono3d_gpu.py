@@ -5,7 +5,7 @@ import torch
 
 from conftest import load_fixture, subsample_like
 import torch_port as tp
-from test_stereo3d_gpu import assert_dets_match
+from detector_harness import assert_dets_match, run_with_stages
 
 pytestmark = pytest.mark.gpu
 
@@ -14,24 +14,6 @@ def build(kind):
     from visualdet3d_b200.detectors import build_synthetic_mono3d
     det, sd, cfg, priors = build_synthetic_mono3d(kind, seed=0)
     return det.cuda().eval(), sd, cfg, priors
-
-
-def run_with_stages(det, img, P2):
-    from visualdet3d_b200.engine import Act
-    st = {}
-
-    def hook(name, v):
-        st[name] = v.to_nchw().cpu() if isinstance(v, Act) else v.detach().cpu().clone()
-    det.stage_hook = hook
-    try:
-        with torch.no_grad():
-            res = det.forward_batch(img.cuda(), P2.cuda())
-    finally:
-        det.stage_hook = None
-    B = img.shape[0]
-    st["cls_preds"] = st["cls_preds"].permute(0, 2, 3, 1).reshape(B, -1, det.num_cls_output)
-    st["reg_preds"] = st["reg_preds"].permute(0, 2, 3, 1).reshape(B, -1, 12)
-    return res, st
 
 
 @pytest.mark.parametrize("kind,tag", [("Yolo3D", "yolo3d_96x320"), ("Yolo3D", "yolo3d_288x1280"),
@@ -43,7 +25,7 @@ def test_against_reference_fixture(kind, tag):
     fx = load_fixture(tag)
     H, W, B, seed = [int(v) for v in fx["meta"]]
     img, P2 = synth.synth_mono_inputs(B, H, W, seed=1)
-    res, st = run_with_stages(det, img, P2)
+    res, st = run_with_stages(det, img, P2, flatten_heads=True)
     rep = {nm: float(np.abs(subsample_like(st[nm], fx[nm]) - fx[nm]["samples"]).max())
            for nm in ["features", "cls_preds", "reg_preds"] + (["gac"] if "gac" in fx else [])}
     print(tag, "stage max|diff| vs reference:", rep)

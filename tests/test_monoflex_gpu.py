@@ -8,6 +8,7 @@ import torch.nn.functional as F
 
 from conftest import GOLDEN, load_fixture, subsample_like
 import torch_port as tp
+from detector_harness import match_dets, run_with_stages
 
 pytestmark = pytest.mark.gpu
 
@@ -41,38 +42,6 @@ def mf():
     from visualdet3d_b200.detectors import build_synthetic_monoflex
     det, sd, cfg = build_synthetic_monoflex(seed=0)
     return det.cuda().eval(), sd, cfg
-
-
-def run_with_stages(det, img, P2):
-    from visualdet3d_b200.engine import Act
-    st = {}
-    det.stage_hook = lambda name, v: st.__setitem__(name, v.to_nchw().cpu() if isinstance(v, Act) else v.detach().cpu().clone())
-    try:
-        with torch.no_grad():
-            res = det.forward_batch(img.cuda(), P2.cuda())
-    finally:
-        det.stage_hook = None
-    return res, st
-
-
-def match_dets(got, ref, got_index, atol=1e-3):
-    """same peak set; same order except between score-tied rows; values within atol (boxes rtol 1e-5 on top)."""
-    s, bx, ci = [t.cpu() for t in got]
-    rs, rb, rc, rflat = ref
-    assert len(s) == len(rs), (len(s), len(rs))
-    if len(s) == 0:
-        return
-    gi = got_index.cpu().long()
-    assert torch.equal(torch.sort(gi)[0], torch.sort(rflat)[0]), "kept peak sets differ"
-    if not torch.equal(gi, rflat):
-        pos = {int(a): i for i, a in enumerate(rflat.tolist())}
-        perm = torch.tensor([pos[int(a)] for a in gi.tolist()])
-        for i in (perm != torch.arange(len(perm))).nonzero()[:, 0].tolist():
-            assert abs(float(rs[perm[i]]) - float(rs[i])) < 1e-5
-        rs, rb, rc = rs[perm], rb[perm], rc[perm]
-    assert ci.shape == rc.shape and torch.equal(ci, rc)
-    assert float((s - rs).abs().max()) < atol
-    np.testing.assert_allclose(bx.numpy(), rb.numpy(), atol=atol, rtol=1e-5)
 
 
 @pytest.mark.parametrize("tag", ["monoflex_96x320", "monoflex_192x640", "monoflex_384x1280"])     # the last one = BASELINE configs[3] shape

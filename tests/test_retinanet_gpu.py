@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from conftest import load_fixture, subsample_like
+from detector_harness import run_with_stages
 
 pytestmark = pytest.mark.gpu
 
@@ -49,21 +50,6 @@ def test_decode_stage_on_reference_head_outputs():
         # boxes: the same expression order as the reference; the device expf may differ from the host's by an ulp, which at coordinates of
         # hundreds of pixels is ~3e-5 absolute, so the bound is in ulps (measured: at most 1)
         np.testing.assert_array_max_ulp(bx.numpy(), fx[f"bboxes_{b}"], maxulp=2)
-
-
-def run_with_stages(det, img):
-    from visualdet3d_b200.engine import Act
-    st = {}
-
-    def hook(name, v):
-        st[name] = v.to_nchw().cpu() if isinstance(v, Act) else v.detach().cpu().clone()
-    det.stage_hook = hook
-    try:
-        with torch.no_grad():
-            res = det.forward_batch(img.cuda())
-    finally:
-        det.stage_hook = None
-    return res, st
 
 
 @pytest.mark.parametrize("tag", ["retinanet_96x320", "retinanet_288x1280", "retinanet_64x128_nopre"])
@@ -153,6 +139,25 @@ def test_batch8_equals_single_images_and_graph_replay():
         assert torch.equal(rows[:, :4], r8[b][1]) and torch.equal(rows[:, 4:11], torch.zeros_like(rows[:, 4:11]))
     with pytest.raises(Exception, match="2-D"):
         graphs.GraphedStep(det, [ic], P2.cuda(), rec, kmax, geometry=True, enabled=False)()
+
+
+def test_in_place_batchnorm_statistic_refolds_the_plan():
+    """Scaling a BatchNorm running_var in place re-folds the weights on the next launch: its outputs equal a freshly built detector loaded
+    with the changed state, and differ from the outputs before the change."""
+    from visualdet3d_b200 import synth
+    det, _, _ = build()
+    img, _ = synth.synth_mono_inputs(2, 96, 320, seed=1)
+    res0, st0 = run_with_stages(det, img)
+    with torch.no_grad():
+        det.core.backbone.bn1.running_var.mul_(2.0)
+    res1, st1 = run_with_stages(det, img)
+    fresh, _, _ = build()
+    fresh.load_state_dict(det.state_dict())
+    res2, st2 = run_with_stages(fresh, img)
+    assert sorted(st1) == sorted(st2)
+    assert all(torch.equal(st1[k], st2[k]) for k in st1)
+    assert all(torch.equal(x, y) for a, b in zip(res1, res2) for x, y in zip(a, b))
+    assert not torch.equal(st1["cls0"], st0["cls0"])
 
 
 @pytest.mark.parametrize("B", [1, 8])

@@ -7,6 +7,7 @@ import torch
 
 from conftest import load_fixture, subsample_like
 import torch_port as tp
+from detector_harness import assert_dets_match, run_with_stages
 
 pytestmark = pytest.mark.gpu
 
@@ -18,50 +19,6 @@ def det_bundle():
     return det.cuda().eval(), sd, cfg, priors
 
 
-def assert_dets_match(got, ref, got_anchor, atol=1e-3):
-    """got = (scores, boxes, cls) from the CUDA path, ref = oracle (scores, boxes, cls, anchor_idx).  The kept ANCHOR SET must
-    be identical; the row order must be identical except between rows whose scores are within 1e-5 of each other
-    (a descending sort of scores that differ by an ulp between host and device libm); values within `atol`."""
-    s, bx, ci = [t.cpu() for t in got]
-    rs, rb, rc, ridx = ref
-    ga = got_anchor.cpu().long()
-    assert len(s) == len(rs), (len(s), len(rs))
-    if len(s) == 0:
-        return 0
-    assert torch.equal(torch.sort(ga)[0], torch.sort(ridx)[0]), "kept anchor sets differ"
-    swaps = 0
-    if not torch.equal(ga, ridx):
-        pos = {int(a): i for i, a in enumerate(ridx.tolist())}
-        perm = torch.tensor([pos[int(a)] for a in ga.tolist()])
-        moved = (perm != torch.arange(len(perm))).nonzero()[:, 0]
-        swaps = len(moved)
-        for i in moved.tolist():
-            assert abs(float(rs[perm[i]]) - float(rs[i])) < 1e-5, "order differs between rows that are not score-tied"
-        rs, rb, rc = rs[perm], rb[perm], rc[perm]
-    assert torch.equal(ci, rc)
-    assert float((s - rs).abs().max()) < atol, float((s - rs).abs().max())
-    assert float((bx - rb).abs().max()) < atol, float((bx - rb).abs().max())
-    return swaps
-
-
-def run_with_stages(det, left, right, P2):
-    from visualdet3d_b200.engine import Act
-    st = {}
-
-    def hook(name, v):
-        st[name] = v.to_nchw().cpu() if isinstance(v, Act) else v.detach().cpu().clone()
-    det.stage_hook = hook
-    try:
-        with torch.no_grad():
-            res = det.forward_batch(left.cuda(), right.cuda(), P2.cuda())
-    finally:
-        det.stage_hook = None
-    B = left.shape[0]
-    st["cls_preds"] = st["cls_preds"].permute(0, 2, 3, 1).reshape(B, -1, det.num_cls_output)
-    st["reg_preds"] = st["reg_preds"].permute(0, 2, 3, 1).reshape(B, -1, 12)
-    return res, st
-
-
 @pytest.mark.parametrize("tag", ["stereo3d_96x320", "stereo3d_192x640", "stereo3d_384x1280"])    # the last one = BASELINE configs[1] shape
 def test_against_reference_fixture(det_bundle, tag):
     from visualdet3d_b200 import synth
@@ -69,7 +26,7 @@ def test_against_reference_fixture(det_bundle, tag):
     fx = load_fixture(tag)
     H, W, B, seed = [int(v) for v in fx["meta"]]
     left, right, P2, P3 = synth.synth_stereo_inputs(B, H, W, seed=1)
-    res, st = run_with_stages(det, left, right, P2)
+    res, st = run_with_stages(det, left, right, P2, flatten_heads=True)
     report = {}
     for nm in ["feat4", "vol4", "vol8", "vol16", "features", "cls_preds", "reg_preds"]:
         got = subsample_like(st[nm], fx[nm])
@@ -93,7 +50,7 @@ def test_against_oracle_ragged_batch(det_bundle):
     det, sd, cfg, (pm, ps) = det_bundle
     B, H, W = 3, 128, 384
     left, right, P2, P3 = synth.synth_stereo_inputs(B, H, W, seed=7)
-    res, st = run_with_stages(det, left, right, P2)
+    res, st = run_with_stages(det, left, right, P2, flatten_heads=True)
     ost = {}
     ref = tp.stereo3d_forward(sd, left, right, P2, cfg, pm, ps, ost)
     for nm in ["feat4", "feat8", "feat16", "vol4", "vol8", "vol16", "features", "cls_preds", "reg_preds"]:

@@ -1,8 +1,9 @@
-"""Shared machinery of the anchor-based 3-D detectors (Stereo3D, Yolo3D, GroundAwareYolo3D): config parsing, lazily folded /
-packed weights ("plan"), device anchor tables, the batched decode + NMS stage and the reference's list protocol."""
+"""Host shell shared by the native detectors: the lazily folded / packed weights ("plan"), stage hooks, in-situ kernel timing, decoder
+buffers, launch-input checks and the reference's list protocol (`NativeDetector`); and the config parsing, device anchor tables and
+batched decode + NMS of the anchor-based 3-D detectors Stereo3D, Yolo3D and GroundAwareYolo3D (`Anchor3DDetector`)."""
 from __future__ import annotations
 
-from typing import Optional
+import contextlib
 
 import torch
 import torch.nn as nn
@@ -12,9 +13,100 @@ from .._lib import Vd3dError
 from ..anchors import AnchorTable, load_priors
 
 
-class Anchor3DDetector(nn.Module):
-    """Subclasses build `self.core` / `self.bbox_head` (parameter holders) and implement `build_plan(dev)` and
-    `network(...) -> (cls Act, reg Act)`; everything from the head outputs to the detection triples lives here."""
+class NativeDetector(nn.Module):
+    """Subclasses hold the parameters, implement `build_plan(dev)` and `launch(images, P2)` -> the decoder holding the fixed-capacity
+    device outputs; everything around that lives here."""
+    N_IMAGES = 1          # images per sample of `launch` (pipeline.StreamedInference)
+
+    def __init__(self):
+        super().__init__()
+        self._plan = None
+        self._plan_version = None
+        self._arena = E.Arena()
+        self._decoders = {}
+        self._last_decoder = None
+        self.stage_hook = None            # tests: callable(name, Act-or-tensor)
+        self.profile_events = None        # bench: list collecting (name, start, end) CUDA events of a profiled kernel
+
+    # ---- plan (folded / packed weights) -------------------------------------------------------------------
+    def build_plan(self, dev) -> dict:  # pragma: no cover
+        raise NotImplementedError
+
+    def prepare(self, force: bool = False):
+        """Fold BN into conv weights, pack for the kernels, upload.  Re-run automatically when a parameter or buffer (a BatchNorm running
+        statistic) changes; graphs.GraphedStep re-captures on the same version."""
+        dev = next(self.parameters()).device
+        if dev.type != "cuda":
+            raise Vd3dError(f"{type(self).__name__} has no CPU path: move the module to a CUDA device first")
+        ver = (tuple(p._version for p in self.parameters()) + tuple(b._version for b in self.buffers()), str(dev))
+        if self._plan is not None and not force and ver == self._plan_version:
+            return self._plan
+        self._plan, self._plan_version = self.build_plan(dev), ver
+        return self._plan
+
+    def _hook(self, name, value):
+        if self.stage_hook is not None:
+            self.stage_hook(name, value)
+
+    @contextlib.contextmanager
+    def _timed(self, name: str):
+        """CUDA events around a kernel IN SITU when `profile_events` is a list (bench.py sets it for the timed region; the events are
+        recorded on the current stream, nothing synchronises); a no-op otherwise."""
+        if self.profile_events is None:
+            yield
+            return
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+        yield
+        e1 = torch.cuda.Event(enable_timing=True)
+        e1.record()
+        self.profile_events.append((name, e0, e1))
+
+    def _decoder(self, key, make):
+        """The decoder buffers cached under `key` (built by `make()` on first use); they become `_last_decoder`."""
+        if key not in self._decoders:
+            self._decoders[key] = make()
+        self._last_decoder = self._decoders[key]
+        return self._last_decoder
+
+    @staticmethod
+    def _device_inputs(*named):
+        """(tensor, name) pairs -> the tensors as contiguous float32; a tensor off the GPU is refused by name."""
+        for t, name in named:
+            E._require_cuda(t, name)
+        return [t.float().contiguous() for t, _ in named]
+
+    # ---- detections ---------------------------------------------------------------------------------------
+    @staticmethod
+    def _result(scores, boxes, cls):
+        """One image's triple in the reference's shapes (RetinaNet: 4 box columns; KM3D: cls [K, 1])."""
+        return scores, boxes, cls
+
+    def results(self, dec: E.DecodeNms):
+        """Per-image (scores, bboxes, cls) triples (one D2H read of the counts)."""
+        return [tuple(t.clone() for t in self._result(s, b, c)) for (s, b, c) in dec.results()]
+
+    def forward_batch(self, images, P2=None):
+        return self.results(self.launch(images, P2))
+
+    def test_forward(self, img_batch, P2=None):
+        assert img_batch.shape[0] == 1   # the reference's test_forward takes one image; use forward_batch for B > 1
+        return self.forward_batch(img_batch, P2)[0]
+
+    def train_forward(self, *a, **k):
+        raise NotImplementedError("training forward is out of scope of the native inference path (SURVEY.md section 2)")
+
+    def forward(self, inputs):
+        """The reference's list protocol: [image, P2] -> one image's triple; a 3-element list is a training step (raises)."""
+        if isinstance(inputs, list) and len(inputs) == 3:
+            return self.train_forward(*inputs)
+        img_batch, P2 = inputs
+        return self.test_forward(img_batch, P2)
+
+
+class Anchor3DDetector(NativeDetector):
+    """Subclasses build `self.core` / `self.bbox_head` (parameter holders) and implement `build_plan(dev)` and the forward up to the
+    head outputs; the anchors, decode + NMS and post-optimisation live here."""
 
     def __init__(self, network_cfg):
         super().__init__()
@@ -52,58 +144,7 @@ class Anchor3DDetector(nn.Module):
         # R/heads/detection_3d_head.py:294-308 (hill climbing on the yaw, SURVEY.md 8(f).2): device kernel after the NMS (`decode`)
         self.post_optimization = bool(self.test_cfg.get("post_optimization", False))
         self.max_detections = int(self.test_cfg.get("max_candidates", 2048))   # fixed capacity of the decode / NMS stage
-        self._plan = None
-        self._plan_version = None
-        self._arena = E.Arena()
         self._anchor_tables = {}
-        self._decoders = {}
-        self._last_decoder = None
-        self.stage_hook = None            # tests: callable(name, Act-or-tensor)
-        self.profile_events = None        # bench: list collecting (start, end) CUDA events of a profiled kernel
-
-    # ---- plan (folded / packed weights) -------------------------------------------------------------------
-    def _param_version(self):
-        return tuple(p._version for p in self.parameters()) + tuple(b._version for b in self.buffers())
-
-    def _device(self):
-        return next(self.parameters()).device
-
-    def build_plan(self, dev) -> dict:  # pragma: no cover
-        raise NotImplementedError
-
-    def prepare(self, force: bool = False):
-        """Fold BN into conv weights, pack for the kernels, upload.  Re-run automatically when parameters change."""
-        dev = self._device()
-        if dev.type != "cuda":
-            raise Vd3dError(f"{type(self).__name__} (B200) has no CPU path: move the module to a CUDA device first")
-        ver = (self._param_version(), str(dev))
-        if self._plan is not None and not force and ver == self._plan_version:
-            return self._plan
-        self._plan, self._plan_version = self.build_plan(dev), ver
-        return self._plan
-
-    def _hook(self, name, value):
-        if self.stage_hook is not None:
-            self.stage_hook(name, value)
-
-    def _timed(self, name: str):
-        """Context manager: CUDA events around a kernel IN SITU when `profile_events` is a list (bench.py sets it for the timed region; the
-        events are recorded on the current stream, nothing synchronises); a no-op otherwise."""
-        det = self
-
-        class _T:
-            def __enter__(self_t):
-                if det.profile_events is not None:
-                    self_t.e0 = torch.cuda.Event(enable_timing=True)
-                    self_t.e0.record()
-
-            def __exit__(self_t, *a):
-                if det.profile_events is not None:
-                    e1 = torch.cuda.Event(enable_timing=True)
-                    e1.record()
-                    det.profile_events.append((name, self_t.e0, e1))
-                return False
-        return _T()
 
     def _anchor_table(self, H, W, dev) -> AnchorTable:
         key = (H, W, str(dev))
@@ -126,26 +167,14 @@ class Anchor3DDetector(nn.Module):
         else:
             mask.fill_(1)
         self._hook("mask", mask)
-        key = (B, str(dev))
-        if key not in self._decoders:
-            self._decoders[key] = E.DecodeNms(B, self.max_detections, dev)
-        dec = self._decoders[key]
+        dec = self._decoder((B, str(dev)), lambda: E.DecodeNms(B, self.max_detections, dev))
         dec.run(cls.t.view(B, N, self.num_cls_output), reg.t.view(B, N, 12), tab.anchors, tab.mean_std, mask,
                 self.num_classes, self.test_cfg.get("score_thr", 0.5), self.test_cfg.get("nms_iou_thr", 0.5), W, H)
         if self.post_optimization:
             # head.test_cfg.post_optimization (R/heads/detection_3d_head.py:294-308): yaw hill climbing of the kept car boxes deeper than
             # 3 m, in place on the fixed-capacity NMS output, stream-ordered (the reference searches on the CPU with one `.item()` per box)
             dec.post_opt(P2)
-        self._last_decoder = dec
         return dec
-
-    @staticmethod
-    def results(dec: E.DecodeNms):
-        """Per-image (scores, bboxes, cls) triples (one D2H read of the counts)."""
-        return [(s.clone(), b.clone(), c.clone()) for (s, b, c) in dec.results()]
-
-    def train_forward(self, *a, **k):
-        raise NotImplementedError("training forward is out of scope of the B200 inference path (SURVEY.md section 2)")
 
 
 def synth_load(det: nn.Module, seed: int):

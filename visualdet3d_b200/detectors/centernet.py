@@ -9,8 +9,6 @@ output convs write their channel slices of one [B,H/4,W/4,56] tensor that the de
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
-
 import torch
 import torch.nn as nn
 
@@ -19,7 +17,7 @@ from .. import _lib
 from .._lib import Vd3dError, call
 from ..plugin import DETECTOR_DICT
 from . import modules as M
-from .base import synth_load
+from .base import NativeDetector, synth_load
 from .dla import DLAP, DLARunner, DLASegUpsampleP, DLAUpRunner
 
 
@@ -75,9 +73,12 @@ class KM3DHeadP(M.Holder):
         self.input_features, self.head_features = cin, feat
 
 
-class _CenterNetBase(nn.Module):
+class _CenterNetBase(NativeDetector):
+    """Subclasses name the decode entry (`DECODE`, `WORKSPACE`), the head maps it reads (`REQUIRED`, in the entry's argument order), the
+    peak-list capacities and the decode's own scalar arguments."""
     WITH_POSITION_LOSS = False
-    N_IMAGES = 1          # images per sample of `launch` (pipeline.StreamedInference)
+    DECODE = WORKSPACE = None
+    REQUIRED = ()
 
     def __init__(self, network_cfg):
         super().__init__()
@@ -92,22 +93,8 @@ class _CenterNetBase(nn.Module):
         self.uncertainty_range = tuple(lc.get("uncertainty_range", [-10, 10]))
         self.num_classes = self.bbox_head.num_classes
         self.topk = 100
-        self._plan, self._plan_version = None, None
-        self._arena = E.Arena()
-        self._decoders = {}
-        self._last_decoder = None
-        self.stage_hook = None
 
-    def _param_version(self):
-        return tuple(p._version for p in self.parameters()) + tuple(b._version for b in self.buffers())
-
-    def prepare(self, force: bool = False):
-        dev = next(self.parameters()).device
-        if dev.type != "cuda":
-            raise Vd3dError(f"{type(self).__name__} (B200) has no CPU path: move the module to a CUDA device first")
-        ver = (self._param_version(), str(dev))
-        if self._plan is not None and not force and ver == self._plan_version:
-            return self._plan
+    def build_plan(self, dev) -> dict:
         pl = dict(dla=DLARunner(self.core.backbone, dev, first_used_level=self.core.deconv_layers.first_level), up=DLAUpRunner(self.core.deconv_layers, dev))
         hl = self.bbox_head.head_layers
         names = list(hl.keys())
@@ -132,12 +119,7 @@ class _CenterNetBase(nn.Module):
             off[n] = co
             co += n_pad
         pl["outs"], pl["offsets"], pl["out_channels"], pl["names"] = outs, off, co, names
-        self._plan, self._plan_version = pl, ver
         return pl
-
-    def _hook(self, name, value):
-        if self.stage_hook is not None:
-            self.stage_hook(name, value)
 
     def network(self, images: torch.Tensor) -> E.Act:
         """core (DLA + up-sampling) + heads -> one NHWC tensor [B, H/4, W/4, out_channels] holding every head output."""
@@ -166,59 +148,43 @@ class _CenterNetBase(nn.Module):
         self._hook("heads", out)
         return out
 
-    def train_forward(self, *a, **k):
-        raise NotImplementedError("training forward is out of scope of the B200 inference path (SURVEY.md section 2)")
+    def launch(self, images, P2):
+        images, P2 = self._device_inputs((images, "image"), (P2, "P2"))
+        _, _, H, W = images.shape
+        return self.decode_maps(self.network(images), P2, H, W)
 
-    def test_forward(self, img_batch, P2):
-        assert img_batch.shape[0] == 1   # reference contract (KM3D.py:72)
-        return self.forward_batch(img_batch, P2)[0]
+    def _check_head(self, off):
+        missing = [k for k in self.REQUIRED if k not in off]
+        if missing:
+            raise Vd3dError(f"{type(self).__name__} head_dict lacks {missing}")
 
-    def forward(self, inputs):
-        if isinstance(inputs, list) and len(inputs) == 3:
-            return self.train_forward(*inputs)
-        img_batch, calib = inputs
-        return self.test_forward(img_batch, calib)
+    def decode_maps(self, out: E.Act, P2: torch.Tensor, H: int, W: int):
+        """The head's get_bboxes on the head maps `out` ([B, H/4, W/4, out_channels], the channel offsets of the plan); split from
+        `launch` so that tests can feed the decode with the oracle's maps."""
+        off = self.prepare()["offsets"]
+        self._check_head(off)
+        B, dev = out.B, out.t.device
+        caps = self._peak_caps(out.H * out.W)
+        dec = self._decoder((B, str(dev)) + caps,
+                            lambda: E.DecodeNms(B, 128, dev, ws_bytes=getattr(_lib.load(), self.WORKSPACE)(B, *caps)))
+        call(self.DECODE, out.ptr, B, out.H, out.W, self.num_classes, out.cs, *[off[k] for k in self.REQUIRED], P2.data_ptr(),
+             float(self.test_cfg.get("score_thr", 0.1)), float(self.test_cfg.get("nms_iou_thr", 0.5)), self.topk,
+             *self._decode_scalars(W, H, caps), dec.ws.data_ptr(), dec.cap, dec.scores.data_ptr(), dec.boxes.data_ptr(), dec.cls.data_ptr(),
+             dec.anchor.data_ptr(), dec.count.data_ptr(), dec.ncand.data_ptr(), E._stream())
+        return dec
 
 
 @DETECTOR_DICT.register_module
 class MonoFlex(_CenterNetBase):
     """R/detectors/KM3D.py:90-96 + MonoFlexHead.get_bboxes (R/heads/monoflex_head.py:114-179)."""
     REQUIRED = ("hm", "bbox2d", "hps", "rot", "dim", "reg", "depth", "depth_uncertainty", "corner_uncertainty")
+    DECODE, WORKSPACE = "vd3d_monoflex_decode", "vd3d_monoflex_decode_workspace"
 
-    def launch(self, images, P2):
-        for t, nm in ((images, "image"), (P2, "P2")):
-            E._require_cuda(t, nm)
-        images, P2 = images.float().contiguous(), P2.float().contiguous()
-        _, _, H, W = images.shape
-        return self.decode_maps(self.network(images), P2, H, W)
+    def _peak_caps(self, n_cells):
+        return (_peak_capacity(self.num_classes * n_cells),)
 
-    def decode_maps(self, out: E.Act, P2: torch.Tensor, H: int, W: int):
-        """MonoFlexHead.get_bboxes (R/heads/monoflex_head.py:114-179) on the head maps `out` ([B, H/4, W/4, out_channels], the
-        channel offsets of `prepare()`); split from `launch` so that tests can feed the decode with the oracle's maps."""
-        pl = self.prepare()
-        off = pl["offsets"]
-        missing = [k for k in self.REQUIRED if k not in off]
-        if missing:
-            raise Vd3dError(f"MonoFlex head_dict lacks {missing}")
-        B, dev = out.B, out.t.device
-        cap = _peak_capacity(self.num_classes * out.H * out.W)
-        key = (B, str(dev), cap)
-        if key not in self._decoders:
-            d = E.DecodeNms(B, 128, dev)
-            d.ws = torch.empty(int(_lib.load().vd3d_monoflex_decode_workspace(B, cap)), dtype=torch.uint8, device=dev)
-            self._decoders[key] = d
-        dec = self._decoders[key]
-        call("vd3d_monoflex_decode", out.ptr, B, out.H, out.W, self.num_classes, out.cs, off["hm"], off["bbox2d"], off["hps"], off["rot"],
-             off["dim"], off["reg"], off["depth"], off["depth_uncertainty"], off["corner_uncertainty"], P2.data_ptr(),
-             float(self.test_cfg.get("score_thr", 0.1)), float(self.test_cfg.get("nms_iou_thr", 0.5)), self.topk,
-             float(self.uncertainty_range[0]), float(self.uncertainty_range[1]), float(W), float(H), cap, dec.ws.data_ptr(), dec.cap,
-             dec.scores.data_ptr(), dec.boxes.data_ptr(), dec.cls.data_ptr(), dec.anchor.data_ptr(), dec.count.data_ptr(),
-             dec.ncand.data_ptr(), E._stream())
-        self._last_decoder = dec
-        return dec
-
-    def forward_batch(self, images, P2):
-        return [(s.clone(), b.clone(), c.clone()) for (s, b, c) in self.launch(images, P2).results()]
+    def _decode_scalars(self, W, H, caps):
+        return (float(self.uncertainty_range[0]), float(self.uncertainty_range[1]), float(W), float(H)) + caps
 
 
 @DETECTOR_DICT.register_module
@@ -226,42 +192,24 @@ class KM3D(_CenterNetBase):
     """R/detectors/KM3D.py:16-88 + KM3DHead.get_bboxes/_decode (R/heads/km3d_head.py:155-314) + gen_position
     (R/utils/rtm3d_utils.py:314-455)."""
     REQUIRED = ("hm", "wh", "hps", "rot", "dim", "prob", "reg", "hm_hp", "hp_offset")
+    DECODE, WORKSPACE = "vd3d_km3d_decode", "vd3d_km3d_decode_workspace"
     WITH_POSITION_LOSS = True
 
-    def launch(self, images, P2):
-        for t, nm in ((images, "image"), (P2, "P2")):
-            E._require_cuda(t, nm)
-        images, P2 = images.float().contiguous(), P2.float().contiguous()
-        _, _, H, W = images.shape
-        return self.decode_maps(self.network(images), P2, H, W)
-
-    def decode_maps(self, out: E.Act, P2: torch.Tensor, H: int, W: int):
-        """KM3DHead.get_bboxes/_decode + gen_position on the head maps `out` (see MonoFlex.decode_maps)."""
-        off = self.prepare()["offsets"]
-        missing = [k for k in self.REQUIRED if k not in off]
-        if missing:
-            raise Vd3dError(f"KM3D head_dict lacks {missing}")
+    def _check_head(self, off):
+        super()._check_head(off)
         if self.bbox_head.head_dict["hps"] != 18 or self.bbox_head.head_dict["hm_hp"] != 9:
             raise Vd3dError("KM3D decode expects 9 keypoints (hps = 18, hm_hp = 9)")
-        B, dev = out.B, out.t.device
-        cap, hp_cap = _peak_capacity(self.num_classes * out.H * out.W), _peak_capacity(out.H * out.W)
-        key = (B, str(dev), cap, hp_cap)
-        if key not in self._decoders:
-            d = E.DecodeNms(B, 128, dev)
-            d.ws = torch.empty(int(_lib.load().vd3d_km3d_decode_workspace(B, cap, hp_cap)), dtype=torch.uint8, device=dev)
-            self._decoders[key] = d
-        dec = self._decoders[key]
-        call("vd3d_km3d_decode", out.ptr, B, out.H, out.W, self.num_classes, out.cs, off["hm"], off["wh"], off["hps"], off["rot"], off["dim"],
-             off["prob"], off["reg"], off["hm_hp"], off["hp_offset"], P2.data_ptr(), float(self.test_cfg.get("score_thr", 0.1)),
-             float(self.test_cfg.get("nms_iou_thr", 0.5)), self.topk, float(W), float(H), cap, hp_cap, dec.ws.data_ptr(), dec.cap,
-             dec.scores.data_ptr(), dec.boxes.data_ptr(), dec.cls.data_ptr(), dec.anchor.data_ptr(), dec.count.data_ptr(),
-             dec.ncand.data_ptr(), E._stream())
-        self._last_decoder = dec
-        return dec
 
-    def forward_batch(self, images, P2):
+    def _peak_caps(self, n_cells):
+        return _peak_capacity(self.num_classes * n_cells), _peak_capacity(n_cells)
+
+    def _decode_scalars(self, W, H, caps):
+        return (float(W), float(H)) + caps
+
+    @staticmethod
+    def _result(scores, boxes, cls):
         # the reference's KM3D returns cls_indexes with shape [K, 1] (km3d_head.py:276 slices dets[mask, 40:41])
-        return [(s.clone(), b.clone(), c.clone().view(-1, 1)) for (s, b, c) in self.launch(images, P2).results()]
+        return scores, boxes, cls.view(-1, 1)
 
 
 def km3d_cfg(obj_types=("Car", "Pedestrian", "Cyclist")):

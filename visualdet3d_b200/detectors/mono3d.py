@@ -58,8 +58,6 @@ class LookGroundRunner:
 class _Mono3DBase(Anchor3DDetector):
     head_cls = None
 
-    N_IMAGES = 1          # images per sample of `launch` (pipeline.StreamedInference)
-
     def __init__(self, network_cfg):
         super().__init__(network_cfg)
         self.bbox_head = self.head_cls(**self.head_kwargs)
@@ -77,9 +75,7 @@ class _Mono3DBase(Anchor3DDetector):
         raise NotImplementedError
 
     def launch(self, images, P2):
-        for t, nm in ((images, "image"), (P2, "P2")):
-            E._require_cuda(t, nm)
-        images, P2 = images.float().contiguous(), P2.float().contiguous()
+        images, P2 = self._device_inputs((images, "image"), (P2, "P2"))
         B, _, H, W = images.shape
         if H % 16 or W % 16:
             raise Vd3dError(f"{type(self).__name__}: image size {H}x{W} must be a multiple of 16")
@@ -93,19 +89,6 @@ class _Mono3DBase(Anchor3DDetector):
         reg = self.run_reg(pl, feat, P2, ar)
         self._hook("cls_preds", cls), self._hook("reg_preds", reg)
         return self.decode(cls, reg, P2, H, W)
-
-    def forward_batch(self, images, P2):
-        return self.results(self.launch(images, P2))
-
-    def test_forward(self, img_batch, P2):
-        assert img_batch.shape[0] == 1   # reference contract (yolomono3d_detector.py:110)
-        return self.forward_batch(img_batch, P2)[0]
-
-    def forward(self, inputs):
-        if isinstance(inputs, list) and len(inputs) == 3:
-            return self.train_forward(*inputs)
-        img_batch, calib = inputs
-        return self.test_forward(img_batch, calib)
 
 
 @DETECTOR_DICT.register_module

@@ -15,18 +15,19 @@ stream-ordered one (graphs.GraphedStep, pipeline.StreamedInference).
 from __future__ import annotations
 
 import ctypes
-from typing import List, Optional
+from typing import List
 
 import numpy as np
 import torch
 import torch.nn as nn
 
 from .. import engine as E
+from .. import _lib
 from .._lib import Vd3dError, call
 from ..anchors import grid_anchors
 from ..plugin import DETECTOR_DICT
 from . import modules as M
-from .base import synth_load
+from .base import NativeDetector, synth_load
 from .stereo3d import ResNetRunner
 
 
@@ -35,10 +36,8 @@ class RetinaDecode(E.DecodeNms):
     the record block of parallel.pack_records_device carries the 4 box columns) plus the top-k workspace."""
 
     def __init__(self, B: int, N: int, cap: int, device):
-        super().__init__(B, cap, device)
-        from .. import _lib
+        super().__init__(B, cap, device, ws_bytes=_lib.load().vd3d_retina_decode_workspace(B, N, cap))
         self.N = N
-        self.ws = torch.empty(int(_lib.load().vd3d_retina_decode_workspace(B, N, cap)), dtype=torch.uint8, device=device)
 
     def run_levels(self, cls_levels, reg_levels, level_pix, cls_cs, reg_cs, anchors, A, ncls, nms_pre, means, stds, score_thr, iou_thr):
         L = len(level_pix)
@@ -68,9 +67,8 @@ def _cfg_get(d, k, default):
 
 
 @DETECTOR_DICT.register_module
-class RetinaNet(nn.Module):
+class RetinaNet(NativeDetector):
     """R/detectors/retinanet_2d.py:75-151 (inference).  `network_cfg` is the reference's `cfg.detector` (backbone, neck, head)."""
-    N_IMAGES = 1          # images per sample of `launch` (pipeline.StreamedInference)
 
     def __init__(self, network_cfg):
         super().__init__()
@@ -109,28 +107,9 @@ class RetinaNet(nn.Module):
                 raise ValueError(f"neck.in_channels[{i}] = {in_ch[i]} but ResNet stage {s} has {self.core.backbone.out_channels(s)} channels")
         self.bbox_head = M.RetinaHeadP(self.num_anchors, int(head.get("stacked_convs", 4)), int(head.get("in_channels", 256)),
                                        int(head.get("feat_channels", 256)), self.num_classes, self.reg_output, dict(head.get("loss_cfg", {}) or {}))
-        self._plan = None
-        self._plan_version = None
-        self._arena = E.Arena()
         self._anchors = {}
-        self._decoders = {}
-        self._last_decoder = None
-        self.stage_hook = None            # tests: callable(name, Act-or-tensor)
 
     # ---- plan (packed weights) -------------------------------------------------------------------------------
-    def _device(self):
-        return next(self.parameters()).device
-
-    def prepare(self, force: bool = False):
-        dev = self._device()
-        if dev.type != "cuda":
-            raise Vd3dError("RetinaNet has no CPU path: move the module to a CUDA device first")
-        ver = (tuple(p._version for p in self.parameters()), str(dev))
-        if self._plan is not None and not force and ver == self._plan_version:
-            return self._plan
-        self._plan, self._plan_version = self.build_plan(dev), ver
-        return self._plan
-
     def build_plan(self, dev) -> dict:
         neck, hd = self.core.neck, self.bbox_head
         conv = lambda c, **kw: E.ConvLayer(c.weight, c.bias, None, device=dev, **kw)
@@ -153,10 +132,6 @@ class RetinaNet(nn.Module):
             if l.engine != "tc16":
                 raise Vd3dError(f"RetinaNet runs on the fp16-split tensor-core engine (VD3D_CONV_ENGINE=tc16); a {l.Cin}->{l.Cout} conv got '{l.engine}'")
         return pl
-
-    def _hook(self, name, value):
-        if self.stage_hook is not None:
-            self.stage_hook(name, value)
 
     def _anchor_table(self, H, W, dev) -> torch.Tensor:
         key = (H, W, str(dev))
@@ -213,8 +188,7 @@ class RetinaNet(nn.Module):
         return list(zip(out["cls"], out["reg"]))
 
     def launch(self, images, P2=None):
-        E._require_cuda(images, "image")
-        images = images.float().contiguous()
+        [images] = self._device_inputs((images, "image"))
         B, _, H, W = images.shape
         if H % 32 or W % 32:
             raise Vd3dError(f"RetinaNet: image size {H}x{W} must be a multiple of 32 (the FPN top-down add needs every level twice the next)")
@@ -237,35 +211,14 @@ class RetinaNet(nn.Module):
         cap = self.nms_pre if 0 < self.nms_pre < N else N
         if cap > 4096:
             raise Vd3dError(f"RetinaNet: {cap} NMS candidates per image exceed the capacity (4096): set test_cfg.nms_pre <= 4096")
-        key = (B, N, cap, str(dev))
-        if key not in self._decoders:
-            self._decoders[key] = RetinaDecode(B, N, cap, dev)
-        dec = self._decoders[key]
+        dec = self._decoder((B, N, cap, str(dev)), lambda: RetinaDecode(B, N, cap, dev))
         dec.run_levels([c.t for c, _ in heads], [r.t for _, r in heads], pix, heads[0][0].cs, heads[0][1].cs, anchors, self.num_anchors,
                        self.num_classes, self.nms_pre, self.target_means, self.target_stds, self.score_thr, self.nms_iou_thr)
-        self._last_decoder = dec
         return dec
 
     @staticmethod
-    def results(dec: RetinaDecode):
-        """Per-image (scores [K], bboxes [K, 4], labels [K]) (one D2H read of the counts)."""
-        return [(s.clone(), b[:, :4].clone(), c.clone()) for (s, b, c) in dec.results()]
-
-    def forward_batch(self, images, P2: Optional[torch.Tensor] = None):
-        return self.results(self.launch(images, P2))
-
-    def test_forward(self, img_batch):
-        assert img_batch.shape[0] == 1   # reference contract (retinanet_2d.py:134)
-        return self.forward_batch(img_batch)[0]
-
-    def train_forward(self, *a, **k):
-        raise NotImplementedError("training forward is out of scope of the native inference path")
-
-    def forward(self, inputs):
-        if isinstance(inputs, list) and len(inputs) == 3:
-            return self.train_forward(*inputs)
-        img_batch, _calib = inputs
-        return self.test_forward(img_batch)
+    def _result(scores, boxes, cls):
+        return scores, boxes[:, :4], cls          # the 2-D box columns of the DecodeNms rows
 
 
 def build_synthetic_retinanet(seed: int = 0, depth: int = 50, nms_pre: int = 1000):

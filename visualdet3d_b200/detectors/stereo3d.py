@@ -341,10 +341,7 @@ class Stereo3D(Anchor3DDetector):
     def launch(self, left, right, P2, P3=None):
         """Enqueue the whole forward (backbone .. NMS) on the current stream; no host synchronisation.
         Returns the DecodeNms object holding the fixed-capacity device outputs."""
-        for t, nm in ((left, "left"), (right, "right"), (P2, "P2")):
-            E._require_cuda(t, nm)
-        left, right = left.float().contiguous(), right.float().contiguous()
-        P2 = P2.float().contiguous()
+        left, right, P2 = self._device_inputs((left, "left"), (right, "right"), (P2, "P2"))
         _, _, H, W = left.shape
         _, cls, reg = self.core_forward(left, right)
         return self.decode(cls, reg, P2, H, W)
@@ -359,6 +356,7 @@ class Stereo3D(Anchor3DDetector):
         return self.forward_batch(left_images, right_images, P2, P3)[0]
 
     def forward(self, inputs):
+        """The reference's stereo list: [left, right, P2, P3] is a test step, five or more elements a training step (raises)."""
         if isinstance(inputs, list) and len(inputs) >= 5:
             return self.train_forward(*inputs)
         return self.test_forward(*inputs)

@@ -749,12 +749,14 @@ def fp16_range_overflowed(reset: bool = True) -> bool:
 
 
 class DecodeNms:
-    """Fixed-capacity decode + NMS outputs for a batch (buffers are reused across calls)."""
+    """Fixed-capacity decode + NMS outputs for a batch (buffers are reused across calls).  `ws_bytes`: the workspace of the decode that
+    fills them (default: this anchor decode + NMS; the CenterNet and RetinaNet decodes pass their own size)."""
 
-    def __init__(self, B: int, cap: int, device):
+    def __init__(self, B: int, cap: int, device, ws_bytes=None):
         self.B, self.cap = B, cap
-        nbytes = int(_lib.load().vd3d_decode_nms_workspace(B, cap))
-        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        if ws_bytes is None:
+            ws_bytes = _lib.load().vd3d_decode_nms_workspace(B, cap)
+        self.ws = torch.empty(int(ws_bytes), dtype=torch.uint8, device=device)
         self.scores = torch.empty(B, cap, dtype=torch.float32, device=device)
         self.boxes = torch.empty(B, cap, 11, dtype=torch.float32, device=device)
         self.cls = torch.empty(B, cap, dtype=torch.int64, device=device)
