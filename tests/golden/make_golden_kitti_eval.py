@@ -189,6 +189,29 @@ def run_reference(E, KE, KC, ids, labels, results, classes, one_part):
     return texts, captured, ious, gt_annos, dt_annos
 
 
+def store_case(out, name, ids, labels, results, classes, texts, captured, ious, gt_annos, dt_annos):
+    """One case under the keys `name/...` (what tests/test_kitti_eval_cpu.py::write_case and the GPU tests read); returns (ng, nd)."""
+    p = f"{name}/"
+    out.update({p + "ids": ids, p + "label_text": np.array(labels), p + "result_text": np.array(results),
+                p + "classes": np.array(classes, dtype=np.int64), p + "texts": np.array(texts)})
+    for m in ("bbox", "bev", "3d"):
+        for key in ("precision", "thresholds", "orientation"):
+            if key == "orientation" and m != "bbox":
+                continue
+            out[p + f"{m}_{key}"] = np.concatenate([r[m][key] for r in captured], 0)
+    ng = np.array([len(a["name"]) for a in gt_annos])
+    nd = np.array([len(a["name"]) for a in dt_annos])
+    out[p + "ng"], out[p + "nd"] = ng, nd
+    out[p + "overlaps"] = np.stack([np.concatenate([o.reshape(-1) for o in ious[m]]) for m in range(3)])
+    for who, annos in (("gt", gt_annos), ("dt", dt_annos)):
+        out[p + f"{who}_name"] = np.array([n for a in annos for n in a["name"]], dtype=str)   # an empty file parses to float64
+        for k in ANNO_KEYS[1:]:
+            out[p + f"{who}_{k}"] = np.concatenate([a[k] for a in annos], 0)
+    per_image = [np.stack([ious[1][i], ious[2][i]]) for i in range(len(ids))]
+    out[p + "margin"] = np.float64(margin_of(per_image))
+    return ng, nd
+
+
 def main():
     refload.load_reference()
     import visualDet3D.evaluator.kitti.eval as E
@@ -210,25 +233,8 @@ def main():
         ids, labels, results = make_case(E, KC, c["seed"], c["n_img"], c.get("two_d", False), c.get("no_cyclist_gt", False),
                                          c.get("dontcare", True))
         texts, captured, ious, gt_annos, dt_annos = run_reference(E, KE, KC, ids, labels, results, c["classes"], c["n_img"] < 50)
-        p = f"{name}/"
-        out.update({p + "ids": ids, p + "label_text": np.array(labels), p + "result_text": np.array(results),
-                    p + "classes": np.array(c["classes"], dtype=np.int64), p + "texts": np.array(texts)})
-        for m in ("bbox", "bev", "3d"):
-            for key in ("precision", "thresholds", "orientation"):
-                if key == "orientation" and m != "bbox":
-                    continue
-                out[p + f"{m}_{key}"] = np.concatenate([r[m][key] for r in captured], 0)
-        ng = np.array([len(a["name"]) for a in gt_annos])
-        nd = np.array([len(a["name"]) for a in dt_annos])
-        out[p + "ng"], out[p + "nd"] = ng, nd
-        out[p + "overlaps"] = np.stack([np.concatenate([o.reshape(-1) for o in ious[m]]) for m in range(3)])
-        for who, annos in (("gt", gt_annos), ("dt", dt_annos)):
-            out[p + f"{who}_name"] = np.array([n for a in annos for n in a["name"]], dtype=str)   # an empty file parses to float64
-            for k in ANNO_KEYS[1:]:
-                out[p + f"{who}_{k}"] = np.concatenate([a[k] for a in annos], 0)
-        per_image = [np.stack([ious[1][i], ious[2][i]]) for i in range(len(ids))]
-        out[p + "margin"] = np.float64(margin_of(per_image))
-        print(f"{name}: {len(ids)} images, {ng.sum()} gt, {nd.sum()} dt, margin {float(out[p + 'margin']):.3g}")
+        ng, nd = store_case(out, name, ids, labels, results, c["classes"], texts, captured, ious, gt_annos, dt_annos)
+        print(f"{name}: {len(ids)} images, {ng.sum()} gt, {nd.sum()} dt, margin {float(out[name + '/margin']):.3g}")
         print(texts[0])
     np.savez_compressed(os.path.join(HERE, "kitti_eval.npz"), **out)
 
