@@ -380,7 +380,8 @@ CN_HEADS = {"MonoFlex": {"hm": CN_NCLS, "bbox2d": 4, "hps": 20, "rot": 8, "dim":
 
 def cn_maps(kind, peaks, seed=0, hm_fill=None):
     """head maps {name: [B, n, H, W]}: heat logit -10 (sigmoid far below 0.1) except at `peaks` (one list of (c, y, x, logit) per
-    image); box regressions on the 0.5 grid so that box columns 0..3 are exact; the rest random."""
+    image, or (c, y, x, logit, box): the box regression at (y, x) decodes to box = (x1, y1, x2, y2), integers in image pixels); box
+    regressions on the 0.5 grid so that box columns 0..3 are exact; the rest random."""
     rng = np.random.default_rng(seed)
     B = len(peaks)
     m = {}
@@ -390,7 +391,7 @@ def cn_maps(kind, peaks, seed=0, hm_fill=None):
     for b, pk in enumerate(peaks):
         if hm_fill is not None and hm_fill[b] is not None:
             m["hm"][b].fill_(hm_fill[b])
-        for c, y, x, lg in pk:
+        for c, y, x, lg, *_ in pk:
             m["hm"][b, c, y, x] = float(lg)
     m["dim"] = torch.from_numpy(rng.uniform(1, 4, (B, 3, CN_H, CN_W)).astype(F32))
     if kind == "MonoFlex":
@@ -400,6 +401,16 @@ def cn_maps(kind, peaks, seed=0, hm_fill=None):
         m["reg"] = torch.from_numpy(half(rng.uniform(0, 1, (B, 2, CN_H, CN_W))))
         m["hm_hp"].fill_(-10.0)
         m["hp_offset"].zero_()
+    for b, pk in enumerate(peaks):
+        for c, y, x, _, *box in pk:
+            if not box:
+                continue
+            x1, y1, x2, y2 = box[0]                            # quarters / eighths of integers: every step below is exact
+            if kind == "MonoFlex":                             # 4 * (x - l, y - t, x + r, y + b)
+                m["bbox2d"][b, :, y, x] = torch.tensor([x - x1 / 4, y - y1 / 4, x2 / 4 - x, y2 / 4 - y])
+            else:                                              # 4 * (x + dx -+ w / 2, y + dy -+ h / 2)
+                m["reg"][b, :, y, x] = torch.tensor([(x1 + x2) / 8 - x, (y1 + y2) / 8 - y])
+                m["wh"][b, :, y, x] = torch.tensor([(x2 - x1) / 4, (y2 - y1) / 4])
     return m
 
 
@@ -450,6 +461,29 @@ def _isolated(n, scores, rng, classes=CN_NCLS):
     return [cells[i] + (lg[j],) for j, i in enumerate(pick)]
 
 
+SWEEP_N, SWEEP_PAIR, SWEEP_CHAIN = 90, 10, 61
+
+
+def _sweep_peaks(rng):
+    """SWEEP_N isolated peaks in score order with chosen boxes: disjoint 8 x 8 tiles, except a pair at sorted positions SWEEP_PAIR and
+    SWEEP_PAIR + 1 nested at IoU exactly 0.5 (8 x 8 and 8 x 4 sharing a corner), and a staircase over positions SWEEP_CHAIN .. + 5
+    (IoU 14/26 with a neighbour, 8/32 with the next one) that crosses sorted positions 63 / 64"""
+    pk = _isolated(SWEEP_N, score_ladder(SWEEP_N), rng, classes=1)      # one class: the box regression maps are shared by all
+    pk = [(int(k), y, x, lg) for (_, y, x, lg), k in zip(pk, rng.integers(0, CN_NCLS, SWEEP_N))]
+    tiles = iter((10 * (i % 16) + 1, 10 * (i // 16) + 1) for i in range(96))
+    boxes = []
+    for p in range(SWEEP_N):
+        if p in (SWEEP_PAIR, SWEEP_PAIR + 1):
+            boxes.append((60, 70, 68, 78 if p == SWEEP_PAIR else 74))
+        elif SWEEP_CHAIN <= p < SWEEP_CHAIN + 6:
+            x1 = 1 + 6 * (p - SWEEP_CHAIN)
+            boxes.append((x1, 70, x1 + 20, 80))
+        else:
+            x1, y1 = next(tiles)
+            boxes.append((x1, y1, x1 + 8, y1 + 8))
+    return [q + (bx,) for q, bx in zip(pk, boxes)]
+
+
 def cn_cases():
     """name -> (peaks per image, hm_fill per image or None, tie_free: the reference's topk order is defined, plateau cells to check)"""
     rng = np.random.default_rng(3)
@@ -483,6 +517,8 @@ def cn_cases():
     cases["class_ties_at_K"] = ([_isolated(95, score_ladder(95, hi=0.9995, lo=0.98), rng) + tie], None, False, dict(peaks=[], not_peaks=[]))
     # peak-capacity overflow: image 0 is one plateau of heat 0.5 over every cell of every class
     cases["overflow"] = ([[], pl], [0.0, None], False, dict(peaks=[], not_peaks=[]))
+    # more than 64 kept rows, a suppression chain across sorted positions 63 / 64 and a pair at IoU exactly nms_iou_thr (kept)
+    cases["sweep_words"] = ([_sweep_peaks(rng)], None, True, dict(peaks=[], not_peaks=[]))
     return cases
 
 
@@ -644,6 +680,13 @@ def test_centernet_cases_are_what_they_claim(kind):
                 assert sorted(s.tolist()) == sorted(rs.tolist()) or name == "plateaus", name
     peaks = cn_cases()["K_and_K+1"][0]
     assert [len(p) for p in peaks] == [CN_K, CN_K + 1]
+    pk = cn_cases()["sweep_words"][0][0]
+    s, flat, bx = cn_restate(kind, cn_maps(kind, [pk], seed=1), 0, thr, iou)
+    kept = [p for p in range(SWEEP_N) if p not in (SWEEP_CHAIN + 1, SWEEP_CHAIN + 3, SWEEP_CHAIN + 5)]   # 63 kept suppresses 64
+    assert SWEEP_CHAIN + 3 == 64 and len(kept) > 64
+    assert flat.tolist() == [(pk[p][0] * CN_H + pk[p][1]) * CN_W + pk[p][2] for p in kept]
+    assert torch.equal(bx, torch.tensor([pk[p][4] for p in kept], dtype=torch.float32))
+    assert F32(tv_iou(pk[SWEEP_PAIR][4], pk[SWEEP_PAIR + 1][4])) == F32(iou)
     maps = cn_maps(kind, cn_cases()["plateaus"][0], seed=1)
     heat = torch.sigmoid(maps["hm"])
     assert int((heat[0, 2, 15:17, 30:32] == 1).sum()) == 4 and int((heat[0, 0, 3:6, 30:33] == 1).sum()) == 9

@@ -7,7 +7,7 @@
 //
 // Order equivalence: the reference keeps the K best peaks, then drops scores <= score_thr; selecting peaks > score_thr first
 // and keeping the best K of those yields the same set and order (scores are sorted descending, ties by flat index).
-#include "common.cuh"
+#include "decode_common.cuh"
 #include "km3d_position.cuh"
 
 namespace vd3d {
@@ -16,18 +16,18 @@ struct CnLayout {            // channel offsets inside the concatenated head-out
     int cs, hm, bbox2d, hps, rot, dim, reg, depth, dunc, cunc;
 };
 
-__device__ __forceinline__ float sigm(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-x))); }
-
-// ---- stage 1: peaks above the threshold -> unordered (key, flat index) list ------------------------------------------------
-__global__ void cn_peaks_kernel(const float* __restrict__ out, int B, int H, int W, int ncls, CnLayout L, float score_thr, int cap,
-                                unsigned long long* __restrict__ keys, int* __restrict__ ncand) {
+// ---- stage 1: peaks (3x3 local maxima) of channels base .. base + nch - 1 above thr -> unordered key lists ----------------------------
+// per_channel: one list per (image, channel) with index y * W + x (KM3D's keypoint joints); otherwise one list per image with the flat
+// index (c * H + y) * W + x.
+__global__ void cn_peaks_kernel(const float* __restrict__ out, int B, int H, int W, int cs, int base, int nch, bool per_channel, float thr,
+                                int cap, unsigned long long* __restrict__ keys, int* __restrict__ ncand) {
     long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total = (long long)B * ncls * H * W;
+    long long total = (long long)B * nch * H * W;
     if (idx >= total) return;
-    int w = (int)(idx % W); long long r = idx / W; int h = (int)(r % H); r /= H; int c = (int)(r % ncls); int b = (int)(r / ncls);
-    const float* base = out + ((long long)b * H * W) * L.cs + L.hm + c;
-    float s = sigm(__ldg(base + ((long long)h * W + w) * L.cs));
-    if (!(s > score_thr)) return;
+    int w = (int)(idx % W); long long r = idx / W; int h = (int)(r % H); r /= H; int c = (int)(r % nch); int b = (int)(r / nch);
+    const float* p = out + ((long long)b * H * W) * cs + base + c;
+    float s = sigmoid_ref(__ldg(p + ((long long)h * W + w) * cs));
+    if (!(s > thr)) return;
     float m = s;
 #pragma unroll
     for (int dy = -1; dy <= 1; ++dy)
@@ -35,18 +35,19 @@ __global__ void cn_peaks_kernel(const float* __restrict__ out, int B, int H, int
         for (int dx = -1; dx <= 1; ++dx) {
             int hh = h + dy, ww = w + dx;
             if ((dy | dx) == 0 || hh < 0 || hh >= H || ww < 0 || ww >= W) continue;
-            m = fmaxf(m, sigm(__ldg(base + ((long long)hh * W + ww) * L.cs)));
+            m = fmaxf(m, sigmoid_ref(__ldg(p + ((long long)hh * W + ww) * cs)));
         }
     if (m != s) return;                                  // keep = (hmax == heat)
-    int slot = atomicAdd(ncand + b, 1);
+    const int list = per_channel ? b * nch + c : b;
+    int slot = atomicAdd(ncand + list, 1);
     if (slot >= cap) return;
-    unsigned int flat = (unsigned int)((c * H + h) * W + w);
-    keys[(long long)b * cap + slot] = ((unsigned long long)(~__float_as_uint(s)) << 32) | flat;
+    keys[(long long)list * cap + slot] = score_key(s, (unsigned int)((per_channel ? h : c * H + h) * W + w));
 }
 
 // ---- stage 2: one CTA per image: sort, keep K, decode, NMS ----------------------------------------------------------------
 constexpr int CN_THREADS = 1024;
 constexpr int CN_MAXK = 128;
+constexpr int CN_MASK_WPR = CN_MAXK / 64;      // words per row of the NMS sweep's suppression mask
 
 __global__ void __launch_bounds__(CN_THREADS) cn_decode_nms_kernel(
     const float* __restrict__ out, const float* __restrict__ P2, int H, int W, int ncls, CnLayout L, int cap, int cap_pow2, int K,
@@ -57,31 +58,21 @@ __global__ void __launch_bounds__(CN_THREADS) cn_decode_nms_kernel(
     extern __shared__ __align__(16) unsigned char sm_raw[];
     unsigned long long* skey = reinterpret_cast<unsigned long long*>(sm_raw);            // [cap_pow2]
     __shared__ float sbox[CN_MAXK][11];
+    __shared__ float4 sbox4[CN_MAXK];
     __shared__ float sarea[CN_MAXK];
-    __shared__ unsigned char ssup[CN_MAXK];
-    __shared__ int s_nkeep;
+    __shared__ int skeep[CN_MAXK];
+    __shared__ unsigned long long smask[64 * CN_MASK_WPR];
     const int b = blockIdx.x, t = threadIdx.x;
     int n = ncand[b];
     if (t == 0) o_ncand[b] = n;
     if (n > cap) { if (t == 0) o_count[b] = -1; return; }
-    { int n2 = 2; while (n2 < n) n2 <<= 1; cap_pow2 = n2 < cap_pow2 ? n2 : cap_pow2; }      // sort only the occupied power of two (block-uniform)
+    cap_pow2 = min(next_pow2(n, 2), cap_pow2);          // sort only the occupied power of two (block-uniform)
     for (int i = t; i < cap_pow2; i += CN_THREADS) skey[i] = (i < n) ? keys[(long long)b * cap + i] : ~0ull;
     __syncthreads();
-    for (int k = 2; k <= cap_pow2; k <<= 1)
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = t; i < cap_pow2; i += CN_THREADS) {
-                int ixj = i ^ j;
-                if (ixj > i) {
-                    bool up = ((i & k) == 0);
-                    unsigned long long a = skey[i], c = skey[ixj];
-                    if ((a > c) == up) { skey[i] = c; skey[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
+    block_sort<CN_THREADS, false>(skey, nullptr, cap_pow2);
     const int nk = min(n, K);
     if (t < nk) {
-        unsigned int flat = (unsigned int)(skey[t] & 0xffffffffu);
+        unsigned int flat = key_index(skey[t]);
         int x = flat % W; int r = flat / W; int y = r % H;
         const float* px = out + (((long long)b * H + y) * W + x) * L.cs;
         float xs = (float)x, ys = (float)y;
@@ -120,37 +111,25 @@ __global__ void __launch_bounds__(CN_THREADS) cn_decode_nms_kernel(
         float* sb = sbox[t];
         sb[0] = bx1; sb[1] = by1; sb[2] = bx2; sb[3] = by2; sb[4] = cx; sb[5] = cy; sb[6] = z;
         sb[7] = px[L.dim + 0]; sb[8] = px[L.dim + 1]; sb[9] = px[L.dim + 2]; sb[10] = alpha;
-        sarea[t] = __fmul_rn(__fsub_rn(bx2, bx1), __fsub_rn(by2, by1));
-        ssup[t] = 0;
+        const float4 bx = make_float4(bx1, by1, bx2, by2);
+        sbox4[t] = bx;
+        sarea[t] = box_area(bx);
     }
-    if (t == 0) s_nkeep = 0;
     __syncthreads();
-    for (int i = 0; i < nk; ++i) {
-        if (ssup[i]) continue;
-        for (int j = i + 1 + t; j < nk; j += CN_THREADS) {
-            if (ssup[j]) continue;
-            float xx1 = fmaxf(sbox[i][0], sbox[j][0]), yy1 = fmaxf(sbox[i][1], sbox[j][1]);
-            float xx2 = fminf(sbox[i][2], sbox[j][2]), yy2 = fminf(sbox[i][3], sbox[j][3]);
-            float w = fmaxf(0.f, __fsub_rn(xx2, xx1)), h = fmaxf(0.f, __fsub_rn(yy2, yy1));
-            float inter = __fmul_rn(w, h);
-            float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(sarea[i], sarea[j]), inter));
-            if ((double)ovr > iou_thr) ssup[j] = 1;
-        }
-        if (t == 0) {
-            int k = s_nkeep++;
-            unsigned long long key = skey[i];
-            unsigned int flat = (unsigned int)(key & 0xffffffffu);
-            o_scores[(long long)b * out_cap + k] = __uint_as_float(~(unsigned int)(key >> 32));
-            o_index[(long long)b * out_cap + k] = (int)flat;
-            o_cls[(long long)b * out_cap + k] = (long long)(flat / (unsigned int)(H * W));
-            float* op = o_boxes + ((long long)b * out_cap + k) * 11;
+    const int nkeep = nms_sweep<CN_THREADS>(sbox4, sarea, nk, CN_MASK_WPR, iou_thr, smask, skeep);
+    // ordered write-out of the kept rows, one per thread (nkeep <= K < CN_THREADS)
+    if (t < nkeep) {
+        const int k = t, i = skeep[k];
+        const unsigned long long key = skey[i];
+        const unsigned int flat = key_index(key);
+        o_scores[(long long)b * out_cap + k] = key_score(key);
+        o_index[(long long)b * out_cap + k] = (int)flat;
+        o_cls[(long long)b * out_cap + k] = (long long)(flat / (unsigned int)(H * W));
+        float* op = o_boxes + ((long long)b * out_cap + k) * 11;
 #pragma unroll
-            for (int q = 0; q < 11; ++q) op[q] = sbox[i][q];
-        }
-        __syncthreads();
+        for (int q = 0; q < 11; ++q) op[q] = sbox[i][q];
     }
-    __syncthreads();
-    if (t == 0) o_count[b] = s_nkeep;
+    if (t == 0) o_count[b] = nkeep;
 }
 
 // ================================================================================================================
@@ -158,51 +137,11 @@ __global__ void __launch_bounds__(CN_THREADS) cn_decode_nms_kernel(
 // ================================================================================================================
 struct KmLayout { int cs, hm, wh, hps, rot, dim, prob, reg, hm_hp, hp_offset; };
 
-// peaks of the per-joint keypoint heat map above `thr` -> per (image, joint) unordered key list
-__global__ void km_hp_peaks_kernel(const float* __restrict__ out, int B, int H, int W, int J, KmLayout L, float thr, int cap,
-                                   unsigned long long* __restrict__ keys, int* __restrict__ ncand) {
-    long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total = (long long)B * J * H * W;
-    if (idx >= total) return;
-    int w = (int)(idx % W); long long r = idx / W; int h = (int)(r % H); r /= H; int j = (int)(r % J); int b = (int)(r / J);
-    const float* base = out + ((long long)b * H * W) * L.cs + L.hm_hp + j;
-    float s = sigm(__ldg(base + ((long long)h * W + w) * L.cs));
-    if (!(s > thr)) return;
-    float m = s;
-#pragma unroll
-    for (int dy = -1; dy <= 1; ++dy)
-#pragma unroll
-        for (int dx = -1; dx <= 1; ++dx) {
-            int hh = h + dy, ww = w + dx;
-            if ((dy | dx) == 0 || hh < 0 || hh >= H || ww < 0 || ww >= W) continue;
-            m = fmaxf(m, sigm(__ldg(base + ((long long)hh * W + ww) * L.cs)));
-        }
-    if (m != s) return;
-    int slot = atomicAdd(ncand + b * J + j, 1);
-    if (slot >= cap) return;
-    keys[((long long)b * J + j) * cap + slot] = ((unsigned long long)(~__float_as_uint(s)) << 32) | (unsigned int)(h * W + w);
-}
-
-__device__ void bitonic_sort_u64(unsigned long long* k, int n_pow2, int t, int nthreads) {
-    for (int sz = 2; sz <= n_pow2; sz <<= 1)
-        for (int j = sz >> 1; j > 0; j >>= 1) {
-            for (int i = t; i < n_pow2; i += nthreads) {
-                int ixj = i ^ j;
-                if (ixj > i) {
-                    bool up = ((i & sz) == 0);
-                    unsigned long long a = k[i], c = k[ixj];
-                    if ((a > c) == up) { k[i] = c; k[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-}
-
 constexpr int KM_J = 9;
 
 __global__ void __launch_bounds__(CN_THREADS) km3d_decode_nms_kernel(
     const float* __restrict__ out, const float* __restrict__ P2, int H, int W, int ncls, KmLayout L, int cap, int cap_pow2, int hp_cap,
-    int hp_cap_pow2, int K, float score_thr, double iou_thr, float img_w, float img_h, int out_cap,
+    int hp_cap_pow2, int K, double iou_thr, float img_w, float img_h, int out_cap,
     const unsigned long long* __restrict__ keys, const int* __restrict__ ncand,
     const unsigned long long* __restrict__ hp_keys, const int* __restrict__ hp_ncand,
     float* __restrict__ o_scores, float* __restrict__ o_boxes, long long* __restrict__ o_cls, int* __restrict__ o_index,
@@ -213,9 +152,10 @@ __global__ void __launch_bounds__(CN_THREADS) km3d_decode_nms_kernel(
     __shared__ int hpn[KM_J];
     __shared__ unsigned long long dkey[CN_MAXK];
     __shared__ float sbox[CN_MAXK][11];
+    __shared__ float4 sbox4[CN_MAXK];
     __shared__ float sarea[CN_MAXK];
-    __shared__ unsigned char ssup[CN_MAXK], svalid[CN_MAXK];
-    __shared__ int s_nkeep;
+    __shared__ int skeep[CN_MAXK];
+    __shared__ unsigned long long smask[64 * CN_MASK_WPR];
     const int b = blockIdx.x, t = threadIdx.x;
     int n = ncand[b];
     if (t == 0) o_ncand[b] = n;
@@ -223,40 +163,37 @@ __global__ void __launch_bounds__(CN_THREADS) km3d_decode_nms_kernel(
     for (int j = 0; j < KM_J; ++j) overflow = overflow || hp_ncand[b * KM_J + j] > hp_cap;
     if (overflow) { if (t == 0) o_count[b] = -1; return; }      // fixed-capacity candidate lists overflowed: reported, never silently truncated
     // ---- detection peaks: sort, keep the best K -----------------------------------------------------------------------------
-    { int n2 = 2; while (n2 < n) n2 <<= 1; cap_pow2 = n2 < cap_pow2 ? n2 : cap_pow2; }      // sort only the occupied power of two (block-uniform)
+    cap_pow2 = min(next_pow2(n, 2), cap_pow2);          // sort only the occupied power of two (block-uniform)
     for (int i = t; i < cap_pow2; i += CN_THREADS) skey[i] = (i < n) ? keys[(long long)b * cap + i] : ~0ull;
     __syncthreads();
-    bitonic_sort_u64(skey, cap_pow2, t, CN_THREADS);
+    block_sort<CN_THREADS, false>(skey, nullptr, cap_pow2);
     const int nk = min(n, K);
     if (t < nk) dkey[t] = skey[t];
     __syncthreads();
     // ---- keypoint heat-map peaks per joint: best K of those above 0.1, with their sub-pixel offsets ---------------------------
     for (int j = 0; j < KM_J; ++j) {
         int nj = min(hp_ncand[b * KM_J + j], hp_cap);
-        int hp2 = 2; while (hp2 < nj) hp2 <<= 1;
-        hp2 = hp2 < hp_cap_pow2 ? hp2 : hp_cap_pow2;
+        const int hp2 = min(next_pow2(nj, 2), hp_cap_pow2);
         __syncthreads();                                     // the previous joint's readers of skey are done
         for (int i = t; i < hp2; i += CN_THREADS) skey[i] = (i < nj) ? hp_keys[((long long)b * KM_J + j) * hp_cap + i] : ~0ull;
         __syncthreads();
-        bitonic_sort_u64(skey, hp2, t, CN_THREADS);
+        block_sort<CN_THREADS, false>(skey, nullptr, hp2);
         int m = min(nj, K);
         if (t < m) {
             unsigned long long key = skey[t];
-            unsigned int flat = (unsigned int)(key & 0xffffffffu);
+            unsigned int flat = key_index(key);
             int x = flat % W, y = flat / W;
             const float* px = out + (((long long)b * H + y) * W + x) * L.cs;
             hpx[j][t] = (float)x + px[L.hp_offset + 0];
             hpy[j][t] = (float)y + px[L.hp_offset + 1];
-            hps_[j][t] = __uint_as_float(~(unsigned int)(key >> 32));
+            hps_[j][t] = key_score(key);
         }
         if (t == 0) hpn[j] = m;
         __syncthreads();
     }
     // ---- per detection decode --------------------------------------------------------------------------------------------------
     if (t < nk) {
-        unsigned long long key = dkey[t];
-        float score = __uint_as_float(~(unsigned int)(key >> 32));
-        unsigned int flat = (unsigned int)(key & 0xffffffffu);
+        unsigned int flat = key_index(dkey[t]);
         int x = flat % W; int r = flat / W; int y = r % H;
         const float* px = out + (((long long)b * H + y) * W + x) * L.cs;
         float xs0 = (float)x, ys0 = (float)y;
@@ -299,38 +236,25 @@ __global__ void __launch_bounds__(CN_THREADS) km3d_decode_nms_kernel(
         l = fmaxf(l, 0.f); tp = fmaxf(tp, 0.f); rr = fminf(rr, img_w); bt = fminf(bt, img_h);
         float* sb = sbox[t];
         sb[0] = l; sb[1] = tp; sb[2] = rr; sb[3] = bt; sb[4] = cx3; sb[5] = cy3; sb[6] = z3; sb[7] = dw; sb[8] = dh; sb[9] = dl; sb[10] = alpha;
-        sarea[t] = __fmul_rn(__fsub_rn(rr, l), __fsub_rn(bt, tp));
-        ssup[t] = 0;
-        svalid[t] = score > score_thr;
+        const float4 bx = make_float4(l, tp, rr, bt);
+        sbox4[t] = bx;
+        sarea[t] = box_area(bx);
     }
-    if (t == 0) s_nkeep = 0;
     __syncthreads();
-    for (int i = 0; i < nk; ++i) {
-        if (ssup[i] || !svalid[i]) continue;
-        for (int j = i + 1 + t; j < nk; j += CN_THREADS) {
-            if (ssup[j] || !svalid[j]) continue;
-            float xx1 = fmaxf(sbox[i][0], sbox[j][0]), yy1 = fmaxf(sbox[i][1], sbox[j][1]);
-            float xx2 = fminf(sbox[i][2], sbox[j][2]), yy2 = fminf(sbox[i][3], sbox[j][3]);
-            float w = fmaxf(0.f, __fsub_rn(xx2, xx1)), h = fmaxf(0.f, __fsub_rn(yy2, yy1));
-            float inter = __fmul_rn(w, h);
-            float ovr = __fdiv_rn(inter, __fsub_rn(__fadd_rn(sarea[i], sarea[j]), inter));
-            if ((double)ovr > iou_thr) ssup[j] = 1;
-        }
-        if (t == 0) {
-            int k = s_nkeep++;
-            unsigned long long key = dkey[i];
-            unsigned int flat = (unsigned int)(key & 0xffffffffu);
-            o_scores[(long long)b * out_cap + k] = __uint_as_float(~(unsigned int)(key >> 32));
-            o_index[(long long)b * out_cap + k] = (int)flat;
-            o_cls[(long long)b * out_cap + k] = (long long)(flat / (unsigned int)(H * W));
-            float* op = o_boxes + ((long long)b * out_cap + k) * 11;
+    const int nkeep = nms_sweep<CN_THREADS>(sbox4, sarea, nk, CN_MASK_WPR, iou_thr, smask, skeep);
+    // ordered write-out of the kept rows, one per thread (nkeep <= K < CN_THREADS)
+    if (t < nkeep) {
+        const int k = t, i = skeep[k];
+        const unsigned long long key = dkey[i];
+        const unsigned int flat = key_index(key);
+        o_scores[(long long)b * out_cap + k] = key_score(key);
+        o_index[(long long)b * out_cap + k] = (int)flat;
+        o_cls[(long long)b * out_cap + k] = (long long)(flat / (unsigned int)(H * W));
+        float* op = o_boxes + ((long long)b * out_cap + k) * 11;
 #pragma unroll
-            for (int q = 0; q < 11; ++q) op[q] = sbox[i][q];
-        }
-        __syncthreads();
+        for (int q = 0; q < 11; ++q) op[q] = sbox[i][q];
     }
-    __syncthreads();
-    if (t == 0) o_count[b] = s_nkeep;
+    if (t == 0) o_count[b] = nkeep;
 }
 
 }  // namespace vd3d
@@ -353,9 +277,9 @@ extern "C" int vd3d_monoflex_decode(const float* heads, int B, int H, int W, int
     int* ncand = (int*)((unsigned char*)wsp + (long long)B * cap * 8);
     VD3D_CUDA(cudaMemsetAsync(ncand, 0, sizeof(int) * B, st));
     long long total = (long long)B * ncls * H * W;
-    cn_peaks_kernel<<<cdiv(total, 256), 256, 0, st>>>(heads, B, H, W, ncls, L, score_thr, cap, keys, ncand);
+    cn_peaks_kernel<<<cdiv(total, 256), 256, 0, st>>>(heads, B, H, W, cs, hm_co, ncls, false, score_thr, cap, keys, ncand);
     VD3D_CHECK_LAUNCH("cn_peaks");
-    int cp2 = 1; while (cp2 < cap) cp2 <<= 1;
+    int cp2 = next_pow2(cap);
     size_t smem = (size_t)cp2 * 8;
     VD3D_CUDA(cudaFuncSetAttribute(cn_decode_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cn_decode_nms_kernel<<<B, CN_THREADS, smem, st>>>(heads, P2, H, W, ncls, L, cap, cp2, K, unc_lo, unc_hi, iou_thr, img_w, img_h, out_cap,
@@ -379,24 +303,24 @@ extern "C" int vd3d_km3d_decode(const float* heads, int B, int H, int W, int ncl
     VD3D_REQUIRE(score_thr > 0.f, "km3d_decode: score_thr must be positive");
     cudaStream_t st = (cudaStream_t)stream;
     KmLayout L{cs, hm_co, wh_co, hps_co, rot_co, dim_co, prob_co, reg_co, hm_hp_co, hp_offset_co};
-    CnLayout Lc{cs, hm_co, 0, 0, 0, 0, 0, 0, 0, 0};
     unsigned char* p = (unsigned char*)wsp;
     unsigned long long* keys = (unsigned long long*)p; p += (long long)B * cap * 8;
     unsigned long long* hp_keys = (unsigned long long*)p; p += (long long)B * 9 * hp_cap * 8;
     int* ncand = (int*)p; int* hp_ncand = ncand + B;
     VD3D_CUDA(cudaMemsetAsync(ncand, 0, sizeof(int) * B * 10, st));
-    // detection peaks: the reference keeps the K best then drops scores <= score_thr; pre-filtering with the threshold is equivalent
+    // detection peaks: the reference keeps the K best then drops scores <= score_thr; pre-filtering with the threshold is equivalent, and
+    // it is the only score test: every decoded peak is above score_thr
     long long total = (long long)B * ncls * H * W;
-    cn_peaks_kernel<<<cdiv(total, 256), 256, 0, st>>>(heads, B, H, W, ncls, Lc, score_thr, cap, keys, ncand);
+    cn_peaks_kernel<<<cdiv(total, 256), 256, 0, st>>>(heads, B, H, W, cs, hm_co, ncls, false, score_thr, cap, keys, ncand);
     VD3D_CHECK_LAUNCH("km3d_peaks");
     long long total_hp = (long long)B * 9 * H * W;
-    km_hp_peaks_kernel<<<cdiv(total_hp, 256), 256, 0, st>>>(heads, B, H, W, 9, L, 0.1f, hp_cap, hp_keys, hp_ncand);
+    cn_peaks_kernel<<<cdiv(total_hp, 256), 256, 0, st>>>(heads, B, H, W, cs, hm_hp_co, 9, true, 0.1f, hp_cap, hp_keys, hp_ncand);
     VD3D_CHECK_LAUNCH("km3d_hp_peaks");
-    int cp2 = 1; while (cp2 < cap) cp2 <<= 1;
-    int hp2 = 1; while (hp2 < hp_cap) hp2 <<= 1;
+    int cp2 = next_pow2(cap);
+    int hp2 = next_pow2(hp_cap);
     size_t smem = (size_t)(cp2 > hp2 ? cp2 : hp2) * 8;
     VD3D_CUDA(cudaFuncSetAttribute(km3d_decode_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    km3d_decode_nms_kernel<<<B, CN_THREADS, smem, st>>>(heads, P2, H, W, ncls, L, cap, cp2, hp_cap, hp2, K, score_thr, iou_thr, img_w, img_h,
+    km3d_decode_nms_kernel<<<B, CN_THREADS, smem, st>>>(heads, P2, H, W, ncls, L, cap, cp2, hp_cap, hp2, K, iou_thr, img_w, img_h,
                                                        out_cap, keys, ncand, hp_keys, hp_ncand, out_scores, out_boxes, out_cls, out_index,
                                                        out_count, out_ncand);
     VD3D_CHECK_LAUNCH("km3d_decode_nms");

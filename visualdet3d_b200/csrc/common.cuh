@@ -44,6 +44,8 @@ constexpr float kFp16Overflow = 65520.0f;      // smallest magnitude that rounds
     } while (0)
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+// the least power of two >= v, and >= lo (a power of two)
+__host__ __device__ __forceinline__ int next_pow2(int v, int lo = 1) { int p = lo; while (p < v) p <<= 1; return p; }
 
 constexpr int kNumSMs = 132;  // H100 SXM: persistent grids and tile-cost models
 

@@ -6,14 +6,10 @@
 // comparisons whose operands are computed with the SAME operation order as the reference's eager ops and with
 // FMA contraction disabled (explicit __fmul_rn/__fadd_rn/__fdiv_rn), so they only differ where the CUDA libm
 // (expf/atan2f) differs from the host libm by an ulp on a knife edge.
-#include "common.cuh"
+#include "decode_common.cuh"
 #include <cstring>
 
 namespace vd3d {
-
-__device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b); }
 
 // ---------------------------------------------------------------------------------------------------------
 // useful mask (R/heads/anchors.py:93-111)
@@ -46,11 +42,6 @@ __global__ void anchor_mask_kernel(const float* __restrict__ anchors, const floa
 // index-ordered candidate list.
 // workspace layout per image: keys u64[cap], boxes f32[cap][11], labels i32[cap]
 // ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float sigmoidf_ref(float x) {
-    // torch CPU sigmoid: 1 / (1 + exp(-x))
-    return __fdiv_rn(1.0f, add(1.0f, expf(-x)));
-}
-
 struct DecodeWs {
     unsigned long long* keys;   // [B][cap]
     float* boxes;               // [B][cap][11]
@@ -68,14 +59,14 @@ __global__ void decode_candidates_kernel(const float* __restrict__ cls, const fl
     const float* cp = cls + idx * (ncls + 1);
     float best = -1.f; int label = 0;
     for (int c = 0; c < ncls; ++c) {
-        float p = sigmoidf_ref(__ldg(cp + c));
+        float p = sigmoid_ref(__ldg(cp + c));
         if (p > best) { best = p; label = c; }     // first maximum wins (torch.max over dim)
     }
     if (!(best > score_thr)) return;
     const float* ms = mean_std + ((long long)n * T + label) * 12;   // [6][2]
     float z_mean = __ldg(ms + 0);
     if (!(z_mean > 0.f)) return;                                    // `mask = selected_mean_std[:,0,0] > 0` (:242)
-    float alpha_score = sigmoidf_ref(__ldg(cp + ncls));
+    float alpha_score = sigmoid_ref(__ldg(cp + ncls));
 
     float4 a = ldg4(anchors + 4 * (long long)n);
     const float* d = reg + idx * 12;
@@ -102,17 +93,14 @@ __global__ void decode_candidates_kernel(const float* __restrict__ cls, const fl
 
     int slot = atomicAdd(ws.ncand + b, 1);
     if (slot >= cap) return;                       // overflow: flagged through ncand > cap
-    unsigned int sb = __float_as_uint(best);       // best in (0.75, 1] -> positive float, bit pattern monotone
-    ws.keys[(long long)b * cap + slot] = ((unsigned long long)(~sb) << 32) | (unsigned int)n;   // ascending key = score desc, index asc
+    ws.keys[(long long)b * cap + slot] = score_key(best, (unsigned int)n);     // best > score_thr > 0
     float* bp = ws.boxes + ((long long)b * cap + slot) * 11;
     bp[0] = x1; bp[1] = y1; bp[2] = x2; bp[3] = y2; bp[4] = cx1; bp[5] = cy1; bp[6] = z; bp[7] = w3; bp[8] = h3; bp[9] = l3; bp[10] = alpha;
     ws.labels[(long long)b * cap + slot] = label;
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// stage 2 (one CTA per image): bitonic sort of (key, slot) in shared memory, greedy NMS by 64-row bit-matrix blocks, ordered write-out.
-// torchvision CPU nms: areas = (x2-x1)*(y2-y1); inter = max(0, xx2-xx1)*max(0, yy2-yy1);
-//                      ovr = inter / (area_i + area_j - inter); suppress j if ovr > thr.
+// stage 2 (one CTA per image): bitonic sort of (key, slot) in shared memory, greedy NMS (nms_sweep), ordered write-out.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int NMS_THREADS = 1024;
 
@@ -127,98 +115,33 @@ __global__ void __launch_bounds__(NMS_THREADS) sort_nms_kernel(DecodeWs ws, int 
     int* sslot = reinterpret_cast<int*>(sbox + cap_pow2);                                // [cap_pow2]
     float* sarea = reinterpret_cast<float*>(sslot + cap_pow2);                           // [cap_pow2]
     int* skeep = reinterpret_cast<int*>(sarea + cap_pow2);                               // [cap_pow2] sorted positions of the kept boxes
-    __shared__ int s_nkeep;
     const int b = blockIdx.x, t = threadIdx.x;
     const int n = ws.ncand[b];
     if (t == 0) out_ncand[b] = n;
     if (n > cap) { if (t == 0) out_count[b] = -1; return; }
-    int np2 = 64;                                   // sort size: next power of two >= n (the padding keys ~0 sort to the end)
-    while (np2 < n) np2 <<= 1;
+    const int np2 = next_pow2(n, 64);               // sort size (the padding keys ~0 sort to the end)
 
     for (int i = t; i < np2; i += NMS_THREADS) {
         skey[i] = (i < n) ? ws.keys[(long long)b * cap + i] : ~0ull;
         sslot[i] = i;
     }
     __syncthreads();
-    // bitonic sort ascending on key
-    for (int k = 2; k <= np2; k <<= 1) {
-        for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = t; i < np2; i += NMS_THREADS) {
-                int ixj = i ^ j;
-                if (ixj > i) {
-                    bool up = ((i & k) == 0);
-                    unsigned long long a = skey[i], c = skey[ixj];
-                    if ((a > c) == up) {
-                        skey[i] = c; skey[ixj] = a;
-                        int s0 = sslot[i]; sslot[i] = sslot[ixj]; sslot[ixj] = s0;
-                    }
-                }
-            }
-            __syncthreads();
-        }
-    }
+    block_sort<NMS_THREADS, true>(skey, sslot, np2);
     for (int i = t; i < n; i += NMS_THREADS) {
         const float* bp = ws.boxes + ((long long)b * cap + sslot[i]) * 11;
         float4 bx = make_float4(bp[0], bp[1], bp[2], bp[3]);
         sbox[i] = bx;
-        sarea[i] = mul(sub(bx.z, bx.x), sub(bx.w, bx.y));
+        sarea[i] = box_area(bx);
     }
     __syncthreads();
-    // Greedy sweep (box i is kept iff no earlier KEPT box suppresses it), 64 rows at a time: all threads build the suppression bit
-    // matrix of the block (bit j of word w of row r: box 64w + j comes after row box i and IoU(i, 64w + j) > thr), then warp 0 walks
-    // the 64 rows in order with the removed-set held as one 64-bit word per lane.
-    const int nw = (n + 63) >> 6;                   // <= 32 words (cap <= 2048) ... or 64 for cap 4096: two words per lane
-    const int wpr = cap_pow2 >> 6;                  // words per mask row
-    unsigned long long removed0 = 0, removed1 = 0;  // warp 0: lane l holds words l and l + 32
-    int nkeep = 0;
-    const int warp = t >> 5, lane = t & 31;
-    for (int c = 0; c < nw; ++c) {
-        const int words = nw - c;
-        for (int e = t; e < 64 * words; e += NMS_THREADS) {
-            const int r = e & 63, w = c + (e >> 6);
-            const int i = c * 64 + r;
-            unsigned long long bits = 0;
-            if (i < n) {
-                const float4 bi = sbox[i];
-                const float ai = sarea[i];
-                const int j0 = w * 64;
-                const int jend = min(64, n - j0);
-                for (int j = (w == c ? r + 1 : 0); j < jend; ++j) {
-                    const float4 bj = sbox[j0 + j];
-                    float xx1 = fmaxf(bi.x, bj.x), yy1 = fmaxf(bi.y, bj.y);
-                    float xx2 = fminf(bi.z, bj.z), yy2 = fminf(bi.w, bj.w);
-                    float ww = fmaxf(0.f, sub(xx2, xx1)), hh = fmaxf(0.f, sub(yy2, yy1));
-                    float inter = mul(ww, hh);
-                    float ovr = __fdiv_rn(inter, sub(add(ai, sarea[j0 + j]), inter));
-                    if ((double)ovr > iou_thr) bits |= 1ull << j;    // torchvision compares the f32 IoU with a double threshold
-                }
-            }
-            smask[r * wpr + w] = bits;
-        }
-        __syncthreads();
-        if (warp == 0) {
-            const int rows = min(64, n - c * 64);
-            for (int r = 0; r < rows; ++r) {
-                const unsigned long long rc = c < 32 ? __shfl_sync(0xffffffffu, removed0, c) : __shfl_sync(0xffffffffu, removed1, c - 32);
-                if ((rc >> r) & 1ull) continue;                       // warp-uniform
-                if (lane == 0) skeep[nkeep] = c * 64 + r;
-                ++nkeep;
-                if (lane >= c && lane < nw) removed0 |= smask[r * wpr + lane];
-                if (lane + 32 >= c && lane + 32 < nw) removed1 |= smask[r * wpr + lane + 32];
-            }
-        }
-        __syncthreads();
-    }
-    if (t == 0) s_nkeep = nkeep;
-    __syncthreads();
-    nkeep = s_nkeep;
+    const int nkeep = nms_sweep<NMS_THREADS>(sbox, sarea, n, cap_pow2 >> 6, iou_thr, smask, skeep);
     // ordered write-out of the kept boxes, all threads
     for (int k = t; k < nkeep; k += NMS_THREADS) {
         const int i = skeep[k];
         const int slot = sslot[i];
         const unsigned long long key = skey[i];
-        out_scores[(long long)b * cap + k] = __uint_as_float(~(unsigned int)(key >> 32));
-        out_anchor[(long long)b * cap + k] = (int)(unsigned int)(key & 0xffffffffu);
+        out_scores[(long long)b * cap + k] = key_score(key);
+        out_anchor[(long long)b * cap + k] = (int)key_index(key);
         out_cls[(long long)b * cap + k] = (int64_t)ws.labels[(long long)b * cap + slot];
         const float* bp = ws.boxes + ((long long)b * cap + slot) * 11;
         float* op = out_boxes + ((long long)b * cap + k) * 11;
@@ -267,10 +190,10 @@ __global__ void retina_score_kernel(RetinaLevels lv, int B, int N, int ncls, uns
     const float* cp = lv.cls[l] + e;
     float best = -1.f; int label = 0;
     for (int c = 0; c < ncls; ++c) {
-        const float p = sigmoidf_ref(__ldg(cp + c));
+        const float p = sigmoid_ref(__ldg(cp + c));
         if (p > best) { best = p; label = c; }
     }
-    keys[idx] = ~__float_as_uint(best);                 // sigmoid >= +0: the bit pattern is monotone
+    keys[idx] = (unsigned int)(score_key(best, 0u) >> 32);     // the score half of the sort key (sigmoid >= +0)
     labels[idx] = (uint8_t)label;
 }
 
@@ -361,7 +284,7 @@ __global__ void __launch_bounds__(SEL_THREADS) retina_select_kernel(RetinaLevels
         const float gw = mul(pw, expf(dw)), gh = mul(ph, expf(dh));
         const float gx = add(px, mul(pw, dx)), gy = add(py, mul(ph, dy));
         const long long o = (long long)b * cap + pos;
-        ws.keys[o] = ((unsigned long long)key << 32) | (unsigned int)n;
+        ws.keys[o] = score_key(key_score((unsigned long long)key << 32), (unsigned int)n);
         float* bp = ws.boxes + o * 11;
         bp[0] = sub(gx, mul(gw, 0.5f)); bp[1] = sub(gy, mul(gh, 0.5f)); bp[2] = add(gx, mul(gw, 0.5f)); bp[3] = add(gy, mul(gh, 0.5f));
 #pragma unroll
@@ -415,8 +338,6 @@ extern "C" int vd3d_pack_records(const float* scores, const float* boxes, const 
     return VD3D_OK;
 }
 
-static int next_pow2(int v) { int p = 1; while (p < v) p <<= 1; return p; }
-
 extern "C" int vd3d_anchor_mask(const float* anchors, const float* means_z, const float* P2, int B, int N, int T,
                                 float y_min, float y_max, float x_thr, uint8_t* mask, void* stream) {
     VD3D_REQUIRE(anchors && means_z && P2 && mask && B > 0 && N > 0 && T > 0, "anchor_mask: bad args");
@@ -431,6 +352,26 @@ extern "C" long long vd3d_decode_nms_workspace(int B, int cap) {
     return (long long)B * per + 16 * ((B * 4 + 15) / 16) + 64;
 }
 
+static DecodeWs decode_ws(void* wsp, int B, int cap) {
+    DecodeWs ws;
+    unsigned char* p = (unsigned char*)wsp;
+    ws.keys = (unsigned long long*)p; p += (long long)B * cap * 8;
+    ws.boxes = (float*)p; p += (long long)B * cap * 44;
+    ws.labels = (int*)p; p += (long long)B * cap * 4;
+    ws.ncand = (int*)p;
+    return ws;
+}
+
+static int launch_sort_nms(const DecodeWs& ws, int B, int cap, double iou_thr, float* out_scores, float* out_boxes, int64_t* out_cls,
+                           int32_t* out_anchor, int32_t* out_count, int32_t* out_ncand, cudaStream_t st) {
+    const int cp2 = next_pow2(cap, 64);          // the 64-row bit-matrix blocks of the NMS sweep
+    const size_t smem = (size_t)cp2 * (8 + 8 + 16 + 4 + 4 + 4) + 16;
+    VD3D_CUDA(cudaFuncSetAttribute(sort_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    sort_nms_kernel<<<B, NMS_THREADS, smem, st>>>(ws, cap, cp2, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand);
+    VD3D_CHECK_LAUNCH("sort_nms");
+    return VD3D_OK;
+}
+
 extern "C" int vd3d_decode_nms(const float* cls, const float* reg, const float* anchors, const float* mean_std,
                                const uint8_t* mask, int B, int N, int ncls, int T, float score_thr, double iou_thr,
                                float img_w, float img_h, int cap, void* wsp,
@@ -441,23 +382,12 @@ extern "C" int vd3d_decode_nms(const float* cls, const float* reg, const float* 
     VD3D_REQUIRE(B > 0 && N > 0 && ncls > 0 && ncls <= T && cap > 0 && cap <= 4096, "decode_nms: bad shape (cap must be <= 4096)");
     VD3D_REQUIRE(score_thr > 0.f, "decode_nms: score_thr must be positive (sort key relies on positive scores)");
     cudaStream_t st = (cudaStream_t)stream;
-    DecodeWs ws;
-    unsigned char* p = (unsigned char*)wsp;
-    ws.keys = (unsigned long long*)p; p += (long long)B * cap * 8;
-    ws.boxes = (float*)p; p += (long long)B * cap * 44;
-    ws.labels = (int*)p; p += (long long)B * cap * 4;
-    ws.ncand = (int*)p;
+    const DecodeWs ws = decode_ws(wsp, B, cap);
     VD3D_CUDA(cudaMemsetAsync(ws.ncand, 0, sizeof(int) * B, st));
     decode_candidates_kernel<<<cdiv((long long)B * N, 256), 256, 0, st>>>(cls, reg, anchors, mean_std, mask, B, N, ncls, T,
                                                                          score_thr, img_w, img_h, cap, ws);
     VD3D_CHECK_LAUNCH("decode_candidates");
-    int cp2 = next_pow2(cap);
-    if (cp2 < 64) cp2 = 64;                      // the 64-row bit-matrix blocks of the NMS sweep
-    size_t smem = (size_t)cp2 * (8 + 8 + 16 + 4 + 4 + 4) + 16;
-    VD3D_CUDA(cudaFuncSetAttribute(sort_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sort_nms_kernel<<<B, NMS_THREADS, smem, st>>>(ws, cap, cp2, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand);
-    VD3D_CHECK_LAUNCH("sort_nms");
-    return VD3D_OK;
+    return launch_sort_nms(ws, B, cap, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand, st);
 }
 
 extern "C" long long vd3d_retina_decode_workspace(int B, int N, int cap) {
@@ -488,12 +418,7 @@ extern "C" int vd3d_retina_decode(int L, const void* const* cls_levels, const vo
     }
     VD3D_REQUIRE(lv.off[L] == N, "retina_decode: the levels hold %d anchors, N = %d", lv.off[L], N);
     cudaStream_t st = (cudaStream_t)stream;
-    DecodeWs ws;
-    unsigned char* p = (unsigned char*)wsp;
-    ws.keys = (unsigned long long*)p; p += (long long)B * cap * 8;
-    ws.boxes = (float*)p; p += (long long)B * cap * 44;
-    ws.labels = (int*)p; p += (long long)B * cap * 4;
-    ws.ncand = (int*)p;
+    const DecodeWs ws = decode_ws(wsp, B, cap);
     unsigned char* q = (unsigned char*)wsp + vd3d_decode_nms_workspace(B, cap);
     unsigned int* keys = (unsigned int*)q;
     uint8_t* labels = q + ((long long)B * N * 4 + 15) / 16 * 16;
@@ -502,12 +427,8 @@ extern "C" int vd3d_retina_decode(int L, const void* const* cls_levels, const vo
     retina_select_kernel<<<B, SEL_THREADS, 0, st>>>(lv, keys, labels, anchors, N, k, make_float4(means4[0], means4[1], means4[2], means4[3]),
                                                     make_float4(stds4[0], stds4[1], stds4[2], stds4[3]), cap, ws);
     VD3D_CHECK_LAUNCH("retina_select");
-    int cp2 = next_pow2(cap);
-    if (cp2 < 64) cp2 = 64;
-    const size_t smem = (size_t)cp2 * (8 + 8 + 16 + 4 + 4 + 4) + 16;
-    VD3D_CUDA(cudaFuncSetAttribute(sort_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sort_nms_kernel<<<B, NMS_THREADS, smem, st>>>(ws, cap, cp2, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand);
-    VD3D_CHECK_LAUNCH("sort_nms");
+    const int e = launch_sort_nms(ws, B, cap, iou_thr, out_scores, out_boxes, out_cls, out_anchor, out_count, out_ncand, st);
+    if (e != VD3D_OK) return e;
     retina_thresh_kernel<<<B, 256, 0, st>>>(out_scores, cap, score_thr, out_count);
     VD3D_CHECK_LAUNCH("retina_thresh");
     return VD3D_OK;
