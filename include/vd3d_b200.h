@@ -127,7 +127,7 @@ int vd3d_conv2d_tc16_stem(const void* in_hi, const void* in_lo, int B, int H, in
 int vd3d_conv2d_tc16_stem_pool(const void* in_hi, const void* in_lo, int B, int H, int W, int Wp, int KH, int KW, int stride, int pad, int win,
                                const void* w_hi, const void* w_lo, float out_scale, const float* bias,
                                float* pool_out, int Cout, int pool_cs, int pool_co, void* stream);
-/* The ResNet stem as one persistent kernel (csrc/stem_pool.cu): conv 7x7 / stride 2 / pad 3 (<= 4 -> 64 channels) + folded BN + ReLU +
+/* The ResNet stem as one persistent row-strip kernel (stem_pool_kernel, csrc/row_conv.cu): conv 7x7 / stride 2 / pad 3 (<= 4 -> 64 channels) + folded BN + ReLU +
  * MaxPool2d(3, 2, 1) (R/networks/backbones/resnet.py:120-122,186-189).  Replaces vd3d_conv2d_tc16_stem_pool: no window re-reads (the wgmma
  * descriptor walks the overlapping 8-pixel windows inside one staged image row), no atomics, pooled tensor written as fp32 (`out`, may be
  * NULL) and / or fp16 (hi, lo) planes (may be NULL) NHWC [B][Hq][Wq][out_cs], channels [out_co, out_co + 64).

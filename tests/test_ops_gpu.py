@@ -506,7 +506,7 @@ def test_stem_with_fused_maxpool_is_bit_identical(shape):
 @pytest.mark.parametrize("shape", [(2, 3, 64, 96), (3, 3, 70, 154), (1, 3, 34, 30), (2, 3, 96, 320), (16, 3, 96, 160), (2, 3, 384, 1280), (1, 3, 75, 515), (5, 3, 21, 1010)])
 @pytest.mark.parametrize("f32_out", [True, False])
 def test_stem_row_strip_kernel_is_bit_identical(shape, f32_out):
-    """csrc/stem_pool.cu (conv1 + BN + ReLU + MaxPool2d(3, 2, 1) as one row-strip kernel: overlapping windows through a no-swizzle wgmma
+    """stem_pool_kernel in csrc/row_conv.cu (conv1 + BN + ReLU + MaxPool2d(3, 2, 1) as one row-strip kernel: overlapping windows through a no-swizzle wgmma
     descriptor, max-pool in registers, pooled tensor as fp16 planes [+ fp32]) against the stem kernel followed by the max-pool kernel: bit for
     bit, for one and several strips / row segments, odd conv and pooled sizes, image rows above / below the image, a channel slice, repeated calls."""
     E = _E()
@@ -548,6 +548,8 @@ ROW_CONV_CASES = [
     (2, 16, 16, 33, 141, 32, 3, 2, 1),      # level1: stride 2, every fourth operand row
     (3, 16, 16, 96, 320, 32, 3, 2, 1),
     (1, 3, 8, 384, 1280, 16, 7, 1, 3),      # full size: 10 strips, several row segments
+    (2, 3, 4, 40, 150, 16, 7, 2, 3),        # the ResNet stem's conv geometry: 4-channel planes, 7x7 / 2, two K steps per filter row
+    (2, 3, 4, 40, 150, 32, 7, 2, 3),
 ]
 
 

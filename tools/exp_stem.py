@@ -1,4 +1,4 @@
-"""Knock-out timing of the row-strip stem + pool kernel (csrc/stem_pool.cu) at the BASELINE shape (16 images 384x1280):
+"""Knock-out timing of the row-strip stem + pool kernel (stem_pool_kernel in csrc/row_conv.cu) at the BASELINE shape (16 images 384x1280):
 VD3D_TC_DEBUG bit 0 = one MMA per K step, bit 4 = no output stores.  python tools/exp_stem.py"""
 import os
 import sys

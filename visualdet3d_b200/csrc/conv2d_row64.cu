@@ -218,18 +218,6 @@ conv2d_row64_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_const
     }
 }
 
-template <int BN>
-static cudaError_t r64_launch_kernel(const cudaLaunchConfig_t& cfg, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi,
-                                     const CUtensorMap& mWlo, const TcParams& p, const R64Geo& q) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(conv2d_row64_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    return cudaLaunchKernelEx(&cfg, conv2d_row64_kernel<BN>, mA, mAlo, mWhi, mWlo, p, q);
-}
-
 // The conv of `p` (set up by conv2d_tc_launch, eligible per conv2d_row64_eligible) on the row-strip kernel.  Input planes: NHWC fp16 with
 // pixel pitch in_cs, channel offset in_co.
 int conv2d_row64_launch(TcParams& p, const void* in_hi, const void* in_lo, int in_cs, int in_co, const void* w_hi, const void* w_lo, void* stream) {
@@ -268,22 +256,12 @@ int conv2d_row64_launch(TcParams& p, const void* in_hi, const void* in_lo, int i
     const size_t smem = fixed + q.wstages * wstage;
     int grid = q.ntiles < kNumSMs ? (int)q.ntiles : kNumSMs;
     { const char* e = getenv("VD3D_TC_GRID"); const int cap = e ? atoi(e) : 0; if (cap > 0 && cap < grid) grid = cap; }     // diagnostics
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(R64_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
     cudaError_t le = cudaErrorInvalidValue;
     switch (BN) {
-        case 16: le = r64_launch_kernel<16>(cfg, mA, mAlo, mWhi, mWlo, p, q); break;
-        case 32: le = r64_launch_kernel<32>(cfg, mA, mAlo, mWhi, mWlo, p, q); break;
-        case 48: le = r64_launch_kernel<48>(cfg, mA, mAlo, mWhi, mWlo, p, q); break;
-        case 64: le = r64_launch_kernel<64>(cfg, mA, mAlo, mWhi, mWlo, p, q); break;
+        case 16: le = tc_launch<conv2d_row64_kernel<16>>(grid, R64_THREADS, smem, stream, mA, mAlo, mWhi, mWlo, p, q); break;
+        case 32: le = tc_launch<conv2d_row64_kernel<32>>(grid, R64_THREADS, smem, stream, mA, mAlo, mWhi, mWlo, p, q); break;
+        case 48: le = tc_launch<conv2d_row64_kernel<48>>(grid, R64_THREADS, smem, stream, mA, mAlo, mWhi, mWlo, p, q); break;
+        case 64: le = tc_launch<conv2d_row64_kernel<64>>(grid, R64_THREADS, smem, stream, mA, mAlo, mWhi, mWlo, p, q); break;
     }
     if (le != cudaSuccess) { set_error("conv2d_row64: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
     VD3D_CHECK_LAUNCH("conv2d_row64");

@@ -500,18 +500,6 @@ static long long* g_trace = nullptr;
 static int g_trace_n = 0;
 extern "C" void vd3d_tc_set_trace(void* dev_i64, int n) { g_trace = (long long*)dev_i64; g_trace_n = n; }
 
-template <int BN, bool F16, bool LV>
-static cudaError_t tcp_launch_kernel(const cudaLaunchConfig_t& cfg, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi,
-                                     const CUtensorMap& mWlo, const TcParams& p, const std::conditional_t<LV, TcLevelMaps, TcNoLevelMaps>& lm) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(conv2d_tcp_kernel<BN, F16, LV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    return cudaLaunchKernelEx(&cfg, conv2d_tcp_kernel<BN, F16, LV>, mA, mAlo, mWhi, mWlo, p, lm);
-}
-
 // launch of the persistent kernel: p.BN (<= TC_MAX_BN) / p.chunk / tile counts are set by the caller, the weight maps have BN rows per box;
 // `lm`: the per-level activation maps of a multi-level launch (p.n_levels > 0, fp16 operands only)
 static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAlo, const CUtensorMap& mWhi, const CUtensorMap& mWlo, void* stream,
@@ -549,26 +537,17 @@ static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAl
     const int units = p.m_tiles * p.n_tiles;
     int grid = units < kNumSMs ? units : kNumSMs;
     { const char* e = getenv("VD3D_TC_GRID"); const int cap = e ? atoi(e) : 0; if (cap > 0 && cap < grid) grid = cap; }     // diagnostics
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(TCP_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
     cudaError_t le = cudaErrorInvalidValue;
     VD3D_REQUIRE(!lm || (p.f16 && p.n_levels > 0), "conv2d_tc: multi-level launches take fp16 operands");
     const TcNoLevelMaps nolm{0};
-#define VD3D_TCP_CASE(N) case N: le = lm ? tcp_launch_kernel<N, true, true>(cfg, mA, mAlo, mWhi, mWlo, p, *lm) : p.f16 ? \
-        tcp_launch_kernel<N, true, false>(cfg, mA, mAlo, mWhi, mWlo, p, nolm) : tcp_launch_kernel<N, false, false>(cfg, mA, mAlo, mWhi, mWlo, p, nolm); break
+#define VD3D_TCP_LAUNCH(N, F16, LV, LM) tc_launch<conv2d_tcp_kernel<N, F16, LV>>(grid, TCP_THREADS, smem, stream, mA, mAlo, mWhi, mWlo, p, LM)
+#define VD3D_TCP_CASE(N) case N: le = lm ? VD3D_TCP_LAUNCH(N, true, true, *lm) : p.f16 ? VD3D_TCP_LAUNCH(N, true, false, nolm) : VD3D_TCP_LAUNCH(N, false, false, nolm); break
     switch (BN) {
         VD3D_TCP_CASE(16); VD3D_TCP_CASE(32); VD3D_TCP_CASE(48); VD3D_TCP_CASE(64);
         VD3D_TCP_CASE(80); VD3D_TCP_CASE(96); VD3D_TCP_CASE(112); VD3D_TCP_CASE(128);
     }
 #undef VD3D_TCP_CASE
+#undef VD3D_TCP_LAUNCH
     if (le != cudaSuccess) { set_error("conv2d_tcp: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
     VD3D_CHECK_LAUNCH("conv2d_tcp");
     return VD3D_OK;
@@ -800,42 +779,11 @@ extern "C" int vd3d_conv2d_tc16_res_up2(const void* in_hi, const void* in_lo, in
 // ----------------------------------------------------------------------------------------------------------------
 // Few-channel KHxKW convolution (the 7x7 stride-2 stem) on the tensor cores, without im2col:
 // the image is kept as fp16 (hi, lo) planes [B][H][Wp][4] (<= 4 channels per pixel, `xoff` zero pixels on the left, zeros
-// on the right).  The KW*4 <= 64 values a filter row needs for output column wo are CONTIGUOUS in that layout, starting at
-// pixel wo*stride (= wo*stride - pad + xoff with xoff == pad).  A tensor map with the overlapping W' stride of `stride`
+// on the right; written by vd3d_image_to_h16_rows in row_conv.cu).  The KW*4 <= 64 values a filter row needs for output
+// column wo are CONTIGUOUS in that layout, starting at pixel wo*stride (= wo*stride - pad + xoff with xoff == pad).  A tensor map with the overlapping W' stride of `stride`
 // pixels therefore presents the image as a virtual NHWC tensor [B][H][Wo][64] and the conv becomes a KHx1 convolution with
 // 64 "channels" (kw*4 + c; weights zero beyond KW*4) and stride (stride, 1): exactly what conv2d_tcp_kernel runs.
 // ----------------------------------------------------------------------------------------------------------------
-__global__ void image_to_h16_rows_kernel(const float* __restrict__ in, __half* __restrict__ hi, __half* __restrict__ lo, int C, int H, int W,
-                                         long long total, int Wp, int xoff, int* __restrict__ range_flag) {
-    long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= total) return;
-    const long long HW = (long long)H * W;
-    const long long b = idx / HW, pq = idx - b * HW;
-    const int y = (int)(pq / W), x = (int)(pq - (long long)y * W);
-    const float* ip = in + b * C * HW + pq;
-    float v[4] = {0.f, 0.f, 0.f, 0.f};
-    for (int c = 0; c < C; ++c) v[c] = __ldg(ip + (long long)c * HW);
-    note_fp16_range(fmaxf(fmaxf(fabsf(v[0]), fabsf(v[1])), fmaxf(fabsf(v[2]), fabsf(v[3]))), range_flag);
-    __half h[4], l[4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) { h[c] = __float2half_rn(v[c]); l[c] = __float2half_rn(v[c] - __half2float(h[c])); }
-    const long long o = ((b * H + y) * Wp + x + xoff) * 4;
-    __half2 h01 = __halves2half2(h[0], h[1]), h23 = __halves2half2(h[2], h[3]), l01 = __halves2half2(l[0], l[1]), l23 = __halves2half2(l[2], l[3]);
-    uint2 hv, lv;
-    hv.x = *reinterpret_cast<uint32_t*>(&h01); hv.y = *reinterpret_cast<uint32_t*>(&h23);
-    lv.x = *reinterpret_cast<uint32_t*>(&l01); lv.y = *reinterpret_cast<uint32_t*>(&l23);
-    *reinterpret_cast<uint2*>(hi + o) = hv;
-    *reinterpret_cast<uint2*>(lo + o) = lv;
-}
-
-extern "C" int vd3d_image_to_h16_rows(const float* img, int B, int C, int H, int W, void* hi16, void* lo16, int Wp, int xoff, void* stream) {
-    VD3D_REQUIRE(img && hi16 && lo16 && B > 0 && C >= 1 && C <= 4 && H > 0 && W > 0 && xoff >= 0 && Wp >= W + xoff, "image_to_h16_rows: bad args");
-    const long long total = (long long)B * H * W;
-    image_to_h16_rows_kernel<<<cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(img, (__half*)hi16, (__half*)lo16, C, H, W, total, Wp, xoff, fp16_range_flag());
-    VD3D_CHECK_LAUNCH("image_to_h16_rows");
-    return VD3D_OK;
-}
-
 extern "C" int vd3d_stem_row_pitch(int W, int KW, int stride, int pad) {
     // pixels per padded row: left pad `pad`, the image, and enough zeros for the 16-pixel window of the last output column; even
     const int Wo = (W + 2 * pad - KW) / stride + 1;

@@ -63,6 +63,11 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, u
         "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
+// 1-D bulk copy of `bytes` (a multiple of 16, both addresses 16-byte aligned) from global to shared memory, completing on `bar`
+__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes),
+                 "r"(smem_u32(bar)) : "memory");
+}
 // one elected lane of a fully converged warp (the compiler knows exactly one thread runs the guarded code)
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;

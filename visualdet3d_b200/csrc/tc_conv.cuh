@@ -347,6 +347,26 @@ inline bool pdl_enabled() {
     return v == 1;
 }
 
+// Launch of a tensor-core kernel: `threads` per CTA, `smem` bytes of dynamic shared memory (the first launch of each kernel raises its limit to
+// 227 KB), as a programmatic dependent of its predecessor when pdl_enabled().
+template <auto Kernel, class... Args>
+inline cudaError_t tc_launch(int grid, int threads, size_t smem, void* stream, const Args&... args) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        if (e != cudaSuccess) return e;
+        attr_set = true;
+    }
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)threads); cfg.dynamicSmemBytes = smem; cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, Kernel, args...);
+}
+
 inline int make_map_wgt(CUtensorMap* m, const void* base, int Cout, int K, int BN, int esize = 4, int rowb = 128) {
     EncodeTiledFn enc = get_encode();
     if (!enc) { set_error("conv2d_tc: cuTensorMapEncodeTiled unavailable"); return VD3D_ECUDA; }

@@ -387,7 +387,7 @@ class StemLayer:
         return (H + 2 * self.pad - self.KH) // self.stride + 1, (W + 2 * self.pad - self.KW) // self.stride + 1
 
     def row_kernel_ok(self) -> bool:
-        """the row-strip stem + pool kernel (csrc/stem_pool.cu) covers this layer: 7x7 / 2 / 3, 64 outputs, ReLU, 32-element windows (VD3D_STEM_ROWS=0: off)"""
+        """the row-strip stem + pool kernel (stem_pool_kernel, csrc/row_conv.cu) covers this layer: 7x7 / 2 / 3, 64 outputs, ReLU, 32-element windows (VD3D_STEM_ROWS=0: off)"""
         import os
         return (self.KH, self.KW, self.stride, self.pad, self.Cout, self.win) == (7, 7, 2, 3, 64, 32) and self.relu and \
             os.environ.get("VD3D_STEM_ROWS", "1") != "0"
@@ -406,7 +406,7 @@ class StemLayer:
         import os
         pool = pool and os.environ.get("VD3D_STEM_POOL", "1") != "0"
         if pool and self.row_kernel_ok() and out.h16:
-            # conv + BN + ReLU + MaxPool2d(3, 2, 1) as the row-strip kernel (csrc/stem_pool.cu): `out` is the POOLED tensor, written as fp16 planes
+            # conv + BN + ReLU + MaxPool2d(3, 2, 1) as the row-strip kernel (stem_pool_kernel, csrc/row_conv.cu): `out` is the POOLED tensor, written as fp16 planes
             # (the layer-1 convs and their plane residual read nothing else) and as fp32 only when `f32_out` asks for it
             Hs, Ws = self.out_hw(H, W)
             assert (out.H, out.W) == ((Hs - 1) // 2 + 1, (Ws - 1) // 2 + 1) and out.h16, "fused stem: pooled shape, fp16 planes"
