@@ -455,16 +455,18 @@ deform_conv_fused_staged_kernel(const __grid_constant__ CUtensorMap mapX, const 
 
 using namespace vd3d;
 
-// sets the shared-memory limit of a kernel instance once, then launches it
-template <typename K, typename... Args>
-static cudaError_t df_launch(K kernel, int grid, size_t smem, void* stream, Args... args) {
-    static bool attr_set = false;      // one flag per kernel instance (K differs per instance)
+// sets the shared-memory limit of a kernel instance once, then launches it.  The kernel is a template argument, so each BN instance has
+// its own flag: keyed on the kernel's type, the four instances (same signature) would share one, and only the first one launched would get
+// the 227 KB limit.
+template <auto Kernel, typename... Args>
+static cudaError_t df_launch(int grid, size_t smem, void* stream, Args... args) {
+    static bool attr_set = false;
     if (!attr_set) {
-        const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    kernel<<<grid, DF_THREADS, smem, (cudaStream_t)stream>>>(args...);
+    Kernel<<<grid, DF_THREADS, smem, (cudaStream_t)stream>>>(args...);
     return cudaGetLastError();
 }
 
@@ -534,7 +536,7 @@ extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C
         q.stages = ws;
         const size_t smem = fixed + (size_t)ws * 2 * BN * 128;
         cudaError_t le = cudaErrorInvalidValue;
-#define VD3D_DFS_CASE(N) case N: le = df_launch(deform_conv_fused_staged_kernel<N>, grid, smem, stream, mX, mWhi, mWlo, p, q); break
+#define VD3D_DFS_CASE(N) case N: le = df_launch<deform_conv_fused_staged_kernel<N>>(grid, smem, stream, mX, mWhi, mWlo, p, q); break
         switch (BN) { VD3D_DFS_CASE(16); VD3D_DFS_CASE(32); VD3D_DFS_CASE(48); VD3D_DFS_CASE(64); }
 #undef VD3D_DFS_CASE
         if (le != cudaSuccess) { set_error("deform_conv_fused_staged: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
@@ -549,7 +551,7 @@ extern "C" int vd3d_deform_conv_fused(const float* x, int B, int H, int W, int C
     q.stages = stages;
     const size_t smem = (size_t)stages * q.stage_bytes + fixed;
     cudaError_t le = cudaErrorInvalidValue;
-#define VD3D_DF_CASE(N) case N: le = df_launch(deform_conv_fused_kernel<N>, grid, smem, stream, mWhi, mWlo, p, q); break
+#define VD3D_DF_CASE(N) case N: le = df_launch<deform_conv_fused_kernel<N>>(grid, smem, stream, mWhi, mWlo, p, q); break
     switch (BN) { VD3D_DF_CASE(16); VD3D_DF_CASE(32); VD3D_DF_CASE(48); VD3D_DF_CASE(64); }
 #undef VD3D_DF_CASE
     if (le != cudaSuccess) { set_error("deform_conv_fused: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
