@@ -10,8 +10,8 @@
 // * No im2col: for k-block (tap, channel chunk) the A operand is ONE 4-D TMA box [chunk][16 w][8 h][1 b] of the input shifted by the tap
 //   offset; conv zero padding is TMA out-of-bounds fill.  Swizzled K-major operands (128-byte rows; 64-byte rows for the 32-element stem window).
 // * Persistent: one CTA per SM strides over the 128-pixel x BN-channel output tiles (unit_tile: M fastest inside L2-sized M blocks).
-//   Warp 8 = TMA producer (one lane) feeding a multi-stage mbarrier ring; warps 0..7 = two consumer warpgroups; warps 9..11 = epilogue
-//   (tiles wider than 64 columns; narrower tiles run it on the consumers, tcp_store_tile / tcp_pool_tile).
+//   Warp 8 = TMA producer (one lane) feeding a multi-stage mbarrier ring; warps 0..7 = two consumer warpgroups; warps 9..15 = epilogue
+//   (tiles wider than 64 columns, 512 threads; narrower tiles run it on the consumers, tcp_store_tile / tcp_pool_tile, 384 threads).
 //   Warpgroup w issues the wgmma of tile rows 64 w .. 64 w + 63 as soon as a stage has landed, keeps one k-block in flight, frees a stage when
 //   its MMAs are done, promotes every chunk (wg_promote) and at the end of the tile stages its accumulator in shared memory and hands it to the
 //   epilogue warps (tcp_epi_tile), then goes straight on with the next tile's MMAs while the epilogue runs.
@@ -116,30 +116,34 @@ __global__ void pool_border_zero_kernel(float* __restrict__ out, int B, int Hp, 
 // share a slot, so the later one was loaded only after the consumers (or the epilogue, after the consumers staged the tile) released the
 // earlier one, and they had read its log entry by then.  Every slot keeps its own phase bit on both sides.
 // ----------------------------------------------------------------------------------------------------------------
-// Warps 0..7 = consumers, warp 8 = TMA producer, warps 9..11 = epilogue.  ptxas budgets registers per whole warpgroup (65536 / 384 = 168 per
-// thread here; a fourth warpgroup would cap every thread at 128, below what the 128-column consumers need), so the epilogue gets the three
-// warps of the producer's warpgroup.
-constexpr int TCP_EPI = 96;
-constexpr int TCP_THREADS = TC_CONSUMERS + 32 + TCP_EPI;
 // row pitch (floats) of the staged accumulator: BN + 4 (conflict-free rows); at BN = 128 unpadded rows with the chunk swizzle of wg_stage,
 // so that the 64 KB tile fits in one 64 KB operand stage
 __host__ __device__ constexpr int tcp_tile_ld(int BN) { return BN == TC_MAX_BN ? BN : BN + 4; }
 // Tiles wider than 64 columns hand their epilogue to the epilogue warps.  Narrower tiles keep it on the consumers (the stem's fused
 // max-pool among them): their K loop is short (64 columns: 9 k-blocks of ~890 clocks for a 64-channel 3x3 conv, H100) and the three
-// epilogue warps take longer per tile (~11 k clocks) than the 256 consumer threads, so overlapping made those layers slower.
+// epilogue warps of the 384-thread kernel took longer per tile (~11 k clocks) than the 256 consumer threads, so overlapping made those
+// layers slower; on seven warps 64-column tiles measured no faster (DESIGN §4).
 __host__ __device__ constexpr bool tcp_epi_warps(int BN) { return BN > 64; }
+// Warps 0..7 = consumers, warp 8 = TMA producer, warps 9..15 = epilogue (tiles with epilogue warps: 512 threads; narrower tiles: 384, and
+// warps 9..11 leave at once).  ptxas budgets registers per warpgroup at launch: 65536 / 512 = 128 per thread, below the 145 .. 149 the
+// 128-column consumers need, so right after the barrier setup the consumer warpgroups raise their budget to TCP_REG_CONSUMER and the
+// producer / epilogue warpgroups lower theirs to TCP_REG_EPI (setmaxnreg; 2 x 128 x 160 + 2 x 128 x 96 = 65536).
+constexpr int TCP_EPI = 224;
+constexpr int TCP_REG_CONSUMER = 160, TCP_REG_EPI = 96;
+__host__ __device__ constexpr int tcp_threads(int BN) { return TC_CONSUMERS + 32 + (tcp_epi_warps(BN) ? TCP_EPI : 96); }
+static_assert(2 * 128 * TCP_REG_CONSUMER + 2 * 128 * TCP_REG_EPI == 65536, "setmaxnreg split must hand out exactly the register file");
 // named barrier of the epilogue warps
 __device__ __forceinline__ void epilogue_sync() { asm volatile("bar.sync 3, %0;" ::"n"(TCP_EPI) : "memory"); }
 
 // Epilogue of one staged tile by the epilogue warps (thread et of TCP_EPI).  Item = (pixel row r, 8-column group g), items numbered row-major,
 // thread et takes items et, et + TCP_EPI, ...: consecutive lanes cover consecutive column groups of one pixel, so a warp's residual loads and
 // output stores are whole runs of a pixel's channels (at BN = 128, 256 contiguous bytes per fp16 plane).  The residual loads of U items are
-// issued before the first of them is computed.  Per element the arithmetic is that of tcp_store_tile.  Covers tile rows r0 .. r1 - 1; row r
-// is read at tile + r * ld.
+// issued before the first of them is computed (U x TCP_EPI = 896 item loads in flight per SM).  Per element the arithmetic is that of
+// tcp_store_tile.  Covers tile rows r0 .. r1 - 1; row r is read at tile + r * ld.
 template <int BN>
 __device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* tile, int ld, int u, int mt_units, int et, int swz, int r0, int r1) {
     constexpr int CG = BN / 8;                                   // column groups per pixel
-    constexpr int U = 8;
+    constexpr int U = 4;
     const int ITEMS = r1 * CG;
     int mu, nt;
     unit_tile(p, u, mt_units, mu, nt);
@@ -179,7 +183,7 @@ struct TcLevelMaps { CUtensorMap a[TC_MAX_LEVELS], alo[TC_MAX_LEVELS]; };
 struct TcNoLevelMaps { int unused; };
 
 template <int BN, bool F16, bool LV>
-__global__ void __launch_bounds__(TCP_THREADS, 1)
+__global__ void __launch_bounds__(tcp_threads(BN), 1)
 conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAlo,
                   const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p,
                   const __grid_constant__ std::conditional_t<LV, TcLevelMaps, TcNoLevelMaps> lmaps) {
@@ -226,106 +230,111 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     pdl_launch_dependents();
     pdl_wait();                            // (PDL launches only) the producer of the activations / residual has completed
 
-    if (warp > TC_CONSUMERS / 32) {
-        // ================= epilogue warps: tile i of this CTA is handed over through acc_full / acc_empty phase i =================
-        if (!epi_warps) return;
-        const int et = (int)threadIdx.x - (TC_CONSUMERS + 32);
-        const bool tr0 = p.trace && blockIdx.x == 0 && et == 0;
-        float amax = 0.f;
-        int i = 0;
-        for (int u = u0; u < units; u += ustep, ++i) {
-            const bool tr = tr0 && i < p.trace_n;
-            mbar_wait(acc_full, i & 1);
-            if (tr) p.trace[7 * p.trace_n + i] = clock64();                                     // [7] epilogue starts
-            const int held = *mailbox;
-            const float* tile = in_ring ? reinterpret_cast<const float*>(smem + (size_t)held * stage_bytes) : tile_sep;
-            // split: the held stage's rows first, then give the stage back and do the rest from the half tile
-            for (int part = 0; part < (split ? 2 : 1); ++part) {
-                const bool last = !split || part == 1;
-                amax = fmaxf(amax, tcp_epi_tile<BN>(p, part == 0 ? tile : tile_hi, LD, u, mt_units, et, swz, 64 * part, last ? 128 : 64));
-                // every epilogue thread is done reading the held stage (and the mailbox): give the stage back to the producer (empty[] counts
-                // the 8 consumer warps' arrivals), and at the end the staging buffers to the consumers
-                if (in_ring && part == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic accesses to the stage before the next TMA write into it
-                epilogue_sync();
-                if (et == 0) {
-                    if (in_ring && part == 0) {
-                        mbar_arrive(&empty[held], TC_CONSUMERS / 32);
-                        if (tr) p.trace[8 * p.trace_n + i] = clock64();                         // [8] stage released
-                    }
-                    if (last) {
-                        mbar_arrive(acc_empty);
-                        if (tr) p.trace[11 * p.trace_n + i] = clock64();                        // [11] epilogue done
+    if (warp >= TC_CONSUMERS / 32) {
+        // (epilogue-warp tiles) every warp of a warpgroup executes the same setmaxnreg: before the producer / epilogue split
+        if constexpr (epi_warps) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TCP_REG_EPI));
+        if (warp > TC_CONSUMERS / 32) {
+            // ================= epilogue warps: tile i of this CTA is handed over through acc_full / acc_empty phase i =================
+            if (!epi_warps) return;
+            const int et = (int)threadIdx.x - (TC_CONSUMERS + 32);
+            const bool tr0 = p.trace && blockIdx.x == 0 && et == 0;
+            float amax = 0.f;
+            int i = 0;
+            for (int u = u0; u < units; u += ustep, ++i) {
+                const bool tr = tr0 && i < p.trace_n;
+                mbar_wait(acc_full, i & 1);
+                if (tr) p.trace[7 * p.trace_n + i] = clock64();                                     // [7] epilogue starts
+                const int held = *mailbox;
+                const float* tile = in_ring ? reinterpret_cast<const float*>(smem + (size_t)held * stage_bytes) : tile_sep;
+                // split: the held stage's rows first, then give the stage back and do the rest from the half tile
+                for (int part = 0; part < (split ? 2 : 1); ++part) {
+                    const bool last = !split || part == 1;
+                    amax = fmaxf(amax, tcp_epi_tile<BN>(p, part == 0 ? tile : tile_hi, LD, u, mt_units, et, swz, 64 * part, last ? 128 : 64));
+                    // every epilogue thread is done reading the held stage (and the mailbox): give the stage back to the producer (empty[] counts
+                    // the 8 consumer warps' arrivals), and at the end the staging buffers to the consumers
+                    if (in_ring && part == 0) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic accesses to the stage before the next TMA write into it
+                    epilogue_sync();
+                    if (et == 0) {
+                        if (in_ring && part == 0) {
+                            mbar_arrive(&empty[held], TC_CONSUMERS / 32);
+                            if (tr) p.trace[8 * p.trace_n + i] = clock64();                         // [8] stage released
+                        }
+                        if (last) {
+                            mbar_arrive(acc_empty);
+                            if (tr) p.trace[11 * p.trace_n + i] = clock64();                        // [11] epilogue done
+                        }
                     }
                 }
             }
-        }
-        note_fp16_range(amax, p.range_flag);
-    } else if (warp == TC_CONSUMERS / 32) {
-        if (lane == 0) {
-            // ================= TMA producer =================
-            const bool lo_too = mode != 1 && !(p.dbg & 2);
-            const uint32_t tx = lo_too ? stage_bytes : a_bytes + b_bytes;
-            int it = 0, s = 0, i = 0;
-            int ph = 0;                                         // bit s: parity of slot s's next fill
-            int held = -1;                                      // (in_ring) slot of the latest tile's last k-block, until seen released
-            int le = 0;                                         // slot_log entry of k-block it
-            for (int u = u0; u < units; u += ustep, ++i) {
-                int skips = 0;
-                int mu, nt;
-                unit_tile(p, u, mt_units, mu, nt);
-                const TcGeom geo = tile_geom(p, mu);
-                const int b = geo.b;
-                const int wi0 = geo.tw * TC_TW * p.stride_w - p.pad_w, hi0 = geo.th * TC_TH * p.stride - p.pad;
-                const CUtensorMap* mA = &mapA;
-                const CUtensorMap* mAlo = &mapAlo;
-                if constexpr (LV) { mA = &lmaps.a[geo.lvl]; mAlo = &lmaps.alo[geo.lvl]; }
-                const int n0 = nt * BN;
-                int tap = 0, kh = 0, kw = 0, c0 = 0;
-                for (int kb = 0; kb < KB; ++kb, ++it) {
-                    int slot = s;
-                    if (held < 0) mbar_wait(&empty[s], ((ph >> s) & 1) ^ 1);
-                    else {
-                        // The epilogue may still be reading the held stage.  Take it as soon as it is released; until then take the next
-                        // slot in round-robin order, passing over the held one (the slot after it is not held).
-                        const bool at_held = s == held;
-                        if (at_held && ++s == p.stages) s = 0;
-                        const uint32_t hpar = ((ph >> held) & 1) ^ 1, spar = ((ph >> s) & 1) ^ 1;
-                        long long t0 = 0;
-                        for (uint32_t spins = 1;; ++spins) {
-                            if (mbar_test(&empty[held], hpar)) { slot = held; held = -1; break; }
-                            if (mbar_test(&empty[s], spar)) { slot = s; skips += at_held; break; }
-                            if ((spins & 0xFFFu) == 0) {                // bounded, as mbar_wait
-                                const long long t = clock64();
-                                if (t0 == 0) t0 = t; else if (t - t0 > 4000000000LL) __trap();
+            note_fp16_range(amax, p.range_flag);
+        } else {
+            if (lane == 0) {
+                // ================= TMA producer =================
+                const bool lo_too = mode != 1 && !(p.dbg & 2);
+                const uint32_t tx = lo_too ? stage_bytes : a_bytes + b_bytes;
+                int it = 0, s = 0, i = 0;
+                int ph = 0;                                         // bit s: parity of slot s's next fill
+                int held = -1;                                      // (in_ring) slot of the latest tile's last k-block, until seen released
+                int le = 0;                                         // slot_log entry of k-block it
+                for (int u = u0; u < units; u += ustep, ++i) {
+                    int skips = 0;
+                    int mu, nt;
+                    unit_tile(p, u, mt_units, mu, nt);
+                    const TcGeom geo = tile_geom(p, mu);
+                    const int b = geo.b;
+                    const int wi0 = geo.tw * TC_TW * p.stride_w - p.pad_w, hi0 = geo.th * TC_TH * p.stride - p.pad;
+                    const CUtensorMap* mA = &mapA;
+                    const CUtensorMap* mAlo = &mapAlo;
+                    if constexpr (LV) { mA = &lmaps.a[geo.lvl]; mAlo = &lmaps.alo[geo.lvl]; }
+                    const int n0 = nt * BN;
+                    int tap = 0, kh = 0, kw = 0, c0 = 0;
+                    for (int kb = 0; kb < KB; ++kb, ++it) {
+                        int slot = s;
+                        if (held < 0) mbar_wait(&empty[s], ((ph >> s) & 1) ^ 1);
+                        else {
+                            // The epilogue may still be reading the held stage.  Take it as soon as it is released; until then take the next
+                            // slot in round-robin order, passing over the held one (the slot after it is not held).
+                            const bool at_held = s == held;
+                            if (at_held && ++s == p.stages) s = 0;
+                            const uint32_t hpar = ((ph >> held) & 1) ^ 1, spar = ((ph >> s) & 1) ^ 1;
+                            long long t0 = 0;
+                            for (uint32_t spins = 1;; ++spins) {
+                                if (mbar_test(&empty[held], hpar)) { slot = held; held = -1; break; }
+                                if (mbar_test(&empty[s], spar)) { slot = s; skips += at_held; break; }
+                                if ((spins & 0xFFFu) == 0) {                // bounded, as mbar_wait
+                                    const long long t = clock64();
+                                    if (t0 == 0) t0 = t; else if (t - t0 > 4000000000LL) __trap();
+                                }
                             }
                         }
+                        if (slot == s && ++s == p.stages) s = 0;
+                        ph ^= 1 << slot;
+                        const bool tr = p.trace && blockIdx.x == 0 && it < p.trace_n;
+                        if (tr) p.trace[it] = clock64();                                          // [0] stage free, about to issue the loads
+                        slot_log[le] = slot;
+                        mbar_arrive(&log_bar[le]);
+                        if (++le > p.stages) le = 0;
+                        if (in_ring && kb == KB - 1) held = slot;
+                        uint8_t* st = smem + (size_t)slot * stage_bytes;
+                        const int wi = wi0 + kw * p.dil, hi = hi0 + kh * p.dil;
+                        const int kcol = tap * p.cin_pad + c0;
+                        mbar_expect_tx(&full[slot], tx);
+                        tma_load_4d(st, mA, &full[slot], c0, wi, hi, b);
+                        if (lo_too) tma_load_4d(st + a_bytes, mAlo, &full[slot], c0, wi, hi, b);
+                        tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[slot], kcol, n0);
+                        if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[slot], kcol, n0);
+                        if (tr) { p.trace[p.trace_n + it] = clock64(); p.trace[9 * p.trace_n + it] = slot; }  // [1] loads issued, [9] slot
+                        // k-block order: channel chunk outermost, taps inside
+                        ++tap;
+                        if (++kw == p.KW) { kw = 0; ++kh; }
+                        if (tap == p.KH * p.KW) { tap = 0; kh = 0; kw = 0; c0 += kbc; }
                     }
-                    if (slot == s && ++s == p.stages) s = 0;
-                    ph ^= 1 << slot;
-                    const bool tr = p.trace && blockIdx.x == 0 && it < p.trace_n;
-                    if (tr) p.trace[it] = clock64();                                          // [0] stage free, about to issue the loads
-                    slot_log[le] = slot;
-                    mbar_arrive(&log_bar[le]);
-                    if (++le > p.stages) le = 0;
-                    if (in_ring && kb == KB - 1) held = slot;
-                    uint8_t* st = smem + (size_t)slot * stage_bytes;
-                    const int wi = wi0 + kw * p.dil, hi = hi0 + kh * p.dil;
-                    const int kcol = tap * p.cin_pad + c0;
-                    mbar_expect_tx(&full[slot], tx);
-                    tma_load_4d(st, mA, &full[slot], c0, wi, hi, b);
-                    if (lo_too) tma_load_4d(st + a_bytes, mAlo, &full[slot], c0, wi, hi, b);
-                    tma_load_2d(st + 2 * a_bytes, &mapWhi, &full[slot], kcol, n0);
-                    if (lo_too) tma_load_2d(st + 2 * a_bytes + b_bytes, &mapWlo, &full[slot], kcol, n0);
-                    if (tr) { p.trace[p.trace_n + it] = clock64(); p.trace[9 * p.trace_n + it] = slot; }  // [1] loads issued, [9] slot
-                    // k-block order: channel chunk outermost, taps inside
-                    ++tap;
-                    if (++kw == p.KW) { kw = 0; ++kh; }
-                    if (tap == p.KH * p.KW) { tap = 0; kh = 0; kw = 0; c0 += kbc; }
+                    if (p.trace && blockIdx.x == 0 && i < p.trace_n) p.trace[10 * p.trace_n + i] = skips;     // [10] held slot passed over
                 }
-                if (p.trace && blockIdx.x == 0 && i < p.trace_n) p.trace[10 * p.trace_n + i] = skips;     // [10] held slot passed over
             }
         }
     } else {
+        if constexpr (epi_warps) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TCP_REG_CONSUMER));
         // ================= consumer warpgroups: MMAs, chunk promotion, epilogue =================
         const int wg = warp >> 2;
         const uint32_t sbo = 8u * rowb, lay = rowb == 128u ? 2u : 4u;
@@ -540,7 +549,7 @@ static int tcp_launch(TcParams& p, const CUtensorMap& mA, const CUtensorMap& mAl
     cudaError_t le = cudaErrorInvalidValue;
     VD3D_REQUIRE(!lm || (p.f16 && p.n_levels > 0), "conv2d_tc: multi-level launches take fp16 operands");
     const TcNoLevelMaps nolm{0};
-#define VD3D_TCP_LAUNCH(N, F16, LV, LM) tc_launch<conv2d_tcp_kernel<N, F16, LV>>(grid, TCP_THREADS, smem, stream, mA, mAlo, mWhi, mWlo, p, LM)
+#define VD3D_TCP_LAUNCH(N, F16, LV, LM) tc_launch<conv2d_tcp_kernel<N, F16, LV>>(grid, tcp_threads(N), smem, stream, mA, mAlo, mWhi, mWlo, p, LM)
 #define VD3D_TCP_CASE(N) case N: le = lm ? VD3D_TCP_LAUNCH(N, true, true, *lm) : p.f16 ? VD3D_TCP_LAUNCH(N, true, false, nolm) : VD3D_TCP_LAUNCH(N, false, false, nolm); break
     switch (BN) {
         VD3D_TCP_CASE(16); VD3D_TCP_CASE(32); VD3D_TCP_CASE(48); VD3D_TCP_CASE(64);
@@ -596,14 +605,6 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
                 mt_all += cdiv(Wo_, TC_TW) * cdiv(Ho_, TC_TH) * B;
             }
             BN = pick_bn_cost(Cout, mt_all);
-            // short-K layers (the 1x1 expansion convs of the ResNet bottlenecks: 4 k-blocks, wide output, residual): a tile's MMAs are over
-            // before its epilogue has fetched the first residual columns; 64-column tiles put twice as many CTAs on the output
-            const char* esk = getenv("VD3D_TC_SHORTK");
-            const int shortk = esk ? atoi(esk) : 8;
-            const int kb_total = KH * KW * ((Cin + 63) / 64);
-            const char* esr = getenv("VD3D_TC_SHORTK_RES");          // 1 (default): only layers with a residual; 0: every short-K layer
-            const bool need_res = !(esr && atoi(esr) == 0);
-            if (shortk > 0 && kb_total <= shortk && BN > 64 && Cout % 64 == 0 && (!need_res || res || res_h16_hi)) BN = 64;
         } else BN = vd3d_tc_pick_bn(Cout);
     }
     VD3D_REQUIRE(BN % 16 == 0 && BN >= 16 && BN <= 256, "conv2d_tc: BN must be a multiple of 16 in [16, 256]");
