@@ -75,40 +75,26 @@ int vd3d_conv2d_tc(const float* in, const float* in_lo, int B, int H, int W, int
  * (22 significant bits); three kind::f16 MMAs per k-step (Alo*Whi + Ahi*Wlo + Ahi*Whi), 64 channels per k-block: half the
  * shared-memory / L2 operand bytes and twice the MMA rate of the tf32 form at the same accuracy.  Weights are pre-scaled by a
  * power of two S on the host (so that their lo parts stay normal fp16 numbers); out_scale = 1/S is applied to the accumulator.
- *   in_hi / in_lo   : fp16 NHWC planes with the same pitch / offset convention as the fp32 tensors
- *   w_hi / w_lo     : fp16 [Cout][KH*KW*cin_pad], cin_pad = Cin rounded up to 64 (zero filled)
- *   out             : fp32 NHWC result; out_hi16 / out_lo16 (optional pair): its fp16 planes for the next conv
- *   stride          : 1..4 (strided convs load every stride-th pixel through the TMA traversal stride); Cin % 8 == 0, Cout % 4 == 0 */
-int vd3d_conv2d_tc16(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                     const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
-                     int stride, const float* res, int res_cs, int res_co,
-                     float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int passes, int bn,
-                     void* stream);
-/* Planes-only form of vd3d_conv2d_tc16 (3 passes, persistent engine): between two tensor-core convs an activation is consumed as its
- * fp16 (hi, lo) planes only, so the fp32 copy need not exist at all.  `out` may be NULL (only out_hi16 / out_lo16 are written: half the
- * output bytes of a layer), and the residual may be given as planes (res_hi16 / res_lo16, value = hi + lo, exact to 2^-22 relative: the
- * planes ARE the tensor) instead of an fp32 tensor `res`; pitch / offset res_cs / res_co apply to whichever form is passed. */
-int vd3d_conv2d_tc16_planes(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                            const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
-                            int stride, const float* res, const void* res_hi16, const void* res_lo16, int res_cs, int res_co,
-                            float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
-/* vd3d_conv2d_tc16 with the FPN top-down add fused into the epilogue (R/detectors/retinanet_2d.py:49-52): out = conv(in) + bias +
- * nearest_up2(res), where res is the fp32 tensor [B][res_H][res_W][res_cs] at exactly half the output size (Ho = 2 res_H, Wo = 2 res_W):
- * output pixel (y, x) reads residual pixel (y >> 1, x >> 1).  3 passes; bn <= 0 = the library's tile policy. */
-int vd3d_conv2d_tc16_res_up2(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                             const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
-                             int stride, const float* res, int res_cs, int res_co, int res_H, int res_W,
-                             float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
-/* One launch of the same conv over L <= 5 tensors of different sizes (the shared-weight RetinaNet head over the pyramid levels, whole batch):
- * level l reads in_hi[l] / in_lo[l] [B][H[l]][W[l]][in_cs] (its own zero padding) and writes out[l] / out_hi16[l] / out_lo16[l]; the M tiles of all
- * levels form one persistent tile schedule.  Every output form of level l must lie at a whole-pixel offset from level 0's, the same for all
- * forms (levels concatenated in one allocation per form); likewise res[l] (fp32, optional; res_W[l] > 0: [B][res_H[l]][res_W[l]] at half the
- * output size, read nearest-upsampled).  Bit-identical to L separate vd3d_conv2d_tc16 launches (same K order per output pixel). */
-int vd3d_conv2d_tc16_levels(int L, const void* const* in_hi, const void* const* in_lo, const int* H, const int* W, int B, int Cin, int in_cs,
-                            int in_co, const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad,
-                            int dil, int stride, const void* const* res, const int* res_H, const int* res_W, int res_cs, int res_co,
-                            const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
-                            int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
+ * One launch runs the conv over L <= 5 tensors of different sizes ("levels": the shared-weight RetinaNet head over the pyramid, whole
+ * batch; L = 1 for an ordinary conv).  Every tensor argument is an array of L pointers, one per level; the M tiles of all levels form one
+ * persistent tile schedule, bit-identical to L separate launches (same K order per output pixel).
+ *   in_hi / in_lo     : fp16 NHWC planes [B][H[l]][W[l]] with the same pitch / offset convention as the fp32 tensors (each level its own padding)
+ *   w_hi / w_lo       : fp16 [Cout][KH*KW*cin_pad], cin_pad = Cin rounded up to 64 (zero filled)
+ *   out               : fp32 NHWC result (NULL: not written); out_hi16 / out_lo16 (optional pair): its fp16 planes for the next conv.
+ *                       Between two tensor-core convs an activation may exist as its planes only: half the output bytes of a layer.
+ *   res               : optional fp32 residual; res_W[l] > 0 (res_H / res_W may be NULL): level l's residual is [B][res_H[l]][res_W[l]] at
+ *                       exactly half the output size, added nearest-upsampled (the FPN top-down add, R/detectors/retinanet_2d.py:49-52)
+ *   res_hi16 / res_lo16: or the residual as fp16 planes (value = hi + lo; L = 1, 3 passes); res_cs / res_co apply to either form
+ *   passes            : 3, or 2 (error-budget experiments: the A_lo * W_hi product dropped); bn <= 0: the library's tile policy
+ * With L > 1 every output form (and res) of level l must lie at a whole-pixel offset from level 0's, the same for all forms (levels
+ * concatenated in one allocation per form).  stride 1..4 (strided convs load every stride-th pixel through the TMA traversal stride);
+ * Cin % 8 == 0, Cout % 4 == 0. */
+int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* const* in_lo, const int* H, const int* W, int B, int Cin, int in_cs,
+                     int in_co, const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad,
+                     int dil, int stride, const void* const* res, const void* const* res_hi16, const void* const* res_lo16,
+                     const int* res_H, const int* res_W, int res_cs, int res_co,
+                     const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
+                     int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream);
 /* Few-channel KHxKW convolution (the ResNet / DLA stem: conv1 7x7 stride 2, R/backbones/resnet.py:120,186) on the tensor cores.
  * The image is held as fp16 (hi, lo) planes [B][H][Wp][4] (pixel x at column x + pad, zeros elsewhere: the buffer must be
  * zero-initialised once); Wp = vd3d_stem_row_pitch(W, KW, stride, pad).  vd3d_image_to_h16_rows fills the planes from an

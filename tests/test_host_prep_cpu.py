@@ -37,19 +37,26 @@ def test_fp16_split_carries_22_bits():
 
 
 def test_conv_layer_scales_weights_into_fp16_range():
-    """the tensor-core layer stores W * 2^k with max |W| 2^k in [8192, 16384) and undoes it with out_scale = 2^-k (exact)"""
+    """the tensor-core layers store W * 2^k with max |W| 2^k in [8192, 16384) (k within +-24) and undo it with out_scale = 2^-k (exact)"""
     g = torch.Generator().manual_seed(2)
     for scale in (1e-4, 1.0, 300.0):
         w = torch.randn(32, 64, 3, 3, generator=g) * scale
-        layer = E.ConvLayer(w, None, None, pad=1, device="cpu", engine="tc16")
-        # on a CPU "device" the layer falls back to the SIMT packing (no GPU): the scaling rule itself is what is checked here
-        wk = w.double().abs().max()
+        wm = w.double().reshape(32, -1)
+        hi, lo, out_scale = E.fp16_split_scaled(wm)
+        wk = wm.abs().max()
         k = int(np.floor(np.log2(16384.0 / float(wk))))
         assert 8192.0 <= float(wk) * 2.0 ** k < 16384.0
-        hi, lo = E.fp16_split(w.double() * 2.0 ** k)
-        rec = (hi.double() + lo.double()) * 2.0 ** -k
-        assert float((rec - w.double()).abs().max()) <= float(wk) * 2.0 ** -21
+        k = max(-24, min(24, k))
+        assert out_scale == 2.0 ** -k
+        assert all(torch.equal(a, b) for a, b in zip((hi, lo), E.fp16_split(wm * 2.0 ** k)))
+        rec = (hi.double() + lo.double()) * out_scale
+        assert float((rec - wm).abs().max()) <= float(wk) * 2.0 ** -21
+        layer = E.ConvLayer(w, None, None, pad=1, device="cpu", engine="tc16")
         assert layer.engine == "simt"                 # and a CPU-device layer never claims the tensor-core engine
+    # the scale stays within 2^+-24, and an all-zero matrix is not scaled
+    assert E.fp16_split_scaled(torch.full((4, 8), 1e-12, dtype=torch.float64))[2] == 2.0 ** -24
+    assert E.fp16_split_scaled(torch.full((4, 8), 1e12, dtype=torch.float64))[2] == 2.0 ** 24
+    assert E.fp16_split_scaled(torch.zeros(4, 8, dtype=torch.float64))[2] == 1.0
 
 
 def test_stem_weight_layout():

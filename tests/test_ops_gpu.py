@@ -231,33 +231,11 @@ def test_conv2d_tc_3xtf32_vs_fp32(case):
     assert torch.equal(got_lo, val - _trunc13(val))
 
 
-# (VD3D_TC_HALO, VD3D_TC_PERSIST, VD3D_TC_CG, VD3D_TC_PHALO)
-TC16_MODES = {"default": ("0", "1", "0", "2"), "auto": ("0", "1", "0", "1"), "persistent": ("0", "1", "1", "1"), "pair": ("0", "1", "2", "1"),
-              "auto-generic": ("0", "1", "0", "0"), "persistent-generic": ("0", "1", "1", "0"), "pair-generic": ("0", "1", "2", "0"),
-              "tile": ("0", "0", "1", "0"), "halo2": ("2", "1", "1", "0"), "halo1": ("1", "1", "1", "0")}
-
-
-def _tc16_mode(monkeypatch, mode):
-    """Engine switches of the Blackwell build (on H100 every mode runs the one persistent wgmma kernel; the modes stay as inputs): persistent kernel, CTA pairs for tiles wider than 128 columns and input-halo reuse
-    (A staged once per channel chunk for the nine taps) for those paired 3x3 stride-1 convs; auto / persistent / pair: halo reuse
-    for every 3x3 stride-1 conv with automatic pairing / one CTA per SM / CTA pairs everywhere;
-    *-generic: per-tap input boxes for every conv (no halo reuse); tile: one CTA per output tile (round-1 kernel);
-    halo2 / halo1: round-1 halo kernels."""
-    halo, persist, cg, phalo = TC16_MODES[mode]
-    monkeypatch.setenv("VD3D_TC_HALO", halo)
-    monkeypatch.setenv("VD3D_TC_PERSIST", persist)
-    monkeypatch.setenv("VD3D_TC_CG", cg)
-    monkeypatch.setenv("VD3D_TC_PHALO", phalo)
-
-
-@pytest.mark.parametrize("mode", list(TC16_MODES))
 @pytest.mark.parametrize("case", TC_CASES)
-def test_conv2d_tc16_fp16split_vs_fp64(case, mode, monkeypatch):
+def test_conv2d_tc16_fp16split_vs_fp64(case):
     """fp16-split tensor-core conv (3 kind::f16 MMAs on (hi, lo) fp16 planes, 22 significant bits): same accuracy bar as the
-    3xTF32 form, checked against an fp64 convolution; also checks the fp16 planes the epilogue writes for the next layer.
-    halo = 2 / 1: 3x3 convs stage the input halo once per channel chunk (full / vertical reuse); 0: generic per-tap boxes."""
+    3xTF32 form, checked against an fp64 convolution; also checks the fp16 planes the epilogue writes for the next layer."""
     E = _E()
-    _tc16_mode(monkeypatch, mode)
     B, Cin, H, W, Cout, k, p, d, has_b, has_r, relu = case
     g = torch.Generator().manual_seed(sum(case[:6]) + 1)
     x = torch.randn(B, Cin, H, W, generator=g)
@@ -365,13 +343,11 @@ TC16_EXTRA = [
 ]
 
 
-@pytest.mark.parametrize("mode", ["auto", "persistent", "pair", "tile"])
 @pytest.mark.parametrize("case", TC16_EXTRA)
-def test_conv2d_tc16_strided_and_ragged_channels(case, mode, monkeypatch):
+def test_conv2d_tc16_strided_and_ragged_channels(case):
     """stride > 1 goes through the TMA traversal stride (every stride-th pixel lands densely in shared memory);
     channel counts that are not multiples of the 64-channel k-block / 16-column MMA granule are zero-filled / masked."""
     E = _E()
-    _tc16_mode(monkeypatch, mode)
     B, Cin, H, W, Cout, k, p, s_ = case
     g = torch.Generator().manual_seed(sum(case))
     x = torch.randn(B, Cin, H, W, generator=g)
@@ -393,13 +369,11 @@ def test_conv2d_tc16_strided_and_ragged_channels(case, mode, monkeypatch):
     assert float(out.lo[..., :4].float().min()) == 7.0 and float(out.lo[..., 4 + Cout:].float().min()) == 7.0
 
 
-@pytest.mark.parametrize("mode", ["default", "auto", "persistent", "pair", "auto-generic", "persistent-generic", "pair-generic"])
-def test_conv2d_tc16_persistent_many_tiles(mode, monkeypatch):
+def test_conv2d_tc16_persistent_many_tiles():
     """more output tiles than SMs (every CTA loops several times, the TMA ring and the chunk promotion wrap across tiles),
     an odd number of M tiles (the second CTA of the last pair is dead) and several N tiles; checked against the exact-fp32
     SIMT engine of the same library."""
     E = _E()
-    _tc16_mode(monkeypatch, mode)
     g = torch.Generator().manual_seed(11)
     # Cout = 608 -> three tiles of 208 columns, the last one ragged (192 valid); 1408 -> six tiles of 240 (last 208): the head shape
     for (B, Cin, H, W, Cout) in ((3, 64, 40, 112, 64), (1, 128, 24, 80, 384), (5, 64, 24, 48, 96), (3, 64, 24, 48, 608), (1, 64, 24, 80, 1408),
@@ -415,16 +389,16 @@ def test_conv2d_tc16_persistent_many_tiles(mode, monkeypatch):
         ref = simt(E.Act(xa.t), E.Act(torch.empty(B, H, W, Cout, device="cuda")), res=ra).t
         out = tc(xa, E.Act(torch.zeros(B, H, W, Cout, device="cuda"), 0, None, torch.zeros(2, B, H, W, Cout, device="cuda", dtype=torch.float16)), res=ra)
         err = float((out.t - ref).abs().max())
-        print((B, Cin, H, W, Cout), mode, "max|tc16 - simt|", err)
+        print((B, Cin, H, W, Cout), "max|tc16 - simt|", err)
         assert err < 2e-5, err
         hi = out.t.half()
         assert torch.equal(out.lo[0], hi) and torch.equal(out.lo[1], (out.t - hi.float()).half())
 
 
-def test_conv2d_tc16_tile_policies_are_bit_identical(monkeypatch):
-    """The tile policy depends on the problem size (tile width, CTA pairs, input-halo reuse), so the same layer may run through
-    different kernels at different batch sizes: every persistent variant must accumulate in the same order and give
-    bit-identical results (batch invariance of the detectors rests on this)."""
+def test_conv2d_tc16_tile_policies_are_bit_identical():
+    """The tile policy depends on the problem size (tile width), so the same layer may run with different tiles at different batch
+    sizes: every tile width must accumulate in the same order and give bit-identical results (batch invariance of the detectors rests
+    on this)."""
     E = _E()
     g = torch.Generator().manual_seed(3)
     B, Cin, H, W, Cout = 2, 128, 24, 80, 384
@@ -434,24 +408,20 @@ def test_conv2d_tc16_tile_policies_are_bit_identical(monkeypatch):
     layer = E.ConvLayer(w, b, None, pad=1, relu=True, device="cuda", engine="tc16")
     xa = E.split_lo(E.Act(x.cuda(), 0, None, torch.zeros(2, B, H, W, Cin, device="cuda", dtype=torch.float16)))
     outs = {}
-    for mode in ("default", "auto", "persistent", "pair", "auto-generic", "persistent-generic", "pair-generic"):
-        _tc16_mode(monkeypatch, mode)
-        for bn in (0, 96, 128, 192):
-            layer.bn_tile = bn
-            outs[(mode, bn)] = layer(xa, E.Act(torch.zeros(B, H, W, Cout, device="cuda"))).t.clone()
-    ref = outs[("default", 0)]
+    for bn in (0, 96, 128, 192):
+        layer.bn_tile = bn
+        outs[bn] = layer(xa, E.Act(torch.zeros(B, H, W, Cout, device="cuda"))).t.clone()
+    ref = outs[0]
     for k, v in outs.items():
         assert torch.equal(v, ref), k
 
 
 @pytest.mark.parametrize("win", ["32", "64"])
-@pytest.mark.parametrize("mode", ["persistent", "pair"])
 @pytest.mark.parametrize("shape", [(2, 3, 64, 96), (1, 3, 37, 53), (3, 3, 96, 320)])
-def test_stem_tensor_core_vs_fp64(shape, mode, win, monkeypatch):
+def test_stem_tensor_core_vs_fp64(shape, win, monkeypatch):
     """conv1 7x7 stride 2 + BN + ReLU (R/backbones/resnet.py:120-122) through the row-window tensor-core path
     (image -> zero-padded fp16 row planes -> KHx1 conv over 64 virtual channels) against an fp64 convolution."""
     E = _E()
-    _tc16_mode(monkeypatch, mode)
     monkeypatch.setenv("VD3D_STEM_WIN", win)          # 32: 8-pixel windows on 64-byte swizzle rows (default), 64: 16-pixel windows on 128-byte rows
     B, C, H, W = shape
     g = torch.Generator().manual_seed(sum(shape))
@@ -469,7 +439,7 @@ def test_stem_tensor_core_vs_fp64(shape, mode, win, monkeypatch):
     for _ in range(2):                      # second call reuses the zero-bordered row planes
         layer(x.cuda(), out, arena, "t")
     err = float((out.to_nchw().cpu().double() - ref64).abs().max())
-    print(shape, mode, "stem max|err| vs fp64", err)
+    print(shape, win, "stem max|err| vs fp64", err)
     assert err < 2e-5, err
     assert float(out.t[..., :4].min()) == 7.0 and float(out.t[..., 68:].min()) == 7.0
 

@@ -164,7 +164,7 @@ def test_in_place_batchnorm_statistic_refolds_the_plan():
 @pytest.mark.parametrize("cout", [256, 128, 36, 32])
 @pytest.mark.parametrize("with_res", [False, True])
 def test_multilevel_launch_equals_per_level_launches(B, cout, with_res):
-    """One vd3d_conv2d_tc16_levels launch over ragged levels (sizes not multiples of the 16 x 8 tile) == the same conv launched level by level,
+    """One multi-level vd3d_conv2d_tc16 launch over ragged levels (sizes not multiples of the 16 x 8 tile) == the same conv launched level by level,
     bit for bit in the fp32 output and both fp16 planes; with_res: every level adds a half-resolution residual read nearest-upsampled."""
     from visualdet3d_b200 import engine as E
     g = torch.Generator().manual_seed(7 * B + cout + with_res)

@@ -61,11 +61,9 @@ for name in CASES:
     run(name, "default tile policy", {}, 0)
     for bn in (256, 192, 128, 96, 64):
         run(name, f"bn_tile = {bn}", {}, bn)
-    run(name, "bn 128, CTA pairs", {"VD3D_TC_CG": 2}, 128)
     run(name, "default, no epilogue output", {"VD3D_TC_DEBUG": 16}, 0)
     run(name, "default, no residual loads", {"VD3D_TC_DEBUG": 32}, 0)
     run(name, "default, one MMA per k-step", {"VD3D_TC_DEBUG": 1}, 0)
     run(name, "bn 128, no epilogue output", {"VD3D_TC_DEBUG": 16}, 128)
-    run(name, "default, no halo kernel", {"VD3D_TC_PHALO": 0}, 0)
     for bn in (256, 128, 64):
         run(name, f"planes-only output (+ plane residual), bn {bn}", {}, bn, planes_only=True)

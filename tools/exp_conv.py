@@ -1,5 +1,5 @@
-"""Where does the time of the narrow (64 / 128-channel) tensor-core convs go?  CUDA-event timing of ONE layer shape under engine switches and
-timing knock-outs (VD3D_TC_DEBUG: results wrong), with fp32 + planes output vs planes-only output / plane residual.
+"""Where does the time of the narrow (64 / 128-channel) tensor-core convs go?  CUDA-event timing of ONE layer shape under the tile-order and
+promotion-chunk settings and timing knock-outs (VD3D_TC_DEBUG: results wrong), with fp32 + planes output vs planes-only output / plane residual.
 usage: python tools/exp_conv.py [shape] [reps]     shape: layer1 | layer2 | layer3 | head"""
 import os, sys
 import numpy as np
@@ -57,13 +57,9 @@ for mode in ("f32", "planes", "nores"):
     run("default", {}, mode)
 for l2 in (0, 28, 44, 64):
     run(f"L2-aware tile order, block = {l2} MB", {"VD3D_TC_L2MB": l2}, "f32")
-run("no input-halo reuse / no resident weights (generic kernel)", {"VD3D_TC_PHALO": 0, "VD3D_TC_WRES": 0}, MK)
-run("generic kernel, CTA pairs", {"VD3D_TC_PHALO": 0, "VD3D_TC_WRES": 0, "VD3D_TC_CG": 2}, MK)
-run("halo kernel always, no resident weights", {"VD3D_TC_PHALO": 1, "VD3D_TC_WRES": 0}, MK)
 for dbg, lab in ((16, "knock-out: no epilogue output"), (32, "knock-out: no residual loads"), (48, "knock-out: no output, no residual"),
                  (2, "knock-out: no lo-plane loads"), (1, "knock-out: one MMA per k-step"), (51, "knock-out: 1 MMA, no lo loads, no output, no residual")):
     run(lab, {"VD3D_TC_DEBUG": dbg}, MK)
-    run(lab + " (generic kernel)", {"VD3D_TC_DEBUG": dbg, "VD3D_TC_PHALO": 0, "VD3D_TC_WRES": 0}, MK)
 for dbg, lab in ((64, "knock-out: 1/12 of the MMAs (first K step, one pass), all loads"), (66, "knock-out: 1/12 of the MMAs, no lo loads"),
                  (114, "knock-out: 1/12 MMAs, no lo loads, no output, no residual")):
     run(lab, {"VD3D_TC_DEBUG": dbg}, MK)

@@ -1,15 +1,14 @@
-"""Time single tensor-core convs of the dominant shapes under several engine settings and check each against the exact-fp32 SIMT engine.
-usage: VD3D_TC_ENV_DYNAMIC=1 python tools/prof_conv.py [reps] [configs]
-  configs: comma list of persist:cg:bn  (bn 0 = default tile), e.g. 0:1:0,1:1:0,1:2:0,1:1:256"""
+"""Time single tensor-core convs of the dominant shapes at several tile widths and check each against the exact-fp32 SIMT engine.
+usage: python tools/prof_conv.py [reps] [bns]
+  bns: comma list of tile widths (0 = the library's tile policy), e.g. 0,64,128"""
 import os, sys
-os.environ.setdefault("VD3D_TC_ENV_DYNAMIC", "1")
 import numpy as np
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from visualdet3d_b200 import engine as E
 
 reps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
-configs = [tuple(int(v) for v in (c.split(":") + ["1"])[:4]) for c in (sys.argv[2] if len(sys.argv) > 2 else "1:0:0:0,1:0:0:1").split(",")]   # persist:cg:bn[:phalo]
+bns = [int(v) for v in (sys.argv[2] if len(sys.argv) > 2 else "0").split(",")]
 SHAPES = [("head 1408->1408 @24x80 B8", 8, 24, 80, 1408, 1408, 1), ("layer1 64->64 @96x320 B16", 16, 96, 320, 64, 64, 1),
           ("layer2 128->128 @48x160 B16", 16, 48, 160, 128, 128, 1), ("layer3 256->256 @24x80 B16", 16, 24, 80, 256, 256, 1),
           ("layer2.0 64->128 s2 @96x320 B16", 16, 96, 320, 64, 128, 2), ("odd 72->72 @47x79 B3", 3, 47, 79, 72, 72, 1),
@@ -31,8 +30,7 @@ for name, B, H, W, Cin, Cout, stride in SHAPES:
     ref = ref_layer(E.Act(x.t), E.Act(torch.empty(B, Ho, Wo, Cout, device="cuda")), res=res).t
     torch.cuda.synchronize()
     cases.append((name, B, Ho, Wo, Cin, Cout, layer, 0, x, res, ref))
-for persist, cg, bn, phalo in configs:          # configs outermost: a trapping experimental config cannot hide the results of the safe ones
-    os.environ["VD3D_TC_PERSIST"], os.environ["VD3D_TC_CG"], os.environ["VD3D_TC_PHALO"] = str(persist), str(cg), str(phalo)
+for bn in bns:
     for name, B, Ho, Wo, Cin, Cout, layer, bn0, x, res, ref in cases:
         layer.bn_tile = bn if bn else bn0
         out = E.Act(torch.zeros(B, Ho, Wo, Cout, device="cuda"), 0, None, torch.zeros(2, B, Ho, Wo, Cout, device="cuda", dtype=torch.float16))
@@ -63,7 +61,7 @@ for persist, cg, bn, phalo in configs:          # configs outermost: a trapping 
                 c = smp.stop()
                 clk = f"  sustained {e0.elapsed_time(e1) / n * 1e3:8.1f} us @ {c['sm_mhz']} MHz {c.get('power_w')} W {c['reasons']}"
             fl = 2.0 * B * Ho * Wo * Cin * Cout * 9
-            print(f"{name:34s} persist={persist} cg={cg} bn={layer.bn_tile:3d} halo={phalo}  {ms*1e3:8.1f} us  {3*fl/ms/1e9:7.1f} TF/s(x3)  max|err|={err:.2e}  planes={hl:.1e}{clk}", flush=True)
+            print(f"{name:34s} bn={layer.bn_tile:3d}  {ms*1e3:8.1f} us  {3*fl/ms/1e9:7.1f} TF/s(x3)  max|err|={err:.2e}  planes={hl:.1e}{clk}", flush=True)
         except Exception as ex:
-            print(f"{name:34s} persist={persist} cg={cg} bn={layer.bn_tile:3d} halo={phalo}  FAILED: {ex}", flush=True)
+            print(f"{name:34s} bn={layer.bn_tile:3d}  FAILED: {ex}", flush=True)
             raise SystemExit(1)

@@ -19,9 +19,7 @@ for si in sel:
     x = E.Act(torch.randn(B, H, W, Cin, generator=g).cuda(), 0, None, torch.zeros(2, B, H, W, Cin, device="cuda", dtype=torch.float16))
     E.split_lo(x)
     out = E.Act(torch.zeros(B, H, W, Cout, device="cuda"), 0, None, torch.zeros(2, B, H, W, Cout, device="cuda", dtype=torch.float16))
-    for cfg in os.environ.get("TRACE_CFGS", "0:0,1:128,2:128").split(","):
-        cg, bn = (int(v) for v in cfg.split(":"))
-        os.environ["VD3D_TC_CG"] = str(cg)
+    for bn in (int(v) for v in os.environ.get("TRACE_BNS", "0,128").split(",")):
         layer.bn_tile = bn
         layer(x, out); torch.cuda.synchronize()
         tr = torch.zeros(12, N, dtype=torch.int64, device="cuda")
@@ -35,7 +33,7 @@ for si in sel:
         nkb = int((t[3] > 0).sum())
         first = t[3, :nkb:KB]                                        # first MMAs of each tile
         if len(first) > 2:
-            print(f"{name:30s} cg={cg} bn={bn:3d} tile period (first MMA to first MMA) {np.median(np.diff(first)):7.0f} clk", flush=True)
+            print(f"{name:30s} bn={bn:3d} tile period (first MMA to first MMA) {np.median(np.diff(first)):7.0f} clk", flush=True)
         nt = int((t[5] > 0).sum())
         if nt > 2 and (t[7, :nt] > 0).all():                        # (tiles of <= 64 columns run the epilogue on the consumers: no hand-off)
             ti = np.arange(nt - 1)
@@ -43,7 +41,7 @@ for si in sel:
             nxt = t[3, np.minimum((ti + 1) * KB, N - 1)]
             ok = (ti + 1) * KB < nkb
             med = lambda v: np.median(v[ok]) if ok.any() else float("nan")
-            print(f"{name:30s} cg={cg} bn={bn:3d} tiles={nt} k-blocks/tile={KB}  tile period {np.median(np.diff(t[5, :nt])):7.0f}  "
+            print(f"{name:30s} bn={bn:3d} tiles={nt} k-blocks/tile={KB}  tile period {np.median(np.diff(t[5, :nt])):7.0f}  "
                   f"last MMA -> staged {med(staged - last):6.0f}  staged -> epilogue start {med(estart - staged):6.0f}  "
                   f"stage held {med(erel - estart):6.0f}  epilogue {med(edone - estart):6.0f}  "
                   f"last MMA -> next tile's first MMA {med(nxt - last):6.0f} clk", flush=True)
@@ -61,7 +59,7 @@ for si in sel:
                 print(f"   tile {i:3d}: slots {sl}  longest stage wait {w.max():7.0f} clk at k-block {int(w.argmax()):3d}  "
                       f"held slot passed over {int(t[10, i])}x", flush=True)
         if late:
-            print(f"{name:30s} cg={cg} bn={bn:3d} longest stage wait after a tile's second k-block: median over tiles {np.median(late):7.0f}, "
+            print(f"{name:30s} bn={bn:3d} longest stage wait after a tile's second k-block: median over tiles {np.median(late):7.0f}, "
                   f"max {np.max(late):7.0f} clk; held slot passed over {int(t[10, :nt].sum())}x in {nt} tiles", flush=True)
         n = int((t[0] > 0).sum())
         t = t[:, :n]
@@ -71,7 +69,7 @@ for si in sel:
         issue = t[4] - t[3]                # 12 MMAs + look-ahead (wait, fence, descriptors) + commit
         per = np.diff(t[4])
         sl = slice(20, min(n, 400))
-        print(f"{name:30s} cg={cg} bn={bn:3d} n={n}  period {np.median(per[sl]):7.0f}  free->mma-start {np.median(lat[sl]):7.0f}  "
+        print(f"{name:30s} bn={bn:3d} n={n}  period {np.median(per[sl]):7.0f}  free->mma-start {np.median(lat[sl]):7.0f}  "
               f"issue-loads {np.median((t[1]-t[0])[sl]):5.0f}  half-issue {np.median(wait[sl]):7.0f}  mma-issue {np.median(issue[sl]):6.0f} clk", flush=True)
         k = 40
         print("   k-block:", " ".join(f"{int(v):6d}" for v in range(k, k + 8)))

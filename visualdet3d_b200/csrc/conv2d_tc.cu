@@ -568,40 +568,45 @@ static int fit_bn(int bn) {
     return bn;
 }
 
-// levels of a multi-level launch (vd3d_conv2d_tc16_levels): activation pointers and sizes per level, output / residual pixel offsets
-struct LevelSpec {
-    int L;
-    const void* in_hi[TC_MAX_LEVELS]; const void* in_lo[TC_MAX_LEVELS];
+// One conv as the entries describe it: L input tensors of one channel layout (L > 1: a multi-level launch, fp16 operands only), the weights
+// and the epilogue.  Level l reads in[l] / in_lo[l] [B][H[l]][W[l]]; its outputs and fp32 residual lie out_off[l] / res_off[l] pixels after
+// level 0's (L > 1); res_W[l] > 0: its fp32 residual is [B][res_H[l]][res_W[l]] at half the output size, read nearest-upsampled.
+struct ConvSpec {
+    int f16, L, B, Cin, in_cs, in_co;
+    const void* in[TC_MAX_LEVELS]; const void* in_lo[TC_MAX_LEVELS];
     int H[TC_MAX_LEVELS], W[TC_MAX_LEVELS], res_H[TC_MAX_LEVELS], res_W[TC_MAX_LEVELS];
     long long out_off[TC_MAX_LEVELS], res_off[TC_MAX_LEVELS];
+    const void* w_hi; const void* w_lo; float out_scale; const float* bias;
+    int KH, KW, pad, dil, stride;
+    const float* res; const void* res_h16_hi; const void* res_h16_lo; int res_cs, res_co;
+    float* out; float* out_lo; void* out_h16_hi; void* out_h16_lo;
+    int Cout, out_cs, out_co, relu, passes, bn;
 };
 
-static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                            const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil, int stride,
-                            const float* res, int res_cs, int res_co, float* out, float* out_lo, void* out_h16_hi, void* out_h16_lo,
-                            int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream,
-                            const void* res_h16_hi = nullptr, const void* res_h16_lo = nullptr, int res_up_H = 0, int res_up_W = 0,
-                            const LevelSpec* ls = nullptr) {
-    VD3D_REQUIRE(in && w_hi && (out || out_h16_hi), "conv2d_tc: null pointer");
-    VD3D_REQUIRE(!(res && res_h16_hi) && (!res_h16_hi == !res_h16_lo), "conv2d_tc: the residual is either an fp32 tensor or an fp16 (hi, lo) plane pair");
+static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
+    const int f16 = s.f16, B = s.B, H = s.H[0], W = s.W[0], Cin = s.Cin, KH = s.KH, KW = s.KW, pad = s.pad, dil = s.dil, stride = s.stride;
+    const int Cout = s.Cout, out_cs = s.out_cs, out_co = s.out_co, res_cs = s.res_cs, res_co = s.res_co;
+    VD3D_REQUIRE(s.in[0] && s.w_hi && (s.out || s.out_h16_hi), "conv2d_tc: null pointer");
+    VD3D_REQUIRE(!(s.res && s.res_h16_hi) && (!s.res_h16_hi == !s.res_h16_lo), "conv2d_tc: the residual is either an fp32 tensor or an fp16 (hi, lo) plane pair");
+    int passes = s.passes;
     const int two_pass = (f16 && passes == 2) ? 1 : 0;        // error-budget experiments: 3-pass machinery with the A_lo * W_hi product dropped
     if (two_pass) passes = 3;
     VD3D_REQUIRE(passes == 1 || passes == 3, "conv2d_tc: passes must be 1, 3 (or 2 with the fp16-split engine)");
-    VD3D_REQUIRE(passes == 1 || (in_lo && w_lo), "conv2d_tc: 3-pass mode needs the lo tensors");
+    VD3D_REQUIRE(passes == 1 || (s.in_lo[0] && s.w_lo), "conv2d_tc: 3-pass mode needs the lo tensors");
+    VD3D_REQUIRE(!(two_pass && s.res_h16_hi), "conv2d_tc: the 2-pass experiment takes an fp32 residual only");
     const int esize = f16 ? 2 : 4, bk = 128 / esize;
     VD3D_REQUIRE(f16 ? (Cin % 8 == 0) : (Cin % bk == 0), "conv2d_tc: Cin must be a multiple of %d (got %d)", f16 ? 8 : bk, Cin);
-    VD3D_REQUIRE(in_cs % 8 == 0 && in_co % 8 == 0 && out_cs % 4 == 0 && out_co % 4 == 0 && Cout % 4 == 0, "conv2d_tc: pitches/offsets alignment");
-    VD3D_REQUIRE(!(res || res_h16_hi) || (res_cs % 4 == 0 && res_co % 4 == 0), "conv2d_tc: residual pitch/offset must be multiples of 4");
-    VD3D_REQUIRE(((uintptr_t)in & 15) == 0 && ((uintptr_t)w_hi & 15) == 0 && ((uintptr_t)out & 15) == 0, "conv2d_tc: pointers must be 16-byte aligned");
-    VD3D_REQUIRE(!res_h16_hi || ((((uintptr_t)res_h16_hi | (uintptr_t)res_h16_lo) & 7) == 0), "conv2d_tc: residual planes must be 8-byte aligned");
-    VD3D_REQUIRE(!out_h16_hi || (out_h16_lo && out_cs % 4 == 0), "conv2d_tc: fp16 output planes come in (hi, lo) pairs");
-    int BN = bn;
+    VD3D_REQUIRE(s.in_cs % 8 == 0 && s.in_co % 8 == 0 && out_cs % 4 == 0 && out_co % 4 == 0 && Cout % 4 == 0, "conv2d_tc: pitches/offsets alignment");
+    VD3D_REQUIRE(!(s.res || s.res_h16_hi) || (res_cs % 4 == 0 && res_co % 4 == 0), "conv2d_tc: residual pitch/offset must be multiples of 4");
+    VD3D_REQUIRE(((uintptr_t)s.in[0] & 15) == 0 && ((uintptr_t)s.w_hi & 15) == 0 && ((uintptr_t)s.out & 15) == 0, "conv2d_tc: pointers must be 16-byte aligned");
+    VD3D_REQUIRE(!s.res_h16_hi || ((((uintptr_t)s.res_h16_hi | (uintptr_t)s.res_h16_lo) & 7) == 0), "conv2d_tc: residual planes must be 8-byte aligned");
+    VD3D_REQUIRE(!s.out_h16_hi || (s.out_h16_lo && out_cs % 4 == 0), "conv2d_tc: fp16 output planes come in (hi, lo) pairs");
+    int BN = s.bn;
     if (BN <= 0) {
         if (f16 && passes == 3) {
             int mt_all = 0;
-            for (int l = 0; l < (ls ? ls->L : 1); ++l) {
-                const int h = ls ? ls->H[l] : H, w = ls ? ls->W[l] : W;
-                const int Ho_ = (h + 2 * pad - dil * (KH - 1) - 1) / stride + 1, Wo_ = (w + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+            for (int l = 0; l < s.L; ++l) {
+                const int Ho_ = (s.H[l] + 2 * pad - dil * (KH - 1) - 1) / stride + 1, Wo_ = (s.W[l] + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
                 mt_all += cdiv(Wo_, TC_TW) * cdiv(Ho_, TC_TH) * B;
             }
             BN = pick_bn_cost(Cout, mt_all);
@@ -615,28 +620,28 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.KH = KH; p.KW = KW; p.pad = pad; p.dil = dil; p.stride = stride;
     p.Ho = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1; p.Wo = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
     VD3D_REQUIRE(p.Ho > 0 && p.Wo > 0, "conv2d_tc: empty output");
-    p.Cout = Cout; p.BN = BN; p.passes = passes; p.f16 = f16; p.bk = bk; p.cin_pad = (Cin + bk - 1) / bk * bk; p.out_scale = out_scale;
+    p.Cout = Cout; p.BN = BN; p.passes = passes; p.f16 = f16; p.bk = bk; p.cin_pad = (Cin + bk - 1) / bk * bk; p.out_scale = s.out_scale;
     p.tiles_w = cdiv(p.Wo, TC_TW); p.tiles_h = cdiv(p.Ho, TC_TH);
     p.stride_w = stride; p.pad_w = pad;
     p.cout_pad = (Cout + 15) / 16 * 16;
     p.m_tiles = p.tiles_w * p.tiles_h * B; p.n_tiles = cdiv(p.cout_pad, BN);
     p.rowb = 128;
-    if (ls) {
+    if (s.L > 1) {
         // concatenated M tiles of the levels (tile_geom); the level's own maps give each its zero padding
-        VD3D_REQUIRE(ls->L >= 1 && ls->L <= TC_MAX_LEVELS && f16 && passes == 3 && !res_h16_hi && res_up_W == 0, "conv2d_tc16_levels: bad level set");
-        p.n_levels = ls->L;
+        VD3D_REQUIRE(s.L <= TC_MAX_LEVELS && f16 && s.passes == 3 && !s.res_h16_hi, "conv2d_tc16: bad level set");
+        p.n_levels = s.L;
         int mt = 0;
-        for (int l = 0; l < ls->L; ++l) {
+        for (int l = 0; l < s.L; ++l) {
             TcLevel& v = p.lv[l];
-            v.Ho = (ls->H[l] + 2 * pad - dil * (KH - 1) - 1) / stride + 1; v.Wo = (ls->W[l] + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
-            VD3D_REQUIRE(v.Ho > 0 && v.Wo > 0, "conv2d_tc16_levels: level %d has an empty output", l);
+            v.Ho = (s.H[l] + 2 * pad - dil * (KH - 1) - 1) / stride + 1; v.Wo = (s.W[l] + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+            VD3D_REQUIRE(v.Ho > 0 && v.Wo > 0, "conv2d_tc16: level %d has an empty output", l);
             v.tiles_w = cdiv(v.Wo, TC_TW); v.tiles_h = cdiv(v.Ho, TC_TH);
             v.m_begin = mt;
             mt += v.tiles_w * v.tiles_h * B;
-            v.pix_off = ls->out_off[l]; v.res_off = ls->res_off[l];
-            v.res_H = ls->res_H[l]; v.res_W = ls->res_W[l];
-            VD3D_REQUIRE(v.res_W == 0 || (res && v.Ho == 2 * v.res_H && v.Wo == 2 * v.res_W),
-                         "conv2d_tc16_levels: level %d: an upsampled residual needs exactly half the output size", l);
+            v.pix_off = s.out_off[l]; v.res_off = s.res_off[l];
+            v.res_H = s.res_H[l]; v.res_W = s.res_W[l];
+            VD3D_REQUIRE(v.res_W == 0 || (s.res && v.Ho == 2 * v.res_H && v.Wo == 2 * v.res_W),
+                         "conv2d_tc16: level %d: an upsampled residual needs exactly half the output size", l);
         }
         p.m_tiles = mt;
     }
@@ -657,20 +662,21 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
             }
         }
     }
-    p.v8 = (out_cs % 8 == 0 && out_co % 8 == 0 && ((uintptr_t)out & 31) == 0 && (!bias || ((uintptr_t)bias & 31) == 0) &&
-            (!res || (res_cs % 8 == 0 && res_co % 8 == 0 && ((uintptr_t)res & 31) == 0)) &&
-            (!res_h16_hi || (res_cs % 8 == 0 && res_co % 8 == 0 && ((((uintptr_t)res_h16_hi | (uintptr_t)res_h16_lo) & 15) == 0))) &&
-            (!out_h16_hi || ((((uintptr_t)out_h16_hi | (uintptr_t)out_h16_lo) & 15) == 0))) ? 1 : 0;
-    p.out_cs = out_cs; p.out_co = out_co; p.res_cs = res_cs; p.res_co = res_co; p.relu = relu;
-    p.bias = bias; p.res = res; p.out = out; p.out_lo = out_lo; p.out_h16_hi = out_h16_hi; p.out_h16_lo = out_h16_lo;
-    p.res_h16_hi = res_h16_hi; p.res_h16_lo = res_h16_lo;
-    if (res_up_W > 0) {
-        VD3D_REQUIRE(res && !res_h16_hi && p.Ho == 2 * res_up_H && p.Wo == 2 * res_up_W,
+    p.v8 = (out_cs % 8 == 0 && out_co % 8 == 0 && ((uintptr_t)s.out & 31) == 0 && (!s.bias || ((uintptr_t)s.bias & 31) == 0) &&
+            (!s.res || (res_cs % 8 == 0 && res_co % 8 == 0 && ((uintptr_t)s.res & 31) == 0)) &&
+            (!s.res_h16_hi || (res_cs % 8 == 0 && res_co % 8 == 0 && ((((uintptr_t)s.res_h16_hi | (uintptr_t)s.res_h16_lo) & 15) == 0))) &&
+            (!s.out_h16_hi || ((((uintptr_t)s.out_h16_hi | (uintptr_t)s.out_h16_lo) & 15) == 0))) ? 1 : 0;
+    p.out_cs = out_cs; p.out_co = out_co; p.res_cs = res_cs; p.res_co = res_co; p.relu = s.relu;
+    p.bias = s.bias; p.res = s.res; p.out = s.out; p.out_lo = s.out_lo; p.out_h16_hi = s.out_h16_hi; p.out_h16_lo = s.out_h16_lo;
+    p.res_h16_hi = s.res_h16_hi; p.res_h16_lo = s.res_h16_lo;
+    if (s.L == 1 && s.res_W[0] > 0) {
+        const int res_up_H = s.res_H[0], res_up_W = s.res_W[0];
+        VD3D_REQUIRE(s.res && !s.res_h16_hi && p.Ho == 2 * res_up_H && p.Wo == 2 * res_up_W,
                      "conv2d_tc: an upsampled residual is an fp32 tensor of exactly half the output size (%dx%d vs %dx%d)", res_up_H, res_up_W, p.Ho, p.Wo);
         p.res_up_H = res_up_H; p.res_up_W = res_up_W;
     }
     p.two_pass = two_pass;
-    p.range_flag = out_h16_hi ? fp16_range_flag() : nullptr;
+    p.range_flag = s.out_h16_hi ? fp16_range_flag() : nullptr;
     {
         const char* e = getenv("VD3D_TC_CHUNK");
         p.chunk = e ? atoi(e) : 4;
@@ -681,21 +687,21 @@ static int conv2d_tc_launch(int f16, const void* in, const void* in_lo, int B, i
         // MMA-mode timing experiments (VD3D_TC_DEBUG bits 0 and 1), which only conv2d_tcp_kernel implements.
         const char* e = getenv("VD3D_ROW64");
         const char* d = getenv("VD3D_TC_DEBUG");
-        if (!ls && conv2d_row64_eligible(p) && !(e && atoi(e) == 0) && !(d && (atoi(d) & 3)))
-            return conv2d_row64_launch(p, in, in_lo, in_cs, in_co, w_hi, w_lo, stream);
+        if (s.L == 1 && conv2d_row64_eligible(p) && !(e && atoi(e) == 0) && !(d && (atoi(d) & 3)))
+            return conv2d_row64_launch(p, s.in[0], s.in_lo[0], s.in_cs, s.in_co, s.w_hi, s.w_lo, stream);
     }
     const int K = KH * KW * p.cin_pad;
     CUtensorMap mA, mAlo, mWhi, mWlo;
     int rc;
-    if ((rc = make_map_act(&mA, in, B, H, W, Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
-    if ((rc = make_map_act(&mAlo, in_lo ? in_lo : in, B, H, W, Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
-    if ((rc = make_map_wgt(&mWhi, w_hi, Cout, K, BN, esize))) return rc;
-    if ((rc = make_map_wgt(&mWlo, w_lo ? w_lo : w_hi, Cout, K, BN, esize))) return rc;
-    if (!ls) return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
+    if ((rc = make_map_act(&mA, s.in[0], B, H, W, Cin, s.in_cs, s.in_co, esize, TC_TW, TC_TH, stride))) return rc;
+    if ((rc = make_map_act(&mAlo, s.in_lo[0] ? s.in_lo[0] : s.in[0], B, H, W, Cin, s.in_cs, s.in_co, esize, TC_TW, TC_TH, stride))) return rc;
+    if ((rc = make_map_wgt(&mWhi, s.w_hi, Cout, K, BN, esize))) return rc;
+    if ((rc = make_map_wgt(&mWlo, s.w_lo ? s.w_lo : s.w_hi, Cout, K, BN, esize))) return rc;
+    if (s.L == 1) return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
     TcLevelMaps lm;
-    for (int l = 0; l < ls->L; ++l) {
-        if ((rc = make_map_act(&lm.a[l], ls->in_hi[l], B, ls->H[l], ls->W[l], Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
-        if ((rc = make_map_act(&lm.alo[l], ls->in_lo[l], B, ls->H[l], ls->W[l], Cin, in_cs, in_co, esize, TC_TW, TC_TH, stride))) return rc;
+    for (int l = 0; l < s.L; ++l) {
+        if ((rc = make_map_act(&lm.a[l], s.in[l], B, s.H[l], s.W[l], Cin, s.in_cs, s.in_co, esize, TC_TW, TC_TH, stride))) return rc;
+        if ((rc = make_map_act(&lm.alo[l], s.in_lo[l], B, s.H[l], s.W[l], Cin, s.in_cs, s.in_co, esize, TC_TW, TC_TH, stride))) return rc;
     }
     return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream, &lm);
 }
@@ -706,75 +712,58 @@ static long long level_pix_off(const void* base0, const void* base, int esize, i
     return d % ((long long)esize * cs) ? (-1LL << 62) : d / ((long long)esize * cs);
 }
 
-extern "C" int vd3d_conv2d_tc16_levels(int L, const void* const* in_hi, const void* const* in_lo, const int* H, const int* W, int B, int Cin, int in_cs,
-                                       int in_co, const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad,
-                                       int dil, int stride, const void* const* res, const int* res_H, const int* res_W, int res_cs, int res_co,
-                                       const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
-                                       int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
-    VD3D_REQUIRE(L >= 1 && L <= TC_MAX_LEVELS && in_hi && in_lo && H && W && (out || out_hi16) && (!out_hi16 == !out_lo16),
-                 "conv2d_tc16_levels: 1..%d levels, inputs, sizes and an output are required", TC_MAX_LEVELS);
-    LevelSpec ls;
-    memset(&ls, 0, sizeof(ls));
-    ls.L = L;
+extern "C" int vd3d_conv2d_tc(const float* in, const float* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                              const float* w_hi, const float* w_lo, const float* bias, int KH, int KW, int pad, int dil,
+                              const float* res, int res_cs, int res_co,
+                              float* out, float* out_lo, int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream) {
+    ConvSpec s;
+    memset(&s, 0, sizeof(s));
+    s.f16 = 0; s.L = 1; s.B = B; s.Cin = Cin; s.in_cs = in_cs; s.in_co = in_co;
+    s.in[0] = in; s.in_lo[0] = in_lo; s.H[0] = H; s.W[0] = W;
+    s.w_hi = w_hi; s.w_lo = w_lo; s.out_scale = 1.0f; s.bias = bias;
+    s.KH = KH; s.KW = KW; s.pad = pad; s.dil = dil; s.stride = 1;
+    s.res = res; s.res_cs = res_cs; s.res_co = res_co;
+    s.out = out; s.out_lo = out_lo;
+    s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = passes; s.bn = bn;
+    return conv2d_tc_launch(s, stream);
+}
+
+extern "C" int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* const* in_lo, const int* H, const int* W, int B, int Cin, int in_cs,
+                                int in_co, const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad,
+                                int dil, int stride, const void* const* res, const void* const* res_hi16, const void* const* res_lo16,
+                                const int* res_H, const int* res_W, int res_cs, int res_co,
+                                const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
+                                int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream) {
+    VD3D_REQUIRE(L >= 1 && L <= TC_MAX_LEVELS && in_hi && in_lo && H && W && (out || out_hi16) && (!out_hi16 == !out_lo16) &&
+                 (!res_hi16 == !res_lo16), "conv2d_tc16: 1..%d levels, inputs, sizes and an output are required", TC_MAX_LEVELS);
+    ConvSpec s;
+    memset(&s, 0, sizeof(s));
+    s.f16 = 1; s.L = L; s.B = B; s.Cin = Cin; s.in_cs = in_cs; s.in_co = in_co;
     for (int l = 0; l < L; ++l) {
         VD3D_REQUIRE(in_hi[l] && in_lo[l] && H[l] > 0 && W[l] > 0 && ((((uintptr_t)in_hi[l] | (uintptr_t)in_lo[l]) & 15) == 0),
-                     "conv2d_tc16_levels: level %d: 16-byte aligned input planes and a non-empty size are required", l);
-        ls.in_hi[l] = in_hi[l]; ls.in_lo[l] = in_lo[l]; ls.H[l] = H[l]; ls.W[l] = W[l];
-        ls.res_H[l] = res_H ? res_H[l] : 0; ls.res_W[l] = res_W ? res_W[l] : 0;
+                     "conv2d_tc16: level %d: 16-byte aligned input planes and a non-empty size are required", l);
+        s.in[l] = in_hi[l]; s.in_lo[l] = in_lo[l]; s.H[l] = H[l]; s.W[l] = W[l];
+        s.res_H[l] = res_H ? res_H[l] : 0; s.res_W[l] = res_W ? res_W[l] : 0;
         // every output form of level l sits at the same pixel offset from level 0's (one allocation per form, levels concatenated)
         const long long o32 = out ? level_pix_off(out[0], out[l], 4, out_cs) : 0;
         const long long oh = out_hi16 ? level_pix_off(out_hi16[0], out_hi16[l], 2, out_cs) : o32;
         const long long ol = out_lo16 ? level_pix_off(out_lo16[0], out_lo16[l], 2, out_cs) : o32;
         VD3D_REQUIRE(o32 == oh && oh == ol && (out ? out[l] != nullptr : true) && o32 > (-1LL << 62),
-                     "conv2d_tc16_levels: level %d: the output forms must lie at one common pixel offset from level 0's", l);
-        ls.out_off[l] = out ? o32 : oh;
-        ls.res_off[l] = 0;
+                     "conv2d_tc16: level %d: the output forms must lie at one common pixel offset from level 0's", l);
+        s.out_off[l] = out ? o32 : oh;
+        VD3D_REQUIRE((!res || res[l]) && (!res_hi16 || (res_hi16[l] && res_lo16[l])), "conv2d_tc16: level %d has no residual", l);
         if (res) {
-            VD3D_REQUIRE(res[l], "conv2d_tc16_levels: level %d has no residual", l);
-            ls.res_off[l] = level_pix_off(res[0], res[l], 4, res_cs);
-            VD3D_REQUIRE(ls.res_off[l] > (-1LL << 62), "conv2d_tc16_levels: level %d: residual not at a whole-pixel offset from level 0's", l);
+            s.res_off[l] = level_pix_off(res[0], res[l], 4, res_cs);
+            VD3D_REQUIRE(s.res_off[l] > (-1LL << 62), "conv2d_tc16: level %d: residual not at a whole-pixel offset from level 0's", l);
         }
     }
-    return conv2d_tc_launch(1, in_hi[0], in_lo[0], B, H[0], W[0], Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride,
-                            res ? (const float*)res[0] : nullptr, res_cs, res_co, out ? (float*)out[0] : nullptr, nullptr,
-                            out_hi16 ? (void*)out_hi16[0] : nullptr, out_lo16 ? (void*)out_lo16[0] : nullptr, Cout, out_cs, out_co, relu, 3, bn, stream,
-                            nullptr, nullptr, 0, 0, &ls);
-}
-
-extern "C" int vd3d_conv2d_tc(const float* in, const float* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                              const float* w_hi, const float* w_lo, const float* bias, int KH, int KW, int pad, int dil,
-                              const float* res, int res_cs, int res_co,
-                              float* out, float* out_lo, int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream) {
-    return conv2d_tc_launch(0, in, in_lo, B, H, W, Cin, in_cs, in_co, w_hi, w_lo, 1.0f, bias, KH, KW, pad, dil, 1, res, res_cs, res_co,
-                            out, out_lo, nullptr, nullptr, Cout, out_cs, out_co, relu, passes, bn, stream);
-}
-
-extern "C" int vd3d_conv2d_tc16(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                                const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
-                                int stride, const float* res, int res_cs, int res_co,
-                                float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int passes, int bn,
-                                void* stream) {
-    return conv2d_tc_launch(1, in_hi, in_lo, B, H, W, Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride, res, res_cs, res_co,
-                            out, nullptr, out_hi16, out_lo16, Cout, out_cs, out_co, relu, passes, bn, stream);
-}
-
-extern "C" int vd3d_conv2d_tc16_planes(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                                       const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
-                                       int stride, const float* res, const void* res_hi16, const void* res_lo16, int res_cs, int res_co,
-                                       float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
-    return conv2d_tc_launch(1, in_hi, in_lo, B, H, W, Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride, res, res_cs, res_co,
-                            out, nullptr, out_hi16, out_lo16, Cout, out_cs, out_co, relu, 3, bn, stream, res_hi16, res_lo16);
-}
-
-// FPN lateral conv with the top-down add fused (R/detectors/retinanet_2d.py:49-52): out = conv(in) + nearest_up2(res), the residual being
-// [B][Ho / 2][Wo / 2] (res_H, res_W); everything else as vd3d_conv2d_tc16 (3 passes, library tile policy when bn <= 0)
-extern "C" int vd3d_conv2d_tc16_res_up2(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
-                                        const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
-                                        int stride, const float* res, int res_cs, int res_co, int res_H, int res_W,
-                                        float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
-    VD3D_REQUIRE(res && res_H > 0 && res_W > 0, "conv2d_tc16_res_up2: needs the half-resolution residual");
-    return conv2d_tc_launch(1, in_hi, in_lo, B, H, W, Cin, in_cs, in_co, w_hi, w_lo, out_scale, bias, KH, KW, pad, dil, stride, res, res_cs, res_co,
-                            out, nullptr, out_hi16, out_lo16, Cout, out_cs, out_co, relu, 3, bn, stream, nullptr, nullptr, res_H, res_W);
+    s.w_hi = w_hi; s.w_lo = w_lo; s.out_scale = out_scale; s.bias = bias;
+    s.KH = KH; s.KW = KW; s.pad = pad; s.dil = dil; s.stride = stride;
+    s.res = res ? (const float*)res[0] : nullptr; s.res_cs = res_cs; s.res_co = res_co;
+    s.res_h16_hi = res_hi16 ? res_hi16[0] : nullptr; s.res_h16_lo = res_lo16 ? res_lo16[0] : nullptr;
+    s.out = out ? (float*)out[0] : nullptr; s.out_h16_hi = out_hi16 ? (void*)out_hi16[0] : nullptr; s.out_h16_lo = out_lo16 ? (void*)out_lo16[0] : nullptr;
+    s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = passes; s.bn = bn;
+    return conv2d_tc_launch(s, stream);
 }
 
 // ----------------------------------------------------------------------------------------------------------------

@@ -50,7 +50,7 @@ struct TcParams {
     const float* bias; const float* res; float* out; float* out_lo;
     const void* res_h16_hi; const void* res_h16_lo;   // residual given as fp16 (hi, lo) planes (value = hi + lo) instead of an fp32 tensor (`res`)
     int res_up_H, res_up_W;  // > 0: the residual is [B][res_up_H][res_up_W] at half the output resolution, read nearest-upsampled (tcp_res_pix)
-    // Multi-level launch (vd3d_conv2d_tc16_levels; n_levels = 0: one tensor).  The M tiles of the levels are concatenated: level l owns tiles
+    // Multi-level launch (vd3d_conv2d_tc16 with L > 1; n_levels = 0: one tensor).  The M tiles of the levels are concatenated: level l owns tiles
     // [m_begin, m_begin + B * tiles_h * tiles_w) and reads its own activation maps; its output (residual) pixel p sits at pixel pix_off + p
     // (res_off + p, or of the [B][res_H][res_W] half-resolution residual when res_W > 0) of the `out` (`res`) pointers.
     int n_levels;

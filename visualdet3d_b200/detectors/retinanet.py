@@ -6,9 +6,9 @@ stream-ordered one (graphs.GraphedStep, pipeline.StreamedInference).
 
   ResNet (out_indices (1, 2, 3): C3 / C4 / C5)
   -> FPN: lateral 1x1 convs, the top-down `lat[i-1] += nearest_up2(lat[i])` fused into the lateral conv's residual read
-     (vd3d_conv2d_tc16_res_up2), 3x3 fpn convs, P6 = 3x3/2 on C5, P7 = 3x3/2 on P6, no ReLU
+     (ConvLayer(res_up=True)), 3x3 fpn convs, P6 = 3x3/2 on C5, P7 = 3x3/2 on P6, no ReLU
   -> head: the same cls / reg towers (stacked 3x3 conv + ReLU) and output convs on every level, each layer one persistent launch over all
-     levels and the whole batch (vd3d_conv2d_tc16_levels); the cls output conv is padded to a multiple of 16 zero-weight columns so that it
+     levels and the whole batch (ConvLayer.run_levels); the cls output conv is padded to a multiple of 16 zero-weight columns so that it
      runs on the tensor cores (the decode reads it with that channel pitch)
   -> device decode (vd3d_retina_decode): max-sigmoid score, top-k, _decode, class-agnostic NMS, post-NMS score threshold.
 """

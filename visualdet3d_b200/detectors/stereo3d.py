@@ -69,8 +69,7 @@ class ResNetRunner:
         Hs, Ws = self.stem.out_hw(H, W)
         Hp, Wp = (Hs + 2 - 3) // 2 + 1, (Ws + 2 - 3) // 2 + 1
         import os
-        fuse_pool = (self.stem_tc is not None and -1 not in self.p.out_indices and os.environ.get("VD3D_STEM_POOL", "1") != "0"
-                     and os.environ.get("VD3D_TC_PERSIST", "1") != "0" and os.environ.get("VD3D_TC_CG", "0") != "2")
+        fuse_pool = self.stem_tc is not None and -1 not in self.p.out_indices and os.environ.get("VD3D_STEM_POOL", "1") != "0"
         x = None
         if fuse_pool:
             # stem conv + BN + ReLU + max-pool in ONE kernel (the 64-channel half-resolution stem output never reaches HBM)

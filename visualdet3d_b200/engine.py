@@ -95,10 +95,10 @@ def need_f32(x: "Act", what: str):
 
 
 def planes_mode_ok() -> bool:
-    """Planes-only activations between tensor-core convs (`vd3d_conv2d_tc16_planes`): default on with the persistent fp16-split engine;
+    """Planes-only activations between tensor-core convs (`vd3d_conv2d_tc16` with no fp32 output): default on with the fp16-split engine;
     VD3D_PLANES=0 restores the round-1 behaviour (every conv also writes the fp32 tensor)."""
     import os
-    return conv_engine_default() == "tc16" and os.environ.get("VD3D_TC_PERSIST", "1") != "0" and os.environ.get("VD3D_PLANES", "1") != "0"
+    return conv_engine_default() == "tc16" and os.environ.get("VD3D_PLANES", "1") != "0"
 
 
 def planes_only_ok(layer) -> bool:
@@ -190,6 +190,16 @@ def fp16_split(w: torch.Tensor):
     return hi.contiguous(), lo.contiguous()
 
 
+def fp16_split_scaled(w: torch.Tensor):
+    """Packed float64 weight matrix -> (w_hi, w_lo, out_scale): w * S split by `fp16_split`, S = 2^k the power of two that puts max |w| * S in
+    [8192, 16384) (k clamped to [-24, 24]; 0 for an all-zero matrix) so that the lo parts stay normal fp16 numbers; out_scale = 1 / S (exact)."""
+    wmax = float(w.abs().max())
+    k = int(np.floor(np.log2(16384.0 / wmax))) if wmax > 0 else 0
+    k = max(-24, min(24, k))
+    hi, lo = fp16_split(w * (2.0 ** k))
+    return hi, lo, float(2.0 ** (-k))
+
+
 def tf32_split(w: torch.Tensor):
     """w (float32) -> (hi, lo) with hi = w & 0xFFFFE000 (the bits the tf32 MMA reads) and lo = tf32-truncated (w - hi)."""
     wi = w.contiguous().view(torch.int32)
@@ -232,11 +242,7 @@ class ConvLayer:
             cin64 = (cin_p + 63) // 64 * 64
             wk = torch.zeros(Cout, KH * KW, cin64, dtype=torch.float64)
             wk[:, :, :cin_p] = w.permute(0, 2, 3, 1).reshape(Cout, KH * KW, cin_p)
-            wmax = float(wk.abs().max())
-            k = int(np.floor(np.log2(16384.0 / wmax))) if wmax > 0 else 0      # power-of-two scale: max |w| * S in [8192, 16384)
-            k = max(-24, min(24, k))
-            self.out_scale = float(2.0 ** (-k))
-            hi, lo = fp16_split(wk.reshape(Cout, KH * KW * cin64) * (2.0 ** k))
+            hi, lo, self.out_scale = fp16_split_scaled(wk.reshape(Cout, KH * KW * cin64))
             self.w_hi, self.w_lo = hi.to(device), lo.to(device)
             self.bn_tile = 0          # 0 = the library's policy for the engine in use (vd3d_tc_pick_bn_persistent / vd3d_tc_pick_bn)
             self.passes = 3           # 2 = error-budget experiments (tools/error_budget.py): drop the A_lo * W_hi product
@@ -259,10 +265,31 @@ class ConvLayer:
         if CHECK_LO:
             check_lo(x)
 
+    def _tc16(self, xs: Sequence[Act], outs: Sequence[Act], res: Optional[Sequence[Act]], res_up: bool, relu: bool, f32_out: bool):
+        """One vd3d_conv2d_tc16 launch: outs[l] = conv(xs[l]) [+ res[l]] for every level l.  The residual is read from its fp32 tensor when that
+        is valid, else from its fp16 planes; res_up: it has half the output size and is added nearest-upsampled.  f32_out=False writes the
+        output planes only."""
+        L = len(xs)
+        P, I = ctypes.c_void_p * L, ctypes.c_int * L        # per-level arrays
+
+        def planes(acts):
+            ps = [a.h16_ptrs for a in acts]
+            return P(*[h for h, _ in ps]), P(*[lo for _, lo in ps])
+        o, r0 = outs[0], res[0] if res is not None else None
+        xh, xl = planes(xs)
+        oh, ol = planes(outs) if o.h16 else (None, None)
+        rh, rl = planes(res) if r0 is not None and not r0.f32 else (None, None)
+        call("vd3d_conv2d_tc16", L, xh, xl, I(*[x.H for x in xs]), I(*[x.W for x in xs]), xs[0].B, self.Cin, xs[0].cs, xs[0].co,
+             self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale, self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride,
+             P(*[r.ptr for r in res]) if r0 is not None and r0.f32 else None, rh, rl,
+             I(*[r.H for r in res]) if res_up else None, I(*[r.W for r in res]) if res_up else None,
+             r0.cs if r0 is not None else 0, r0.co if r0 is not None else 0,
+             P(*[t.ptr for t in outs]) if f32_out else None, oh, ol, self.Cout, o.cs, o.co, 1 if relu else 0, self.passes, self.bn_tile, _stream())
+
     def run_levels(self, xs: Sequence[Act], outs: Sequence[Act], res: Optional[Sequence[Act]] = None, res_up: bool = False):
-        """The conv on several tensors of different sizes in ONE persistent launch (vd3d_conv2d_tc16_levels): outs[l] = conv(xs[l]) [+ res[l],
-        nearest-upsampled when res_up].  Each form of `outs` (fp32, fp16 planes) and `res` must be views of one allocation with the levels
-        concatenated (`Arena.level_acts`).  Bit-identical to calling the layer on every level."""
+        """The conv on several tensors of different sizes in ONE persistent launch (vd3d_conv2d_tc16 over L levels): outs[l] = conv(xs[l])
+        [+ res[l], nearest-upsampled when res_up].  Each form of `outs` (fp32, fp16 planes) and `res` must be views of one allocation with the
+        levels concatenated (`Arena.level_acts`).  Bit-identical to calling the layer on every level."""
         L = len(xs)
         assert 1 <= L == len(outs) and (res is None or len(res) == L)
         for x, o in zip(xs, outs):
@@ -272,18 +299,7 @@ class ConvLayer:
         if res is not None:
             for r in res:
                 need_f32(r, "multi-level conv residual")
-        arr = lambda T, vals: (T * L)(*vals)
-        P = ctypes.c_void_p
-        call("vd3d_conv2d_tc16_levels", L, arr(P, [x.h16_ptrs[0] for x in xs]), arr(P, [x.h16_ptrs[1] for x in xs]),
-             arr(ctypes.c_int, [x.H for x in xs]), arr(ctypes.c_int, [x.W for x in xs]), xs[0].B, self.Cin, xs[0].cs, xs[0].co,
-             self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale, self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride,
-             arr(P, [r.ptr for r in res]) if res is not None else None,
-             arr(ctypes.c_int, [r.H if res_up else 0 for r in res]) if res is not None else None,
-             arr(ctypes.c_int, [r.W if res_up else 0 for r in res]) if res is not None else None,
-             res[0].cs if res is not None else 0, res[0].co if res is not None else 0,
-             arr(P, [o.ptr for o in outs]), arr(P, [o.h16_ptrs[0] for o in outs]) if outs[0].h16 else None,
-             arr(P, [o.h16_ptrs[1] for o in outs]) if outs[0].h16 else None,
-             self.Cout, outs[0].cs, outs[0].co, 1 if self.relu else 0, self.bn_tile, _stream())
+        self._tc16(xs, outs, res, res_up and res is not None, self.relu, True)
         for o in outs:
             o.f32, o.lo_fresh = True, o.h16
         return outs
@@ -303,11 +319,7 @@ class ConvLayer:
             if not out.h16 or res is None:
                 raise _lib.Vd3dError("conv with an upsampled residual: needs a residual and an output with fp16 (hi, lo) planes")
             need_f32(res, "upsampled conv residual")
-            xh, xl = x.h16_ptrs
-            oh, ol = out.h16_ptrs
-            call("vd3d_conv2d_tc16_res_up2", xh, xl, x.B, x.H, x.W, x.C, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale,
-                 self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride, res.ptr, res.cs, res.co, res.H, res.W,
-                 out.ptr, oh, ol, self.Cout, out.cs, out.co, 1 if r else 0, self.bn_tile, _stream())
+            self._tc16([x], [out], [res], True, r, True)
             out.f32, out.lo_fresh = True, True
             return out
         if self.engine != "tc16" or not out.h16 or getattr(self, "passes", 3) != 3:
@@ -327,27 +339,13 @@ class ConvLayer:
                 raise _lib.Vd3dError("fp16-split tensor-core conv: input activation has no fp16 (hi, lo) planes (plan bug: missing split_lo)")
             if CHECK_LO:
                 check_lo(x)
-            xh, xl = x.h16_ptrs
-            oh, ol = out.h16_ptrs
             res_planes = res is not None and not res.f32
             if res_planes and self.passes != 3:
                 raise _lib.Vd3dError("the 2-pass experiment mode needs VD3D_PLANES=0 (fp32 residuals)")
-            if not f32_out or res_planes:
-                if res_planes and not res.h16:
-                    raise _lib.Vd3dError("conv residual: neither an fp32 tensor nor fp16 planes are valid")
-                rh, rl = res.h16_ptrs if res_planes else (None, None)
-                call("vd3d_conv2d_tc16_planes", xh, xl, x.B, x.H, x.W, x.C, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale,
-                     self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride,
-                     res.ptr if (res is not None and not res_planes) else None, rh, rl,
-                     res.cs if res is not None else 0, res.co if res is not None else 0,
-                     out.ptr if f32_out else None, oh, ol, self.Cout, out.cs, out.co, 1 if r else 0, self.bn_tile, _stream())
-                out.lo_fresh = oh is not None
-                return out
-            call("vd3d_conv2d_tc16", xh, xl, x.B, x.H, x.W, x.C, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale,
-                 self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, self.stride,
-                 res.ptr if res is not None else None, res.cs if res is not None else 0, res.co if res is not None else 0,
-                 out.ptr, oh, ol, self.Cout, out.cs, out.co, 1 if r else 0, self.passes, self.bn_tile, _stream())
-            out.lo_fresh = oh is not None
+            if res_planes and not res.h16:
+                raise _lib.Vd3dError("conv residual: neither an fp32 tensor nor fp16 planes are valid")
+            self._tc16([x], [out], [res] if res is not None else None, False, r, f32_out)
+            out.lo_fresh = out.h16
             return out
         passes = 3 if self.engine == "tc" else 1
         if passes == 3 and x.lo_ptr is None:
@@ -375,11 +373,7 @@ class StemLayer:
         self.win = 32 if (KW <= 8 and os.environ.get("VD3D_STEM_WIN", "32") != "64") else 64     # window elements per filter row (8 or 16 pixels x 4)
         wk = torch.zeros(Cout, KH, self.win // 4, 4, dtype=torch.float64)
         wk[:, :, :KW, :Cin] = w.permute(0, 2, 3, 1)
-        wmax = float(wk.abs().max())
-        k = int(np.floor(np.log2(16384.0 / wmax))) if wmax > 0 else 0
-        k = max(-24, min(24, k))
-        self.out_scale = float(2.0 ** (-k))
-        hi, lo = fp16_split(wk.reshape(Cout, KH * self.win) * (2.0 ** k))
+        hi, lo, self.out_scale = fp16_split_scaled(wk.reshape(Cout, KH * self.win))
         self.w_hi, self.w_lo = hi.to(device), lo.to(device)
         self.b = b.float().to(device)
 
@@ -477,11 +471,7 @@ class RowConvLayer:
         self.KS = 2 if KW * pc * 2 <= 64 else 4
         wk = torch.zeros(Cout, KH, self.KS * 16, dtype=torch.float64)
         wk[:, :, :KW * pc].view(Cout, KH, KW, pc)[..., :Cin] = w.permute(0, 2, 3, 1)
-        wmax = float(wk.abs().max())
-        k = int(np.floor(np.log2(16384.0 / wmax))) if wmax > 0 else 0
-        k = max(-24, min(24, k))
-        self.out_scale = float(2.0 ** (-k))
-        hi, lo = fp16_split(wk.reshape(Cout, KH * self.KS * 16) * (2.0 ** k))
+        hi, lo, self.out_scale = fp16_split_scaled(wk.reshape(Cout, KH * self.KS * 16))
         self.w_hi, self.w_lo = hi.to(device), lo.to(device)
         self.b = b.float().to(device)
         self.engine = "tc16"
@@ -593,8 +583,7 @@ class DeformConvLayer:
     def fused_ok(self) -> bool:
         """the fused gather + GEMM kernel takes this layer (VD3D_DCN_FUSED=0 forces the im2col-planes + 1x1-conv path, kept for A/B and tests)"""
         import os
-        return (self.main.engine == "tc16" and os.environ.get("VD3D_DCN_FUSED", "1") != "0" and os.environ.get("VD3D_TC_PERSIST", "1") != "0"
-                and self.KH * self.KW <= 9 and self.dg == 1 and self.C % 64 == 0)
+        return (self.main.engine == "tc16" and os.environ.get("VD3D_DCN_FUSED", "1") != "0" and self.KH * self.KW <= 9 and self.dg == 1 and self.C % 64 == 0)
 
 
 class DwConvLayer:
