@@ -277,6 +277,24 @@ int vd3d_preprocess_desc_bytes(void);
 int vd3d_preprocess_describe(void* desc_host, const unsigned char* src_dev, int H, int W, int C, int pitch, int crop_top, int Ho, int Wo);
 int vd3d_preprocess(const void* descs_dev, int B, int C, int Ho, int Wo, const float* mean, const float* stdv, float* out, void* stream);
 
+/* ---- training-time image augmentation (R/data/pipeline/stereo_augmentator.py, the shipped train_augmentation lists) ----
+ * uint8 HWC frame (C == 3) -> geometry -> photometric program -> mirror -> (v / 255 - mean[c]) / std[c] -> [3][Ho][Wo] float32.
+ * vd3d_train_augment_describe packs one frame's descriptor of vd3d_train_augment_desc_bytes() bytes:
+ *   geom 0: CropTop(crop_top) + Resize(preserve aspect, height Ho) cropped / zero padded on the right to Wo; the photometric program runs
+ *           on the source pixels before the interpolation (source step <= 2 per axis);
+ *   geom 1 / 2: cv2.warpAffine of the float32 forward matrix `affine` [2][3] on the uint8 frame (1) or on its float32 copy (2); the
+ *           program runs on the warped values;
+ *   mirror: flip the finished Wo-wide image;  ops[nops <= 8] / args[nops]: 1 brightness +=, 2 contrast *=, 3 RGB->HSV, 4 saturation *=,
+ *           5 hue += with the 360 wrap, 6 HSV->RGB, 7 eigenvalue noise += noise[3] (float64).
+ * vd3d_train_augment_host runs one descriptor on the HOST (src a host pointer; the parity checker); vd3d_train_augment is the CUDA form:
+ * `descs_dev` = n descriptors with device `src` pointers (frames of different sizes, both cameras of a stereo batch), out = [n][3][Ho][Wo],
+ * one launch.  Random draws, calibration and label updates are host work (visualdet3d_b200/train_augment.py). */
+int vd3d_train_augment_desc_bytes(void);
+int vd3d_train_augment_describe(void* desc, const unsigned char* src, int H, int W, int C, int pitch, int geom, int crop_top, int Ho, int Wo,
+                                const float* affine, int mirror, int nops, const int* ops, const float* args, const double* noise);
+int vd3d_train_augment_host(const void* desc, int C, int Ho, int Wo, const float* mean, const float* stdv, float* out);
+int vd3d_train_augment(const void* descs_dev, int n, int C, int Ho, int Wo, const float* mean, const float* stdv, float* out, void* stream);
+
 /* ---- post-optimisation of the yaw by hill climbing (R/lib/fast_utils/hill_climbing.py:24-122; caller detection_3d_head.py:294-308) ----
  * For each detection the yaw ry is moved in +-step_r steps (halved when neither direction improves, until step_r <= r_lim) to maximise
  * the IoU between the detected 2-D box and the hull of the projected 3-D box (clipped to img_w x img_h; the reference hard-codes 1280 x 288).

@@ -83,6 +83,10 @@ _SIGS = {
     "vd3d_preprocess_desc_bytes": (I, []),
     "vd3d_preprocess_describe": (I, [P, P, I, I, I, I, I, I, I]),
     "vd3d_preprocess": (I, [P, I, I, I, I, P, P, P, P]),
+    "vd3d_train_augment_host": (I, [P, I, I, I, P, P, P]),
+    "vd3d_train_augment_desc_bytes": (I, []),
+    "vd3d_train_augment_describe": (I, [P, P, I, I, I, I, I, I, I, I, P, I, I, P, P, P]),
+    "vd3d_train_augment": (I, [P, I, I, I, I, P, P, P, P]),
     "vd3d_post_opt_host": (I, [P, P, I, P, P, P, P, P, P, P, P, c_double, c_double, c_double, c_double, P, P]),
     "vd3d_post_opt": (I, [P, P, P, P, I, I, F, F, F, F, F, I, P]),
     "vd3d_fp16_range_check": (I, [P, I, P]),

@@ -4,6 +4,7 @@
 // One routine per output value, shared by the host entry (vd3d_preprocess_host: parity against the reference's cv2 / numpy pipeline on
 // the CPU) and the CUDA kernel (vd3d_preprocess: one thread per output pixel, frames of different sizes in one batch).
 #include "common.cuh"
+#include "resize_common.cuh"
 #include <math.h>
 
 namespace vd3d {
@@ -20,16 +21,6 @@ struct PreParams {
     int C, Ho, Wo;              // output [C][Ho][Wo] per image (Ho == Hr)
     float mean[4], stdv[4];
 };
-
-// cv2.resize INTER_LINEAR source index / weight of destination index d (resize.cpp: fx = (d + 0.5) * scale - 0.5, clamped at the borders)
-__host__ __device__ inline void lin_coord(int d, double scale, int n, int* s0, float* w1) {
-    const double fd = (d + 0.5) * scale - 0.5;       // fraction taken in double (what the IPP-backed cv2 builds do; OpenCV's own C++ path
-    int s = (int)floor(fd);                           // rounds the coordinate to float32 first, moving the weight by up to 6e-5 at x ~ 1000)
-    float f = (float)(fd - (double)s);
-    if (s < 0) { f = 0.f; s = 0; }
-    if (s >= n - 1) { f = 0.f; s = n - 1; }
-    *s0 = s; *w1 = f;
-}
 
 __host__ __device__ inline float pre_value(const PreImage& im, const PreParams& p, int c, int y, int x) {
     float v = 0.f;                                       // zero padding on the right happens BEFORE Normalize
@@ -63,14 +54,11 @@ static int fill(PreImage* im, PreParams* p, const unsigned char* src, int H, int
                 const float* mean, const float* stdv) {
     VD3D_REQUIRE(src && H > 0 && W > 0 && C >= 1 && C <= 4 && pitch >= W * C && crop_top >= 0 && crop_top < H && Ho > 0 && Wo > 0 && mean && stdv,
                  "preprocess: bad arguments");
-    const int Hc = H - crop_top;
-    const double sf = (double)Ho / (double)Hc;           // Resize(preserve_aspect_ratio): scale_factor = size[0] / image height
+    const ResizeGeom g = resize_geom(H - crop_top, W, Ho);
     im->src = src; im->H = H; im->W = W; im->pitch = pitch; im->crop_top = crop_top;
-    im->Hr = (int)nearbyint((double)Hc * sf);            // np.round
-    im->Wr = (int)nearbyint((double)W * sf);
+    im->Hr = g.Hr; im->Wr = g.Wr;
     VD3D_REQUIRE(im->Hr == Ho, "preprocess: rounded resized height %d != network height %d", im->Hr, Ho);
-    im->scale_y = 1.0 / ((double)im->Hr / (double)Hc);   // cv2: inv_scale = dsize / ssize, scale = 1 / inv_scale
-    im->scale_x = 1.0 / ((double)im->Wr / (double)W);
+    im->scale_y = g.scale_y; im->scale_x = g.scale_x;
     p->C = C; p->Ho = Ho; p->Wo = Wo;
     for (int c = 0; c < C; ++c) { p->mean[c] = mean[c]; p->stdv[c] = stdv[c]; }
     return VD3D_OK;

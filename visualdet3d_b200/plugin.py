@@ -161,3 +161,87 @@ def install_disparity_loss_into_reference():
     from .disparity_loss import forward
     ref_losses.DisparityLoss.forward = forward
     return forward
+
+
+# The reference's training datasets, the position of their images in the collate_fn's tuple, and the training function that consumes it.
+_AUG_DATASETS = (("visualDet3D.data.kitti.dataset.stereo_dataset", "KittiStereoDataset", 2),
+                 ("visualDet3D.data.kitti.dataset.mono_dataset", "KittiMonoDataset", 1),
+                 ("visualDet3D.data.kitti.dataset.KM3D_dataset", "KittiRTM3DDataset", 1))
+_AUG_TRAINERS = {"train_stereo_detection": 2, "train_mono_detection": 1, "train_rtm3d": 1}
+
+
+def install_train_augmentation_into_reference():
+    """Make the REFERENCE's training datasets augment on the GPU (`train_augment.TrainAugmentation`, `csrc/train_augment.cu`):
+      * `build_augmentator` of the three dataset modules returns a `TrainAugmentation` for a training list it supports (one with a random
+        transform; the five shipped training lists) and the reference's own `Compose` for every other list, test lists included;
+      * the `collate_fn` of KittiStereoDataset, KittiMonoDataset and KittiRTM3DDataset (KittiMonoFlexDataset inherits it) stacks the
+        DeferredFrames of a batch into one `train_augment.DeferredBatch` (uint8 staging + parameters; both cameras of a stereo batch in one)
+        where the reference stacked float images; every other element comes from the reference's collate_fn unchanged;
+      * `train_stereo_detection`, `train_mono_detection` and `train_rtm3d` in PIPELINE_DICT turn the DeferredBatch into the CUDA float
+        batch (one upload, one kernel) and call the reference function unchanged.
+    The numpy RNG draws are the reference's, so labels, P2 / P3 and disparity are the reference's and the images agree within the
+    augmentation's parity bound (DESIGN §3.18).  Returns the installed build_augmentator."""
+    import importlib
+    from visualDet3D.data.pipeline import build_augmentator as ref_build     # ImportError if the reference is not on sys.path
+    from visualDet3D.networks.utils import registry as ref
+    from . import train_augment as ta
+
+    def build_augmentator(aug_cfg):
+        if ta.is_training_list(aug_cfg) and ta.supports(aug_cfg):
+            return ta.TrainAugmentation(aug_cfg)
+        return ref_build(aug_cfg)
+
+    for modname, clsname, nimg in _AUG_DATASETS:
+        mod = importlib.import_module(modname)
+        mod.build_augmentator = build_augmentator
+        cls = getattr(mod, clsname)
+        ref_collate = getattr(cls.collate_fn, "_vd3d_ref", cls.collate_fn)           # installing twice wraps the reference once
+        cls.collate_fn = staticmethod(_deferred_collate(ref_collate, nimg))
+
+    for name, nimg in _AUG_TRAINERS.items():
+        fn = ref.PIPELINE_DICT[name]
+        fn = getattr(fn, "_vd3d_ref", fn)
+        ref.PIPELINE_DICT._register_module(_deferred_trainer(fn, nimg), force=True)
+    return build_augmentator
+
+
+def _deferred_collate(ref_collate, nimg):
+    import numpy as np
+    from .train_augment import DeferredBatch, DeferredFrame
+
+    def collate_fn(batch):
+        first = batch[0]["image"]
+        if not isinstance(first[0] if nimg == 2 else first, DeferredFrame):
+            return ref_collate(batch)
+        if nimg == 2:
+            frames = [item["image"][0] for item in batch] + [item["image"][1] for item in batch]
+        else:
+            frames = [item["image"] for item in batch]
+        tiny = np.zeros((1, 1, 3), np.float32)           # the reference stacks these in place of the images; its other outputs are kept
+        rest = ref_collate([dict(item, image=[tiny, tiny] if nimg == 2 else tiny) for item in batch])
+        images = DeferredBatch(frames)
+        return (images,) * nimg + tuple(rest[nimg:])
+
+    collate_fn._vd3d_ref = ref_collate
+    collate_fn.__name__ = "collate_fn"
+    return collate_fn
+
+
+def _deferred_trainer(ref_fn, nimg):
+    import functools
+    from .train_augment import DeferredBatch
+
+    @functools.wraps(ref_fn)
+    def train(data, *args, **kwargs):
+        if isinstance(data[0], DeferredBatch):
+            images = data[0].to_device("cuda")
+            B = len(data[0]) // nimg
+            data = list(data)
+            data[:nimg] = [images[:B], images[B:]] if nimg == 2 else [images]
+            if ref_fn.__name__ == "train_rtm3d":
+                data[1] = data[1].cuda()                 # `image.new(K)` aliases K: it must be on the images' device
+            data = tuple(data)
+        return ref_fn(data, *args, **kwargs)
+
+    train._vd3d_ref = ref_fn
+    return train
