@@ -295,6 +295,26 @@ int vd3d_train_augment_describe(void* desc, const unsigned char* src, int H, int
 int vd3d_train_augment_host(const void* desc, int C, int Ho, int Wo, const float* mean, const float* stdv, float* out);
 int vd3d_train_augment(const void* descs_dev, int n, int C, int Ho, int Wo, const float* mean, const float* stdv, float* out, void* stream);
 
+/* ---- KM3D / MonoFlex training targets (R/data/kitti/dataset/KM3D_dataset.py:57-221 KittiRTM3DDataset._build_target, :346-527
+ * KittiMonoFlexDataset._build_target; R/networks/utils/rtm3d_utils.py:52-109 gaussian_radius / gaussian2D / gen_hm_radius) ----
+ * vd3d_center_targets_pack fills one image's record of vd3d_center_targets_record_bytes() bytes: mode 0 KM3D (9 keypoints) / 1 MonoFlex
+ * (10 keypoints), the augmented image's img_h x img_w, num_classes, the float64 P2 [3][4], n <= 32 objects as float64
+ * objs[n][11] = x, y, z, w, h, l, ry, bbox_l, bbox_t, bbox_r, bbox_b and their class indices cls[n].
+ * outs = 21 pointers, in this order: hm, hm_hp, hps, reg, hp_offset, dim, rots, rotbin, rotres, dep, ind, hp_ind, reg_mask, hps_mask,
+ * hp_mask, wh, location, ori, kp_detph_mask, bboxes2d, bboxes2d_target (the reference's dtypes: float32, int64 for rotbin / ind / hp_ind,
+ * uint8 for the three masks but kp_detph_mask, which is float32; the last three are MonoFlex's and may be null for KM3D).
+ * vd3d_center_targets_host computes one image on the HOST (the parity checker; outs = that image's arrays).  vd3d_center_targets is the
+ * CUDA form: recs_dev = B records of one mode / size / class count, outs = a HOST array of DEVICE pointers to [B, ...] arrays,
+ * splats_dev = B * vd3d_center_targets_splat_bytes() bytes of scratch; two launches, no synchronisation.  edge_indices is a constant of
+ * the image size and is built on the host (visualdet3d_b200/center_targets.py). */
+int vd3d_center_targets_record_bytes(void);
+int vd3d_center_targets_splat_bytes(void);
+int vd3d_center_targets_pack(void* rec, int mode, int img_h, int img_w, int num_classes, const double* P2, int n, const double* objs,
+                             const int* cls);
+int vd3d_center_targets_host(const void* rec, int mode, int img_h, int img_w, int num_classes, void* const* outs);
+int vd3d_center_targets(const void* recs_dev, int B, int mode, int img_h, int img_w, int num_classes, void* const* outs, void* splats_dev,
+                        void* stream);
+
 /* ---- post-optimisation of the yaw by hill climbing (R/lib/fast_utils/hill_climbing.py:24-122; caller detection_3d_head.py:294-308) ----
  * For each detection the yaw ry is moved in +-step_r steps (halved when neither direction improves, until step_r <= r_lim) to maximise
  * the IoU between the detected 2-D box and the hull of the projected 3-D box (clipped to img_w x img_h; the reference hard-codes 1280 x 288).

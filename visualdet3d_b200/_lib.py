@@ -87,6 +87,11 @@ _SIGS = {
     "vd3d_train_augment_desc_bytes": (I, []),
     "vd3d_train_augment_describe": (I, [P, P, I, I, I, I, I, I, I, I, P, I, I, P, P, P]),
     "vd3d_train_augment": (I, [P, I, I, I, I, P, P, P, P]),
+    "vd3d_center_targets_record_bytes": (I, []),
+    "vd3d_center_targets_splat_bytes": (I, []),
+    "vd3d_center_targets_pack": (I, [P, I, I, I, I, P, I, P, P]),
+    "vd3d_center_targets_host": (I, [P, I, I, I, I, P]),
+    "vd3d_center_targets": (I, [P, I, I, I, I, I, P, P, P]),
     "vd3d_post_opt_host": (I, [P, P, I, P, P, P, P, P, P, P, P, c_double, c_double, c_double, c_double, P, P]),
     "vd3d_post_opt": (I, [P, P, P, P, I, I, F, F, F, F, F, I, P]),
     "vd3d_fp16_range_check": (I, [P, I, P]),

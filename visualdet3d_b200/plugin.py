@@ -205,22 +205,66 @@ def install_train_augmentation_into_reference():
     return build_augmentator
 
 
+def install_train_targets_into_reference():
+    """Make the REFERENCE's KM3D and MonoFlex datasets build their training targets on the GPU (`center_targets`,
+    `csrc/center_targets.cu`):
+      * `_build_target` of KittiRTM3DDataset and KittiMonoFlexDataset returns a `center_targets.DeferredTargets` (the image's packed
+        labels; only `image.shape` is read, so a numpy image and a DeferredFrame both work);
+      * their `collate_fn` stacks those into one `center_targets.DeferredTargetBatch` where the reference stacked the target dict;
+      * `train_rtm3d` in PIPELINE_DICT turns it into the reference's target dict of CUDA tensors (one upload, two launches) and calls the
+        reference function unchanged, whose `gts[key].cuda()` is then a no-op.
+    Works alone and with `install_train_augmentation_into_reference()`, in either order.  Returns the installed `_build_target`."""
+    from visualDet3D.data.kitti.dataset import KM3D_dataset as mod              # ImportError if the reference is not on sys.path
+    from visualDet3D.networks.utils import registry as ref
+    from . import center_targets as ct
+
+    def _build_target(self, image, P2, transformed_label, scale=4):
+        if scale != ct.SCALE:
+            raise NotImplementedError(f"_build_target: the GPU targets use the reference's scale {ct.SCALE}, not {scale}")
+        mode = {9: ct.MODE_KM3D, 10: ct.MODE_MONOFLEX}[self.num_vertexes]
+        return ct.DeferredTargets.build(image.shape, P2, transformed_label, [self.obj_types.index(o.type) for o in transformed_label],
+                                        self.num_classes, mode)
+
+    mod.KittiRTM3DDataset._build_target = _build_target
+    mod.KittiMonoFlexDataset._build_target = _build_target
+    cls = mod.KittiRTM3DDataset
+    cls.collate_fn = staticmethod(_deferred_collate(getattr(cls.collate_fn, "_vd3d_ref", cls.collate_fn), 1))
+    fn = ref.PIPELINE_DICT["train_rtm3d"]
+    ref.PIPELINE_DICT._register_module(_deferred_trainer(getattr(fn, "_vd3d_ref", fn), 1), force=True)
+    return _build_target
+
+
+# The position of the target dict in the KM3D / MonoFlex collate_fn's (images, calib, label) tuple.
+_TARGET_SLOT = 2
+
+
 def _deferred_collate(ref_collate, nimg):
+    """The collate_fn of both training installs: DeferredFrames become one DeferredBatch (install_train_augmentation_into_reference) and
+    DeferredTargets one DeferredTargetBatch (install_train_targets_into_reference); everything else comes from the reference's."""
     import numpy as np
+    from .center_targets import DeferredTargetBatch, DeferredTargets
     from .train_augment import DeferredBatch, DeferredFrame
 
     def collate_fn(batch):
         first = batch[0]["image"]
-        if not isinstance(first[0] if nimg == 2 else first, DeferredFrame):
+        images = isinstance(first[0] if nimg == 2 else first, DeferredFrame)
+        targets = isinstance(batch[0].get("label"), DeferredTargets)
+        if not (images or targets):
             return ref_collate(batch)
-        if nimg == 2:
-            frames = [item["image"][0] for item in batch] + [item["image"][1] for item in batch]
-        else:
-            frames = [item["image"] for item in batch]
         tiny = np.zeros((1, 1, 3), np.float32)           # the reference stacks these in place of the images; its other outputs are kept
-        rest = ref_collate([dict(item, image=[tiny, tiny] if nimg == 2 else tiny) for item in batch])
-        images = DeferredBatch(frames)
-        return (images,) * nimg + tuple(rest[nimg:])
+        stub = {}
+        if images:
+            stub["image"] = [tiny, tiny] if nimg == 2 else tiny
+        if targets:
+            stub["label"] = {}                           # an empty target dict collates to {}
+        out = list(ref_collate([dict(item, **stub) for item in batch]))
+        if images:
+            frames = [item["image"][0] for item in batch] + [item["image"][1] for item in batch] if nimg == 2 else \
+                [item["image"] for item in batch]
+            out[:nimg] = [DeferredBatch(frames)] * nimg
+        if targets:
+            out[_TARGET_SLOT] = DeferredTargetBatch([item["label"] for item in batch])
+        return tuple(out)
 
     collate_fn._vd3d_ref = ref_collate
     collate_fn.__name__ = "collate_fn"
@@ -229,10 +273,13 @@ def _deferred_collate(ref_collate, nimg):
 
 def _deferred_trainer(ref_fn, nimg):
     import functools
+    from .center_targets import DeferredTargetBatch
     from .train_augment import DeferredBatch
 
     @functools.wraps(ref_fn)
     def train(data, *args, **kwargs):
+        if ref_fn.__name__ == "train_rtm3d" and isinstance(data[_TARGET_SLOT], DeferredTargetBatch):
+            data = tuple(data[:_TARGET_SLOT]) + (data[_TARGET_SLOT].to_device("cuda"),) + tuple(data[_TARGET_SLOT + 1:])
         if isinstance(data[0], DeferredBatch):
             images = data[0].to_device("cuda")
             B = len(data[0]) // nimg
