@@ -548,6 +548,37 @@ int vd3d_disparity_loss_forward(const float* cost, const float* disp, int B, int
 int vd3d_disparity_loss_backward(const float* cost, const float* disp, const float* lse, int B, int D, int H, int W, const float* grad_loss,
                                  float* grad_cost, void* stream);
 
+/* ---- Stereo3D's disparity ground truth (scripts/disparity_compute.py: compute_dispairity_for_split) --------------------------------
+ * StereoBM: cv2.StereoBM_create(192, 25).compute with cv2's defaults (XSOBEL prefilter, cap 31, texture threshold 10, uniqueness 15 %, no
+ *   speckle filter, no left-right check, minDisparity 0), bit for bit.  left / right [B][H][W]; disp [B][H][W] int16 = 16 x disparity,
+ *   -16 where filtered and on the border StereoBM never computes (rows < 12 or >= H-12, columns < 203 or >= W-12).  26 <= H, 216 <= W
+ *   (cv2 has no defined output below), H, W <= 16384, B <= 65535.  workspace: vd3d_stereo_bm_workspace_bytes(B, H, W) bytes of device
+ *   memory (the prefiltered frames; negative: error code).  Three launches.
+ * vd3d_stereo_bm: uint8 grey frames.
+ * vd3d_stereo_bm_f32: float32 [B][H][W][3] normalised network input (the test augmentation's output); each pixel is de-normalised as the
+ *   script's denorm does (x * std + mean in float64, clipped to [0, 1], * 255, truncated) and converted with COLOR_BGR2GRAY (channel 0
+ *   weighted as blue).  mean_host / std_host: 3 float64 each.  grey [2][B][H][W] uint8 (left frames, then right; may be null) receives
+ *   the grey frames.
+ * vd3d_disparity_block_max: skimage.measure.block_reduce(max(in, 0) as uint16, (4, 4), np.max): in [B][H][W] int16 (is_signed) or uint16,
+ *   out [B][ceil(H/4)][ceil(W/4)] uint16, the far edges zero-padded.  One launch.
+ * vd3d_velo_disparity: generate_dispariy_from_velo (R/data/kitti/utils.py:85-120) for one frame.  points [N][stride] float32 (x, y, z
+ *   first; stride >= 3), R0_host / Tr_host the calibration's 4x4 R0_rect / Tr_velo_to_cam, P2_host [3][4], all float64 host arrays.
+ *   full [H][W] uint16 = uint16(P2[0, 0] * baseline / depth * 16) of the LAST in-view point (cloud order) of each pixel, 0 where none.
+ *   winner: H * W int32 of device scratch.  A memset and two launches.
+ * The _host forms compute one frame on the host with the kernels' per-element routines (the parity checker). */
+long long vd3d_stereo_bm_workspace_bytes(int B, int H, int W);
+int vd3d_stereo_bm(const uint8_t* left, const uint8_t* right, int B, int H, int W, uint8_t* workspace, int16_t* disp, void* stream);
+int vd3d_stereo_bm_f32(const float* left, const float* right, int B, int H, int W, const double* mean_host, const double* std_host,
+                       uint8_t* workspace, uint8_t* grey, int16_t* disp, void* stream);
+int vd3d_disparity_block_max(const void* in, int is_signed, int B, int H, int W, uint16_t* out, void* stream);
+int vd3d_velo_disparity(const float* points, int N, int stride, const double* R0_host, const double* Tr_host, const double* P2_host,
+                        double baseline, int H, int W, int* winner, uint16_t* full, void* stream);
+int vd3d_disparity_grey_host(const float* img, int H, int W, const double* mean, const double* std, uint8_t* grey);
+int vd3d_stereo_bm_host(const uint8_t* left, const uint8_t* right, int H, int W, int16_t* disp);
+int vd3d_disparity_block_max_host(const void* in, int is_signed, int H, int W, uint16_t* out);
+int vd3d_velo_disparity_host(const float* points, int N, int stride, const double* R0, const double* Tr, const double* P2,
+                             double baseline, int H, int W, uint16_t* full);
+
 #ifdef __cplusplus
 }
 #endif

@@ -122,6 +122,15 @@ _SIGS = {
     "vd3d_disparity_loss_workspace_bytes": (c_longlong, [I, I, I, I]),
     "vd3d_disparity_loss_forward": (I, [P, P, I, I, I, I, P, c_longlong, P, P, P]),
     "vd3d_disparity_loss_backward": (I, [P, P, P, I, I, I, I, P, P, P]),
+    "vd3d_stereo_bm_workspace_bytes": (c_longlong, [I, I, I]),
+    "vd3d_stereo_bm": (I, [P, P, I, I, I, P, P, P]),
+    "vd3d_stereo_bm_f32": (I, [P, P, I, I, I, P, P, P, P, P, P]),
+    "vd3d_disparity_block_max": (I, [P, I, I, I, I, P, P]),
+    "vd3d_velo_disparity": (I, [P, I, I, P, P, P, c_double, I, I, P, P, P]),
+    "vd3d_disparity_grey_host": (I, [P, I, I, P, P, P]),
+    "vd3d_stereo_bm_host": (I, [P, P, I, I, P]),
+    "vd3d_disparity_block_max_host": (I, [P, I, I, I, P]),
+    "vd3d_velo_disparity_host": (I, [P, I, I, P, P, P, c_double, I, I, P]),
 }
 
 
