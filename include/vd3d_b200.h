@@ -265,30 +265,20 @@ int vd3d_km3d_decode(const float* heads, int B, int H, int W, int ncls, int cs, 
                      int out_cap, float* out_scores, float* out_boxes, long long* out_cls, int* out_index, int* out_count,
                      int* out_ncand, void* stream);
 
-/* ---- input pipeline (R/data/pipeline/stereo_augmentator.py:29-134,213-258: ConvertToFloat, CropTop, Resize, Normalize) -------------------
- * uint8 HWC frame -> rows [crop_top, H) -> cv2.resize(INTER_LINEAR, float32) to height Ho with the aspect ratio preserved -> cropped / zero
- * padded on the right to Wo -> (v / 255 - mean[c]) / std[c] -> [C][Ho][Wo] float32.  vd3d_preprocess_host runs on the HOST (parity against the
- * reference's cv2 / numpy pipeline); vd3d_preprocess is the batched CUDA form: `descs_dev` = B records of vd3d_preprocess_desc_bytes() bytes
- * each, filled on the host by vd3d_preprocess_describe (frames of different sizes in one batch; src = DEVICE pointer to the uploaded frame),
- * out = [B][C][Ho][Wo].  The calibration update of CropTop / Resize is host arithmetic (visualdet3d_b200/preprocess.py). */
-int vd3d_preprocess_host(const unsigned char* src, int H, int W, int C, int pitch, int crop_top, int Ho, int Wo,
-                         const float* mean, const float* stdv, float* out);
-int vd3d_preprocess_desc_bytes(void);
-int vd3d_preprocess_describe(void* desc_host, const unsigned char* src_dev, int H, int W, int C, int pitch, int crop_top, int Ho, int Wo);
-int vd3d_preprocess(const void* descs_dev, int B, int C, int Ho, int Wo, const float* mean, const float* stdv, float* out, void* stream);
-
-/* ---- training-time image augmentation (R/data/pipeline/stereo_augmentator.py, the shipped train_augmentation lists) ----
+/* ---- image input pipelines (R/data/pipeline/stereo_augmentator.py: the test_augmentation and the shipped train_augmentation lists) ----
  * uint8 HWC frame (C == 3) -> geometry -> photometric program -> mirror -> (v / 255 - mean[c]) / std[c] -> [3][Ho][Wo] float32.
- * vd3d_train_augment_describe packs one frame's descriptor of vd3d_train_augment_desc_bytes() bytes:
+ * vd3d_train_augment_describe packs one frame's descriptor of vd3d_train_augment_desc_bytes() bytes (`pitch` bytes per frame row):
  *   geom 0: CropTop(crop_top) + Resize(preserve aspect, height Ho) cropped / zero padded on the right to Wo; the photometric program runs
  *           on the source pixels before the interpolation (source step <= 2 per axis);
  *   geom 1 / 2: cv2.warpAffine of the float32 forward matrix `affine` [2][3] on the uint8 frame (1) or on its float32 copy (2); the
  *           program runs on the warped values;
  *   mirror: flip the finished Wo-wide image;  ops[nops <= 8] / args[nops]: 1 brightness +=, 2 contrast *=, 3 RGB->HSV, 4 saturation *=,
  *           5 hue += with the 360 wrap, 6 HSV->RGB, 7 eigenvalue noise += noise[3] (float64).
+ * Geometry 0 with no ops and no mirror is the test-time pipeline (ConvertToFloat, CropTop, Resize, Normalize: visualdet3d_b200/preprocess.py
+ * and pipeline.StreamedInference.submit_frames).
  * vd3d_train_augment_host runs one descriptor on the HOST (src a host pointer; the parity checker); vd3d_train_augment is the CUDA form:
  * `descs_dev` = n descriptors with device `src` pointers (frames of different sizes, both cameras of a stereo batch), out = [n][3][Ho][Wo],
- * one launch.  Random draws, calibration and label updates are host work (visualdet3d_b200/train_augment.py). */
+ * one launch.  Random draws, calibration and label updates are host work (visualdet3d_b200/train_augment.py, preprocess.adjust_calib). */
 int vd3d_train_augment_desc_bytes(void);
 int vd3d_train_augment_describe(void* desc, const unsigned char* src, int H, int W, int C, int pitch, int geom, int crop_top, int Ho, int Wo,
                                 const float* affine, int mirror, int nops, const int* ops, const float* args, const double* noise);

@@ -1,5 +1,5 @@
-"""Constructed frames and descriptors for the training augmentation (visualdet3d_b200/csrc/train_augment.cu) and the test-time resize
-(csrc/preprocess.cu), built directly rather than through TrainAugmentation's random draws.  Used by tests/golden/make_golden_augment_cases.py
+"""Constructed frames and descriptors for the augmentation kernel (visualdet3d_b200/csrc/train_augment.cu), for training and as the
+test-time resize, built directly rather than through TrainAugmentation's random draws.  Used by tests/golden/make_golden_augment_cases.py
 (the cv2 / numpy expectation), tests/test_augment_cases_cpu.py and tests/test_augment_cases_gpu.py.
 
 Every case is a dict: id, group ("resize" geometry only, "warp", or "colour" for a photometric program), the uint8 HWC frame, geom, crop_top,

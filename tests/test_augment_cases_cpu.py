@@ -1,4 +1,4 @@
-"""The training augmentation's host form (`vd3d_train_augment_host`) and the test-time resize's host form (`vd3d_preprocess_host`) on the
+"""The augmentation's host form (`vd3d_train_augment_host`), for training and as the test-time resize (`preprocess_host`), on the
 constructed cases of tests/augment_cases.py, without a GPU:
   * against the cv2 / numpy fixture (tests/golden/make_golden_augment_cases.py): 2e-6 on geometry, 5e-5 on colour programs;
   * against float64 closed forms on the impulse, ramp, integral-warp and all-outside cases;

@@ -1,4 +1,4 @@
-"""The training augmentation kernel (`vd3d_train_augment`) and the test-time resize kernel (`vd3d_preprocess`) on the constructed cases of
+"""The augmentation kernel (`vd3d_train_augment`), for training and as the test-time resize (`preprocess_batch`), on the constructed cases of
 tests/augment_cases.py: bit for bit equal to their host forms, and within the CPU bars of the cv2 fixture (2e-6 geometry, 5e-5 colour) and of
 the float64 closed forms.  Each case runs alone, then every case of one output size in a single launch (mixed source sizes, mirrors, both
 warp geometries), twice with the same bits.  The output buffer is filled with NaN before each launch, so an element the kernel never writes

@@ -1,5 +1,5 @@
 """SURVEY.md 8(f) rank 3 — test-time input pipeline (uint8 frame -> CropTop -> cv2-style bilinear Resize -> Normalize -> CHW, calibration
-update): visualdet3d_b200/preprocess.py + `vd3d_preprocess_host` against fixtures generated with the unmodified reference classes
+update): visualdet3d_b200/preprocess.py (`preprocess_host`) against fixtures generated with the unmodified reference classes
 (tests/golden/make_golden_preprocess.py; strided samples, sums, the last column and the first row of every output).
 Tolerance: 2e-5 on the normalised values (cv2's SIMD row / column passes may fuse multiply-adds; the bar of the path is 1e-3)."""
 import os
@@ -7,6 +7,7 @@ import sys
 import time
 
 import numpy as np
+import pytest
 
 from conftest import GOLDEN
 from visualdet3d_b200 import preprocess as pp
@@ -47,12 +48,9 @@ def test_pipeline_matches_reference_fixtures():
 
 def test_bad_arguments_are_reported():
     from visualdet3d_b200 import _lib
-    lib = _lib.load()
-    img = np.zeros((10, 20, 3), dtype=np.uint8)
-    out = np.zeros((3, 8, 16), dtype=np.float32)
-    m = np.zeros(3, dtype=np.float32)
-    import ctypes
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    assert lib.vd3d_preprocess_host(vp(img), 10, 20, 3, 60, 12, 8, 16, vp(m), vp(m), vp(out)) != 0        # crop_top >= H
-    assert lib.vd3d_preprocess_host(None, 10, 20, 3, 60, 2, 8, 16, vp(m), vp(m), vp(out)) != 0
-    assert lib.vd3d_preprocess_desc_bytes() >= 40
+    with pytest.raises(_lib.Vd3dError, match="crop_top"):
+        pp.preprocess_host(np.zeros((10, 20, 3), np.uint8), 12, (8, 16))        # crop_top >= H
+    with pytest.raises(_lib.Vd3dError, match="bad arguments"):
+        pp.preprocess_host(np.zeros((10, 20, 4), np.uint8), 2, (8, 16))         # C != 3
+    with pytest.raises(_lib.Vd3dError, match="shrinks"):
+        pp.preprocess_host(np.zeros((40, 20, 3), np.uint8), 0, (8, 16))         # a 5x source step: beyond the kernel's 2x stage

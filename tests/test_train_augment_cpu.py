@@ -101,13 +101,14 @@ def test_fixture_cases_cover_every_branch():
 
 def _describe(**over):
     a = dict(H=375, W=1242, C=3, geom=0, crop_top=100, Ho=288, Wo=1280, mirror=0, ops=[ta.OP_BRIGHTNESS], args=[3.0],
-             affine=np.array([[1.0, 0, 0], [0, 1.0, 0]], np.float32))
+             affine=np.array([[1.0, 0, 0], [0, 1.0, 0]], np.float32), null_src=False)
     a.update(over)
     frame = np.zeros((a["H"], a["W"], 3), np.uint8)
     desc = np.zeros(int(_lib.load().vd3d_train_augment_desc_bytes()), np.uint8)
     ops, args = np.array(a["ops"], np.int32), np.array(a["args"], np.float32)
     vp = lambda x: x.ctypes.data_as(ctypes.c_void_p)
-    _lib.call("vd3d_train_augment_describe", vp(desc), frame.ctypes.data, a["H"], a["W"], a["C"], a["W"] * 3, a["geom"], a["crop_top"],
+    src = None if a["null_src"] else frame.ctypes.data
+    _lib.call("vd3d_train_augment_describe", vp(desc), src, a["H"], a["W"], a["C"], a["W"] * 3, a["geom"], a["crop_top"],
               a["Ho"], a["Wo"], vp(a["affine"]), a["mirror"], len(ops), vp(ops), vp(args), None)
     return desc
 
@@ -123,6 +124,7 @@ def _describe(**over):
     (dict(Wo=0), "bad arguments"),
     (dict(H=900, W=3000, crop_top=0, Ho=288), "shrinks"),
     (dict(geom=1, affine=np.zeros((2, 3), np.float32)), "singular"),
+    (dict(null_src=True), "bad arguments"),
 ])
 def test_bad_descriptors_are_rejected(over, msg):
     with pytest.raises(_lib.Vd3dError, match=msg):

@@ -79,10 +79,6 @@ _SIGS = {
     "vd3d_monoflex_decode": (I, [P, I, I, I, I, I, I, I, I, I, I, I, I, I, I, P, F, c_double, I, F, F, F, F, I, P, I, P, P, P, P, P, P, P]),
     "vd3d_km3d_decode_workspace": (c_longlong, [I, I, I]),
     "vd3d_km3d_decode": (I, [P, I, I, I, I, I, I, I, I, I, I, I, I, I, I, P, F, c_double, I, F, F, I, I, P, I, P, P, P, P, P, P, P]),
-    "vd3d_preprocess_host": (I, [P, I, I, I, I, I, I, I, P, P, P]),
-    "vd3d_preprocess_desc_bytes": (I, []),
-    "vd3d_preprocess_describe": (I, [P, P, I, I, I, I, I, I, I]),
-    "vd3d_preprocess": (I, [P, I, I, I, I, P, P, P, P]),
     "vd3d_train_augment_host": (I, [P, I, I, I, P, P, P]),
     "vd3d_train_augment_desc_bytes": (I, []),
     "vd3d_train_augment_describe": (I, [P, P, I, I, I, I, I, I, I, I, P, I, I, P, P, P]),

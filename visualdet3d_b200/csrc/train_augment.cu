@@ -1,7 +1,7 @@
-// Training-time image augmentation: uint8 HWC frame -> photometric program / geometry / mirror / Normalize -> CHW float32, the image half
-// of the reference's `train_augmentation` chains.  Reference: R/data/pipeline/stereo_augmentator.py (ConvertToFloat :29-36, Normalize
-// :39-60, Resize :63-134, RandomSaturation :188-211, CropTop :213-258, RandomMirror :373-437, RandomWarpAffine :439-500, RandomHue :502-525,
-// ConvertColor :528-554, RandomContrast :557-578, RandomBrightness :580-598, RandomEigenvalueNoise :600-628, PhotometricDistort :630-668).
+// Image input pipelines: uint8 HWC frame -> photometric program / geometry / mirror / Normalize -> CHW float32.  Reference:
+// R/data/pipeline/stereo_augmentator.py (ConvertToFloat :29-36, Normalize :39-60, Resize :63-134, RandomSaturation :188-211, CropTop
+// :213-258, RandomMirror :373-437, RandomWarpAffine :439-500, RandomHue :502-525, ConvertColor :528-554, RandomContrast :557-578,
+// RandomBrightness :580-598, RandomEigenvalueNoise :600-628, PhotometricDistort :630-668).
 //
 // Two geometries:
 //   chain 1 (Stereo3D / Yolo3D / RetinaNet): the photometric program runs on SOURCE pixels, then CropTop + Resize (cv2 INTER_LINEAR on
@@ -9,13 +9,14 @@
 //   chain 2 (MonoFlex / KM3D): cv2.warpAffine (INTER_LINEAR, BORDER_CONSTANT 0, cv2's fixed-point source coordinates) on the uint8 frame
 //     (MonoFlex: the warp runs before ConvertToFloat) or on its float32 copy (KM3D), then the photometric program on the warped values.
 // Then the mirror (a flip of the finished Wo-wide image: the zero pad of chain 1 ends up on the left) and Normalize.
+// Geometry 0 (AUG_RESIZE) with no ops and no mirror is the test-time pipeline (the reference's `test_augmentation`: ConvertToFloat,
+// CropTop, Resize, Normalize); the other combinations are the image half of its `train_augmentation` chains.
 //
 // One routine per output pixel (aug_pixel) is shared by the host entry (vd3d_train_augment_host: the parity checker) and the CUDA kernel
 // (one launch per batch, frames of different sizes and both cameras of a stereo batch in one grid).  The kernel stages the distorted
-// source rows a tile needs in shared memory, so a chain-1 source pixel is distorted once per tile instead of once per bilinear tap.
+// source rows a tile needs in shared memory, so a chain-1 source pixel is read and distorted once per tile instead of once per bilinear tap.
 // Built with -fmad=false: every product and sum rounds separately, like numpy's float32 in-place ops and cv2's scalar loops.
 #include "common.cuh"
-#include "resize_common.cuh"
 #include <float.h>
 #include <string.h>
 #include <math.h>
@@ -27,6 +28,33 @@ enum { AUG_RESIZE = 0, AUG_WARP_U8 = 1, AUG_WARP_F32 = 2 };
 // > 360 / < 0 wrap), cv2 HSV->RGB, eigenvalue noise (+= a float64 per-channel vector).  No clamping: the reference does none.
 enum { OP_BRIGHTNESS = 1, OP_CONTRAST = 2, OP_RGB2HSV = 3, OP_SATURATION = 4, OP_HUE = 5, OP_HSV2RGB = 6, OP_EIGEN_NOISE = 7 };
 constexpr int AUG_MAX_OPS = 8;
+
+// cv2.resize INTER_LINEAR source index / weight of destination index d (resize.cpp: fx = (d + 0.5) * scale - 0.5, clamped at the borders)
+__host__ __device__ inline void lin_coord(int d, double scale, int n, int* s0, float* w1) {
+    const double fd = (d + 0.5) * scale - 0.5;       // fraction taken in double (what the IPP-backed cv2 builds do; OpenCV's own C++ path
+    int s = (int)floor(fd);                           // rounds the coordinate to float32 first, moving the weight by up to 6e-5 at x ~ 1000)
+    float f = (float)(fd - (double)s);
+    if (s < 0) { f = 0.f; s = 0; }
+    if (s >= n - 1) { f = 0.f; s = n - 1; }
+    *s0 = s; *w1 = f;
+}
+
+// Resize(size) with preserve_aspect_ratio on a frame of Hc x W rows / columns (after CropTop): scale_factor = size[0] / Hc, the resized
+// size np.round(Hc * scale_factor) x np.round(W * scale_factor), and cv2's per-axis source step 1 / (dst / src).
+struct ResizeGeom {
+    int Hr, Wr;
+    double scale_y, scale_x;
+};
+
+static inline ResizeGeom resize_geom(int Hc, int W, int Ho) {
+    ResizeGeom g;
+    const double sf = (double)Ho / (double)Hc;
+    g.Hr = (int)nearbyint((double)Hc * sf);            // np.round
+    g.Wr = (int)nearbyint((double)W * sf);
+    g.scale_y = 1.0 / ((double)g.Hr / (double)Hc);     // cv2: inv_scale = dsize / ssize, scale = 1 / inv_scale
+    g.scale_x = 1.0 / ((double)g.Wr / (double)W);
+    return g;
+}
 
 struct AugImage {
     const unsigned char* src;   // [H][pitch] bytes, 3 interleaved channels (HWC)

@@ -11,19 +11,20 @@ Two input forms:
   * `submit(*images, P2)`          float32 network inputs [B, 3, H, W] (what the reference's dataset + collate_fn produce on the CPU),
   * `submit_frames(*frames, P2)`   uint8 camera frames [B, Hf, Wf, 3]: 4x fewer H2D bytes; ConvertToFloat / CropTop / Resize / Normalize of
                                    the reference's test-time augmentation (R/data/pipeline/stereo_augmentator.py:29-134,213-258) run as one
-                                   kernel per camera on the device (csrc/preprocess.cu) right after the copy.
+                                   augmentation kernel launch per camera on the device (csrc/train_augment.cu) right after the copy.
 The multi-GPU exchange is off the compute stream: the record block of batch i is gathered on a side stream while batch i+1 computes, so
 ranks do not run in lockstep with the slowest GPU (`gather_stream`).
 """
 from __future__ import annotations
 
-import ctypes
 from typing import List, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib, parallel
+from . import train_augment as ta
+from .preprocess import RESIZE_ONLY, RGB_MEAN, RGB_STD
 
 
 class StreamedInference:
@@ -62,11 +63,10 @@ class StreamedInference:
         if self.frame_hw is not None:
             Hf, Wf = self.frame_hw
             self.frame_bufs = [tuple(torch.empty(batch, Hf, Wf, 3, device=dev, dtype=torch.uint8) for _ in range(n_img)) for _ in range(depth)]
-            nb = int(_lib.load().vd3d_preprocess_desc_bytes())
+            nb = int(_lib.load().vd3d_train_augment_desc_bytes())
             self._desc_host = [tuple(torch.zeros(batch, nb, dtype=torch.uint8).pin_memory() for _ in range(n_img)) for _ in range(depth)]
             self._desc_dev = [tuple(torch.empty(batch, nb, device=dev, dtype=torch.uint8) for _ in range(n_img)) for _ in range(depth)]
             self._desc_sizes = [None] * depth
-            from .preprocess import RGB_MEAN, RGB_STD
             self._mean = np.ascontiguousarray(np.array(RGB_MEAN, dtype=np.float32))
             self._std = np.ascontiguousarray(np.array(RGB_STD, dtype=np.float32))
             self.h2d_bytes_frames = n_img * batch * Hf * Wf * 3 + 4 * batch * 12
@@ -130,9 +130,9 @@ class StreamedInference:
             for c in range(self.n_img):
                 dh = self._desc_host[k][c].numpy()
                 for b in range(self.B):
-                    h, w = (key[b] if key is not None else (Hf, Wf))
-                    _lib.call("vd3d_preprocess_describe", dh[b].ctypes.data_as(ctypes.c_void_p), fb[c][b].data_ptr(), h, w, 3, Wf * 3,
-                              self.crop_top, self.H, self.W)
+                    h, w = (key[b] if key is not None else (Hf, Wf))          # stored top-left in the Wf-wide staging frame
+                    dh[b] = ta._describe(fb[c][b].data_ptr(), (h, w, 3), crop_top=self.crop_top, out_hw=(self.H, self.W), pitch=Wf * 3,
+                                         **RESIZE_ONLY)
         with torch.cuda.stream(self.copy_stream):
             if i >= self.depth:
                 self.copy_stream.wait_event(self.ev_free[k])
@@ -147,9 +147,8 @@ class StreamedInference:
                 self._desc_sizes[k] = ("u", key)
             self.ev_copied[k].record(self.copy_stream)
         cur.wait_event(self.ev_copied[k])
-        vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
         for c in range(self.n_img):          # test-time augmentation on the device: uint8 HWC -> cropped, resized, normalised float32 CHW
-            _lib.call("vd3d_preprocess", self._desc_dev[k][c].data_ptr(), self.B, 3, self.H, self.W, vp(self._mean), vp(self._std),
+            _lib.call("vd3d_train_augment", self._desc_dev[k][c].data_ptr(), self.B, 3, self.H, self.W, ta._vp(self._mean), ta._vp(self._std),
                       bufs[c].data_ptr(), cur.cuda_stream)
         return self._run(i, k, bufs[:self.n_img], bufs[self.n_img], bufs[self.n_img + 1] if original_P is not None else None)
 

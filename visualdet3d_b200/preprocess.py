@@ -3,20 +3,24 @@ numpy (R/data/pipeline/stereo_augmentator.py: ConvertToFloat :29-36, CropTop :21
 `KittiStereoDataset.__getitem__` / `collate_fn` (R/data/kitti/dataset/stereo_dataset.py:176-203): uint8 HWC frame -> float32 CHW network
 input, and the calibration matrices moved along.
 
-`preprocess_host` / `preprocess_batch` call the C-ABI library (one routine shared by the host entry and the CUDA kernel); the calibration
-update is host float arithmetic in the reference's order."""
+The image work is the training augmentation's geometry 0 with no photometric program and no mirror: `preprocess_host` / `preprocess_batch`
+are `train_augment.augment_host` / `augment_batch` on such DeferredFrames (one per-pixel routine shared by the host entry and the CUDA
+kernel).  The calibration update is host float arithmetic in the reference's order."""
 from __future__ import annotations
 
-import ctypes
-from typing import List, Sequence, Tuple
+from typing import List, Tuple
 
 import numpy as np
 import torch
 
-from . import _lib
+from . import train_augment as ta
 
 RGB_MEAN = (0.485, 0.456, 0.406)
 RGB_STD = (0.229, 0.224, 0.225)
+
+# The augmentation parameters of the test-time pipeline: CropTop + Resize, no warp, no mirror, no photometric program.
+RESIZE_ONLY = dict(geom=ta.GEOM_RESIZE, affine=np.zeros((2, 3), np.float32), mirror=0, ops=np.zeros(0, np.int32), args=np.zeros(0, np.float32),
+                   noise=np.zeros(3))
 
 
 def adjust_calib(P: np.ndarray, crop_top: int, height: int, out_height: int) -> np.ndarray:
@@ -30,42 +34,17 @@ def adjust_calib(P: np.ndarray, crop_top: int, height: int, out_height: int) -> 
     return P
 
 
-def _f32(v: Sequence[float]) -> np.ndarray:
-    return np.ascontiguousarray(np.array(v, dtype=np.float32))
+def _deferred(frame: np.ndarray, crop_top: int, size: Tuple[int, int], mean, std) -> ta.DeferredFrame:
+    return ta.DeferredFrame(frame, crop_top=int(crop_top), Ho=int(size[0]), Wo=int(size[1]), mean=mean, std=std, **RESIZE_ONLY)
 
 
 def preprocess_host(frame: np.ndarray, crop_top: int, size: Tuple[int, int], mean=RGB_MEAN, std=RGB_STD) -> np.ndarray:
-    """uint8 [H, W, C] -> float32 [C, size[0], size[1]] on the host: the parity checker of the CUDA form (`preprocess_batch` is the product
+    """uint8 [H, W, 3] -> float32 [3, size[0], size[1]] on the host: the parity checker of the CUDA form (`preprocess_batch` is the product
     path; tests pin this routine to the reference and the kernel to this routine)."""
-    assert frame.dtype == np.uint8 and frame.ndim == 3
-    frame = np.ascontiguousarray(frame)
-    H, W, C = frame.shape
-    out = np.empty((C, size[0], size[1]), dtype=np.float32)
-    m, s = _f32(mean), _f32(std)
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    _lib.call("vd3d_preprocess_host", vp(frame), H, W, C, W * C, int(crop_top), int(size[0]), int(size[1]), vp(m), vp(s), vp(out))
-    return out
+    return ta.augment_host(_deferred(frame, crop_top, size, mean, std))
 
 
 def preprocess_batch(frames: List[np.ndarray], crop_top: int, size: Tuple[int, int], mean=RGB_MEAN, std=RGB_STD, device="cuda") -> torch.Tensor:
-    """uint8 HWC frames (sizes may differ) -> [B, C, size[0], size[1]] float32 on `device`: one uint8 upload per frame (3 bytes per pixel
+    """uint8 HWC frames (sizes may differ) -> [B, 3, size[0], size[1]] float32 on `device`: one upload of the uint8 frames (3 bytes per pixel
     instead of 12) and one kernel for the whole batch."""
-    lib = _lib.load()
-    B = len(frames)
-    C = frames[0].shape[2]
-    nb = int(lib.vd3d_preprocess_desc_bytes())
-    descs = np.zeros((B, nb), dtype=np.uint8)
-    dev_frames = []
-    for i, f in enumerate(frames):
-        assert f.dtype == np.uint8 and f.ndim == 3 and f.shape[2] == C
-        t = torch.from_numpy(np.ascontiguousarray(f)).to(device, non_blocking=True)
-        dev_frames.append(t)
-        H, W, _ = f.shape
-        _lib.call("vd3d_preprocess_describe", descs[i].ctypes.data_as(ctypes.c_void_p), t.data_ptr(), H, W, C, W * C, int(crop_top), int(size[0]), int(size[1]))
-    d = torch.from_numpy(descs).to(device)
-    out = torch.empty(B, C, size[0], size[1], dtype=torch.float32, device=device)
-    m, s = _f32(mean), _f32(std)
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    _lib.call("vd3d_preprocess", d.data_ptr(), B, C, int(size[0]), int(size[1]), vp(m), vp(s), out.data_ptr(), torch.cuda.current_stream().cuda_stream)
-    out._vd3d_keepalive = (dev_frames, d)        # the frames / descriptors must outlive the asynchronous kernel
-    return out
+    return ta.augment_batch([_deferred(f, crop_top, size, mean, std) for f in frames], device)

@@ -47,26 +47,27 @@ class DeferredFrame:
 
     def __init__(self, frame, geom, crop_top, affine, mirror, ops, args, noise, Ho, Wo, mean, std):
         self.frame = np.ascontiguousarray(frame)
-        assert self.frame.dtype == np.uint8 and self.frame.ndim == 3 and self.frame.shape[2] == 3, "uint8 HWC frames with 3 channels"
+        assert self.frame.dtype == np.uint8 and self.frame.ndim == 3, "uint8 HWC frames"      # describe() refuses other than 3 channels
         self.geom, self.crop_top, self.affine, self.mirror = geom, crop_top, affine, mirror
         self.ops, self.args, self.noise = ops, args, noise
         self.shape = (Ho, Wo, 3)
-        self.mean, self.std = mean, std
+        self.mean, self.std = np.ascontiguousarray(mean, dtype=np.float32), np.ascontiguousarray(std, dtype=np.float32)
 
     def params(self):
-        """Everything but the frame's bytes: (H, W) of the frame and the kernel parameters."""
-        return (self.frame.shape[:2], self.geom, self.crop_top, self.affine, self.mirror, self.ops, self.args, self.noise, self.shape[:2])
+        """Everything but the frame's bytes: (H, W, C) of the frame and the kernel parameters."""
+        return (self.frame.shape, self.geom, self.crop_top, self.affine, self.mirror, self.ops, self.args, self.noise, self.shape[:2])
 
     def describe(self, src_ptr: int) -> np.ndarray:
         """The packed kernel descriptor of this frame read from `src_ptr` (host or device address of the frame's bytes)."""
         return _describe(src_ptr, *self.params())
 
 
-def _describe(src_ptr, hw, geom, crop_top, affine, mirror, ops, args, noise, out_hw) -> np.ndarray:
+def _describe(src_ptr, hwc, geom, crop_top, affine, mirror, ops, args, noise, out_hw, pitch=None) -> np.ndarray:
+    """The packed descriptor of an H x W x C frame at `src_ptr` whose rows are `pitch` bytes apart (default W * C: a packed frame)."""
     desc = np.zeros(int(_lib.load().vd3d_train_augment_desc_bytes()), dtype=np.uint8)
-    (H, W), (Ho, Wo) = hw, out_hw
-    _lib.call("vd3d_train_augment_describe", _vp(desc), src_ptr, H, W, 3, W * 3, geom, crop_top, Ho, Wo, _vp(affine), mirror, len(ops),
-              _vp(ops), _vp(args), _vp(noise))
+    (H, W, C), (Ho, Wo) = hwc, out_hw
+    _lib.call("vd3d_train_augment_describe", _vp(desc), src_ptr, H, W, C, W * C if pitch is None else pitch, geom, crop_top, Ho, Wo, _vp(affine),
+              mirror, len(ops), _vp(ops), _vp(args), _vp(noise))
     return desc
 
 
