@@ -569,6 +569,29 @@ int vd3d_disparity_block_max_host(const void* in, int is_signed, int H, int W, u
 int vd3d_velo_disparity_host(const float* points, int N, int stride, const double* R0, const double* Tr, const double* P2,
                              double baseline, int H, int W, uint16_t* full);
 
+/* ---- the 3-D anchor priors (scripts/imdb_precompute_3d.py: read_one_split, lines 106-135) ------------------------------------------
+ * One batch of B frames x T classes.  anchors [N][4] float32 (Anchors.forward's table for the post-augmentation shape).  The anchors of
+ *   bin k (scale row * n_ratios + ratio column, the reference's anchors2indexes on the float32 table) are order[bin_start[k] ..
+ *   bin_start[k+1]), ascending; bin_start_host: n_bins + 1 ints on the host.  offsets_host: B*T + 1 ints on the host, segment s = b * T + t
+ *   (frame b, class t) holding boxes offsets[s] .. offsets[s+1] (at most 512 each).  boxes [K_total][4] (x1, y1, x2, y2): float32, or
+ *   float64 with boxes_f64 (the IoU's dtype; the threshold is compared in the same dtype).  gt3 [K_total][3] float64 (z, sin 2a, cos 2a).
+ * For every segment and anchor: calc_iou against the segment's boxes, the first-maximum box, positive where the maximum is >
+ *   fg_iou_threshold.  Each positive adds 1 to examine[t][bin], its gt3 row to sums[t][bin][3] and the row's squares to squared[t][bin][3],
+ *   in frame, class, anchor order: the reference's sequential float64 sums, bit for bit.  usable[t] += the class's boxes whose maximum IoU
+ *   over all anchors is > fg_iou_threshold.  The state (int64 / float64 device arrays) carries over from batch to batch.
+ * vd3d_anchor_prior_accumulate: device pointers except the two _host arrays; workspace: vd3d_anchor_prior_workspace_bytes(N, n_bins, B, T,
+ *   K_total) bytes of device memory (negative: error code).  A copy of the offsets, a memset and two launches; no synchronisation.
+ * vd3d_anchor_prior_host: the same accumulation on host arrays in the reference's loop order (the parity checker); it also checks that
+ *   order lists every anchor once, ascending within each bin. */
+long long vd3d_anchor_prior_workspace_bytes(int N, int n_bins, int B, int T, int K_total);
+int vd3d_anchor_prior_accumulate(const float* anchors, const int* order, const int* bin_start_host, int N, int n_bins,
+                                 const int* offsets_host, int B, int T, const void* boxes, int boxes_f64, const double* gt3, int K_total,
+                                 double fg_iou_threshold, long long* examine, double* sums, double* squared, long long* usable,
+                                 void* workspace, long long workspace_bytes, void* stream);
+int vd3d_anchor_prior_host(const float* anchors, const int* order, const int* bin_start, int N, int n_bins, const int* offsets, int B,
+                           int T, const void* boxes, int boxes_f64, const double* gt3, int K_total, double fg_iou_threshold,
+                           long long* examine, double* sums, double* squared, long long* usable);
+
 #ifdef __cplusplus
 }
 #endif

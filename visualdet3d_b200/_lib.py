@@ -127,6 +127,9 @@ _SIGS = {
     "vd3d_stereo_bm_host": (I, [P, P, I, I, P]),
     "vd3d_disparity_block_max_host": (I, [P, I, I, I, P]),
     "vd3d_velo_disparity_host": (I, [P, I, I, P, P, P, c_double, I, I, P]),
+    "vd3d_anchor_prior_workspace_bytes": (c_longlong, [I, I, I, I, I]),
+    "vd3d_anchor_prior_accumulate": (I, [P, P, P, I, I, P, I, I, P, I, P, I, c_double, P, P, P, P, P, c_longlong, P]),
+    "vd3d_anchor_prior_host": (I, [P, P, P, I, I, P, I, I, P, I, P, I, c_double, P, P, P, P]),
 }
 
 

@@ -44,7 +44,7 @@ __device__ __forceinline__ float sign0(float x) { return x > 0.f ? 1.f : (x < 0.
 // Both callers compile with -fmad=false, so calc_iou rounds like torch's fp32 elementwise ops and the assignment is the reference's.
 
 // calc_iou(a, b) (R/networks/utils/utils.py:83-100), one pair, the reference's expression order
-__device__ __forceinline__ float calc_iou(const float* a, const float* b) {
+__host__ __device__ __forceinline__ float calc_iou(const float* a, const float* b) {
     const float area = (b[2] - b[0]) * (b[3] - b[1]);
     float iw = fminf(a[2], b[2]) - fmaxf(a[0], b[0]);
     float ih = fminf(a[3], b[3]) - fmaxf(a[1], b[1]);
@@ -53,6 +53,20 @@ __device__ __forceinline__ float calc_iou(const float* a, const float* b) {
     float ua = ((a[2] - a[0]) * (a[3] - a[1]) + area) - iw * ih;
     ua = fmaxf(ua, 1e-8f);
     const float inter = iw * ih;
+    return inter / ua;
+}
+
+// calc_iou of float32 anchors against float64 boxes, as torch promotes it: the anchor's coordinates widen exactly, its own area is still
+// rounded in float32, everything else is float64.  Callers compile with -fmad=false.
+__host__ __device__ __forceinline__ double calc_iou(const float* a, const double* b) {
+    const double area = (b[2] - b[0]) * (b[3] - b[1]);
+    double iw = fmin((double)a[2], b[2]) - fmax((double)a[0], b[0]);
+    double ih = fmin((double)a[3], b[3]) - fmax((double)a[1], b[1]);
+    iw = fmax(iw, 0.0);
+    ih = fmax(ih, 0.0);
+    double ua = ((double)((a[2] - a[0]) * (a[3] - a[1])) + area) - iw * ih;
+    ua = fmax(ua, 1e-8);
+    const double inter = iw * ih;
     return inter / ua;
 }
 
