@@ -95,6 +95,18 @@ int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* const* in_lo, 
                      const int* res_H, const int* res_W, int res_cs, int res_co,
                      const void* const* out, const void* const* out_hi16, const void* const* out_lo16,
                      int Cout, int out_cs, int out_co, int relu, int passes, int bn, void* stream);
+/* ConvTranspose2d(kernel 4, stride 2, padding 1) + folded BN / bias [+ ReLU] on the fp16-split engine (the CenterNet up-sampling of the
+ * ResNet KM3D / MonoFlex core, R/detectors/KM3D_core.py:37-47), as its four sub-pixel phases in ONE persistent launch: output pixel
+ * (2m + r, 2n + s) of phase (r, s) is a stride-1 2x2 conv over the H x W input,
+ *   y[2m+r][2n+s][co] = sum_{a,c in {0,1}} sum_ci x[m+r-1+a][n+s-1+c][ci] * Wt[ci][co][3-r-2a][3-s-2c]   (out-of-range input rows / columns = 0)
+ *   in_hi / in_lo     : fp16 NHWC planes [B][H][W] (pitch in_cs, channel offset in_co), 16-byte aligned
+ *   w_hi / w_lo       : fp16 [4 Cout][4 cin_pad], cin_pad = Cin rounded up to 64: row (2r + s) Cout + co, column (2a + c) cin_pad + ci; one
+ *                       power-of-two scale for all phases, undone by out_scale
+ *   out / out_hi16 / out_lo16: [B][2H][2W] NHWC (pitch out_cs, offset out_co), fp32 and / or its fp16 planes, as vd3d_conv2d_tc16
+ * Cin % 8 == 0, Cout % 16 == 0; bn <= 0: the library's tile policy.  Four taps of MMA work per output pixel. */
+int vd3d_convtranspose2d_tc16(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                              const void* w_hi, const void* w_lo, float out_scale, const float* bias,
+                              float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
 /* Few-channel KHxKW convolution (the ResNet / DLA stem: conv1 7x7 stride 2, R/backbones/resnet.py:120,186) on the tensor cores.
  * The image is held as fp16 (hi, lo) planes [B][H][Wp][4] (pixel x at column x + pad, zeros elsewhere: the buffer must be
  * zero-initialised once); Wp = vd3d_stem_row_pitch(W, KW, stride, pad).  vd3d_image_to_h16_rows fills the planes from an

@@ -14,7 +14,9 @@ CASES = [("Yolo3D", "configs[0] shape on the GPU: Yolo3D ResNet-18 (DCNv2 head)"
          ("GroundAwareYolo3D", "configs[2]: Ground-aware Mono3D (GAC head, ResNet-101), batch 8 mono 288x1280", 8, 288, 1280,
           lambda: build_synthetic_mono3d("GroundAwareYolo3D", seed=0)[0]),
          ("MonoFlex", "configs[3]: MonoFlex DLA-34 + DCNv2, batch 8, 384x1280", 8, 384, 1280, lambda: build_synthetic_monoflex(seed=0)[0]),
-         ("KM3D", "configs[3]: KM3D DLA-34 + DCNv2, batch 8, 384x1280", 8, 384, 1280, lambda: build_synthetic_monoflex(seed=0, name="KM3D")[0])]
+         ("KM3D", "configs[3]: KM3D DLA-34 + DCNv2, batch 8, 384x1280", 8, 384, 1280, lambda: build_synthetic_monoflex(seed=0, name="KM3D")[0]),
+         ("KM3D-resnet18", "KM3D_example: ResNet-18 + transposed-conv up-sampling, batch 8, 384x1280", 8, 384, 1280,
+          lambda: build_synthetic_monoflex(seed=0, name="KM3D", backbone="resnet18")[0])]
 for name, desc, B, H, W, mk in CASES:
     if only and name not in only:
         continue

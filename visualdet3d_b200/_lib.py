@@ -54,6 +54,7 @@ _SIGS = {
     "vd3d_tc_pick_bn_persistent": (I, [I]),
     "vd3d_conv2d_tc": (I, [P, P, I, I, I, I, I, I, P, P, P, I, I, I, I, P, I, I, P, P, I, I, I, I, I, I, P]),
     "vd3d_conv2d_tc16": (I, [I, P, P, P, P, I, I, I, I, P, P, F, P, I, I, I, I, I, P, P, P, P, P, I, I, P, P, P, I, I, I, I, I, I, P]),
+    "vd3d_convtranspose2d_tc16": (I, [P, P, I, I, I, I, I, I, P, P, F, P, P, P, P, I, I, I, I, I, P]),
     "vd3d_stem_row_pitch": (I, [I, I, I, I]),
     "vd3d_image_to_h16_rows": (I, [P, I, I, I, I, P, P, I, I, P]),
     "vd3d_conv2d_tc16_stem": (I, [P, P, I, I, I, I, I, I, I, I, I, P, P, F, P, P, P, P, I, I, I, I, P]),

@@ -282,11 +282,11 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                     unit_tile(p, u, mt_units, mu, nt);
                     const TcGeom geo = tile_geom(p, mu);
                     const int b = geo.b;
-                    const int wi0 = geo.tw * TC_TW * p.stride_w - p.pad_w, hi0 = geo.th * TC_TH * p.stride - p.pad;
+                    const int wi0 = geo.tw * TC_TW * p.stride_w - geo.pad_w, hi0 = geo.th * TC_TH * p.stride - geo.pad_h;
                     const CUtensorMap* mA = &mapA;
                     const CUtensorMap* mAlo = &mapAlo;
                     if constexpr (LV) { mA = &lmaps.a[geo.lvl]; mAlo = &lmaps.alo[geo.lvl]; }
-                    const int n0 = nt * BN;
+                    const int n0 = nt * BN + geo.w_row;               // (weight rows only: the epilogue's columns are nt * BN ..)
                     int tap = 0, kh = 0, kw = 0, c0 = 0;
                     for (int kb = 0; kb < KB; ++kb, ++it) {
                         int slot = s;
@@ -571,6 +571,8 @@ static int fit_bn(int bn) {
 // One conv as the entries describe it: L input tensors of one channel layout (L > 1: a multi-level launch, fp16 operands only), the weights
 // and the epilogue.  Level l reads in[l] / in_lo[l] [B][H[l]][W[l]]; its outputs and fp32 residual lie out_off[l] / res_off[l] pixels after
 // level 0's (L > 1); res_W[l] > 0: its fp32 residual is [B][res_H[l]][res_W[l]] at half the output size, read nearest-upsampled.
+// convt: the four sub-pixel phases of a 4x4 / stride-2 / pad-1 transposed conv (vd3d_convtranspose2d_tc16): L = 4 levels over one input,
+// 2x2 taps each, weights [4 Cout][4 cin_pad] (phase l = 2 r + s owns rows l Cout ..), output [B][2 H][2 W].
 struct ConvSpec {
     int f16, L, B, Cin, in_cs, in_co;
     const void* in[TC_MAX_LEVELS]; const void* in_lo[TC_MAX_LEVELS];
@@ -581,7 +583,15 @@ struct ConvSpec {
     const float* res; const void* res_h16_hi; const void* res_h16_lo; int res_cs, res_co;
     float* out; float* out_lo; void* out_h16_hi; void* out_h16_lo;
     int Cout, out_cs, out_co, relu, passes, bn;
+    int convt;
 };
+
+// output size of level l: the conv's, or (convt) the input's -- each phase writes one pixel of every 2x2 output cell
+static void spec_out_hw(const ConvSpec& s, int l, int& Ho, int& Wo) {
+    if (s.convt) { Ho = s.H[l]; Wo = s.W[l]; return; }
+    Ho = (s.H[l] + 2 * s.pad - s.dil * (s.KH - 1) - 1) / s.stride + 1;
+    Wo = (s.W[l] + 2 * s.pad - s.dil * (s.KW - 1) - 1) / s.stride + 1;
+}
 
 static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
     const int f16 = s.f16, B = s.B, H = s.H[0], W = s.W[0], Cin = s.Cin, KH = s.KH, KW = s.KW, pad = s.pad, dil = s.dil, stride = s.stride;
@@ -606,7 +616,8 @@ static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
         if (f16 && passes == 3) {
             int mt_all = 0;
             for (int l = 0; l < s.L; ++l) {
-                const int Ho_ = (s.H[l] + 2 * pad - dil * (KH - 1) - 1) / stride + 1, Wo_ = (s.W[l] + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+                int Ho_, Wo_;
+                spec_out_hw(s, l, Ho_, Wo_);
                 mt_all += cdiv(Wo_, TC_TW) * cdiv(Ho_, TC_TH) * B;
             }
             BN = pick_bn_cost(Cout, mt_all);
@@ -618,7 +629,7 @@ static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
     memset(&p, 0, sizeof(p));
     VD3D_REQUIRE(stride >= 1 && stride <= 4, "conv2d_tc: stride must be in [1, 4]");
     p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.KH = KH; p.KW = KW; p.pad = pad; p.dil = dil; p.stride = stride;
-    p.Ho = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1; p.Wo = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+    spec_out_hw(s, 0, p.Ho, p.Wo);
     VD3D_REQUIRE(p.Ho > 0 && p.Wo > 0, "conv2d_tc: empty output");
     p.Cout = Cout; p.BN = BN; p.passes = passes; p.f16 = f16; p.bk = bk; p.cin_pad = (Cin + bk - 1) / bk * bk; p.out_scale = s.out_scale;
     p.tiles_w = cdiv(p.Wo, TC_TW); p.tiles_h = cdiv(p.Ho, TC_TH);
@@ -633,8 +644,14 @@ static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
         int mt = 0;
         for (int l = 0; l < s.L; ++l) {
             TcLevel& v = p.lv[l];
-            v.Ho = (s.H[l] + 2 * pad - dil * (KH - 1) - 1) / stride + 1; v.Wo = (s.W[l] + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
+            spec_out_hw(s, l, v.Ho, v.Wo);
             VD3D_REQUIRE(v.Ho > 0 && v.Wo > 0, "conv2d_tc16: level %d has an empty output", l);
+            v.pad_h = pad; v.pad_w = pad; v.w_row = 0; v.up = 0;
+            if (s.convt) {
+                // phase (r, s) = (l >> 1, l & 1): y[2m + r][2n + s] = sum_{a,b} x[m + r - 1 + a][n + s - 1 + b] W_rs[a][b]
+                const int r = l >> 1, c = l & 1;
+                v.pad_h = 1 - r; v.pad_w = 1 - c; v.w_row = l * Cout; v.up = 1;
+            }
             v.tiles_w = cdiv(v.Wo, TC_TW); v.tiles_h = cdiv(v.Ho, TC_TH);
             v.m_begin = mt;
             mt += v.tiles_w * v.tiles_h * B;
@@ -695,8 +712,9 @@ static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
     int rc;
     if ((rc = make_map_act(&mA, s.in[0], B, H, W, Cin, s.in_cs, s.in_co, esize, TC_TW, TC_TH, stride))) return rc;
     if ((rc = make_map_act(&mAlo, s.in_lo[0] ? s.in_lo[0] : s.in[0], B, H, W, Cin, s.in_cs, s.in_co, esize, TC_TW, TC_TH, stride))) return rc;
-    if ((rc = make_map_wgt(&mWhi, s.w_hi, Cout, K, BN, esize))) return rc;
-    if ((rc = make_map_wgt(&mWlo, s.w_lo ? s.w_lo : s.w_hi, Cout, K, BN, esize))) return rc;
+    const int w_rows = s.convt ? 4 * Cout : Cout;
+    if ((rc = make_map_wgt(&mWhi, s.w_hi, w_rows, K, BN, esize))) return rc;
+    if ((rc = make_map_wgt(&mWlo, s.w_lo ? s.w_lo : s.w_hi, w_rows, K, BN, esize))) return rc;
     if (s.L == 1) return tcp_launch(p, mA, mAlo, mWhi, mWlo, stream);
     TcLevelMaps lm;
     for (int l = 0; l < s.L; ++l) {
@@ -763,6 +781,33 @@ extern "C" int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* con
     s.res_h16_hi = res_hi16 ? res_hi16[0] : nullptr; s.res_h16_lo = res_lo16 ? res_lo16[0] : nullptr;
     s.out = out ? (float*)out[0] : nullptr; s.out_h16_hi = out_hi16 ? (void*)out_hi16[0] : nullptr; s.out_h16_lo = out_lo16 ? (void*)out_lo16[0] : nullptr;
     s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = passes; s.bn = bn;
+    return conv2d_tc_launch(s, stream);
+}
+
+// ConvTranspose2d(k = 4, s = 2, p = 1) as its four sub-pixel phases, each a stride-1 2x2 conv over the H x W input, in ONE persistent launch:
+//   y[b, 2m + r, 2n + s, co] = sum_{a, c in {0,1}} sum_ci x[b, m + r - 1 + a, n + s - 1 + c, ci] * Wt[ci, co, 3 - r - 2a, 3 - s - 2c]
+// (rows / columns outside the input read as zero: TMA out-of-bounds fill).  Four taps of MMA work per output pixel, against 16 for a
+// zero-inserted 4x4 conv.  w_hi / w_lo: [4 Cout][4 cin64] fp16, phase 2 r + s in rows (2 r + s) Cout .., k = (2 a + c) cin64 + ci
+// (cin64 = Cin rounded up to 64), scaled by one power of two for all phases (out_scale undoes it).  Output [B][2H][2W][out_cs] at channel
+// out_co: fp32 and / or fp16 (hi, lo) planes; epilogue bias / ReLU as vd3d_conv2d_tc16.
+extern "C" int vd3d_convtranspose2d_tc16(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                                         const void* w_hi, const void* w_lo, float out_scale, const float* bias,
+                                         float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream) {
+    VD3D_REQUIRE(in_hi && in_lo && w_hi && w_lo && (out || out_hi16) && (!out_hi16 == !out_lo16) && B > 0 && H > 0 && W > 0,
+                 "convtranspose2d_tc16: input planes, weights, a non-empty size and an output are required");
+    VD3D_REQUIRE(Cout % 16 == 0 && Cout >= 16, "convtranspose2d_tc16: Cout must be a multiple of 16 (got %d)", Cout);
+    VD3D_REQUIRE(((((uintptr_t)in_hi | (uintptr_t)in_lo) & 15) == 0), "convtranspose2d_tc16: 16-byte aligned input planes are required");
+    ConvSpec s;
+    memset(&s, 0, sizeof(s));
+    s.f16 = 1; s.L = 4; s.convt = 1; s.B = B; s.Cin = Cin; s.in_cs = in_cs; s.in_co = in_co;
+    for (int l = 0; l < 4; ++l) {
+        s.in[l] = in_hi; s.in_lo[l] = in_lo; s.H[l] = H; s.W[l] = W;
+        s.out_off[l] = (long long)(l >> 1) * 2 * W + (l & 1);
+    }
+    s.w_hi = w_hi; s.w_lo = w_lo; s.out_scale = out_scale; s.bias = bias;
+    s.KH = 2; s.KW = 2; s.pad = 1; s.dil = 1; s.stride = 1;
+    s.out = out; s.out_h16_hi = out_hi16; s.out_h16_lo = out_lo16;
+    s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = 3; s.bn = bn;
     return conv2d_tc_launch(s, stream);
 }
 

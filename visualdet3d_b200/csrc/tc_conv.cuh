@@ -17,6 +17,9 @@ constexpr int TC_CONSUMERS = 256;
 constexpr int TC_MAX_LEVELS = 5;
 struct TcLevel {
     int Ho, Wo, tiles_w, tiles_h, m_begin, res_H, res_W;
+    int pad_h, pad_w;        // tap origin: input row / column of tap (0, 0) for output (0, 0) is (-pad_h, -pad_w)
+    int w_row;               // first weight row of the level (the levels of a transposed conv each own Cout rows of one matrix)
+    int up;                  // 1: output pixel (ho, wo) of image b is pixel (2 ho, 2 wo) of a [B][2 Ho][2 Wo] tensor, plus pix_off (sub-pixel phase)
     long long pix_off, res_off;
 };
 
@@ -53,6 +56,8 @@ struct TcParams {
     // Multi-level launch (vd3d_conv2d_tc16 with L > 1; n_levels = 0: one tensor).  The M tiles of the levels are concatenated: level l owns tiles
     // [m_begin, m_begin + B * tiles_h * tiles_w) and reads its own activation maps; its output (residual) pixel p sits at pixel pix_off + p
     // (res_off + p, or of the [B][res_H][res_W] half-resolution residual when res_W > 0) of the `out` (`res`) pointers.
+    // vd3d_convtranspose2d_tc16 runs the four sub-pixel phases of a 4x4 / stride-2 transposed conv as four levels over ONE input: each with
+    // its own tap origin, weight rows and interleaved output pixels (TcLevel::pad_h / pad_w / w_row / up).
     int n_levels;
     TcLevel lv[TC_MAX_LEVELS];
 };
@@ -198,10 +203,13 @@ template <int V> using tc_int = std::integral_constant<int, V>;
 // several groups in flight before it computes the first.
 // Output geometry of M tile mu: tile column / row, image, the output size, and the pixel offsets of the output and the residual (the level's,
 // in a multi-level launch; zero otherwise).  The level table is indexed with compile-time indices only, so it stays in parameter space.
-struct TcGeom { int tw, th, b, Ho, Wo, lvl, res_H, res_W; long long pix_off, res_off; };
+// Tap origin (pad_h, pad_w), first weight row (w_row) and output pixel map (up) of the tile's level: p.pad / p.pad_w, 0 and 0 outside
+// multi-level launches.
+struct TcGeom { int tw, th, b, Ho, Wo, lvl, res_H, res_W, pad_h, pad_w, w_row, up; long long pix_off, res_off; };
 __device__ __forceinline__ TcGeom tile_geom(const TcParams& p, int mu) {
     TcGeom g;
     g.lvl = 0; g.Ho = p.Ho; g.Wo = p.Wo; g.res_H = p.res_up_H; g.res_W = p.res_up_W; g.pix_off = 0; g.res_off = 0;
+    g.pad_h = p.pad; g.pad_w = p.pad_w; g.w_row = 0; g.up = 0;
     int tiles_w = p.tiles_w, tiles_h = p.tiles_h;
     if (p.n_levels > 0) {
 #pragma unroll
@@ -209,6 +217,7 @@ __device__ __forceinline__ TcGeom tile_geom(const TcParams& p, int mu) {
             if (i < p.n_levels && mu >= p.lv[i].m_begin) {
                 g.lvl = i; g.Ho = p.lv[i].Ho; g.Wo = p.lv[i].Wo; g.res_H = p.lv[i].res_H; g.res_W = p.lv[i].res_W;
                 g.pix_off = p.lv[i].pix_off; g.res_off = p.lv[i].res_off; tiles_w = p.lv[i].tiles_w; tiles_h = p.lv[i].tiles_h;
+                g.pad_h = p.lv[i].pad_h; g.pad_w = p.lv[i].pad_w; g.w_row = p.lv[i].w_row; g.up = p.lv[i].up;
             }
 #pragma unroll
         for (int i = 0; i < TC_MAX_LEVELS; ++i)
@@ -219,9 +228,10 @@ __device__ __forceinline__ TcGeom tile_geom(const TcParams& p, int mu) {
     return g;
 }
 // Output pixel of (b, ho, wo), and its residual pixel: the same pixel, or (res_W > 0) pixel (ho >> 1, wo >> 1) of the half-resolution
-// residual, i.e. the nearest-neighbour x2 upsampling of the FPN top-down path fused into the residual read.
+// residual, i.e. the nearest-neighbour x2 upsampling of the FPN top-down path fused into the residual read.  A sub-pixel phase level (up = 1)
+// writes pixel (2 ho, 2 wo) of the [B][2 Ho][2 Wo] output; its pix_off (2 W r + s for phase (r, s)) picks the phase's pixel of each 2x2 cell.
 __device__ __forceinline__ long long tcp_out_pix(const TcGeom& g, int ho, int wo) {
-    return g.pix_off + ((long long)g.b * g.Ho + ho) * g.Wo + wo;
+    return g.pix_off + ((((long long)g.b * g.Ho + ho) * g.Wo) << (2 * g.up)) + ((long long)wo << g.up);
 }
 __device__ __forceinline__ long long tcp_res_pix(const TcGeom& g, int ho, int wo) {
     return g.res_off + (g.res_W > 0 ? ((long long)g.b * g.res_H + (ho >> 1)) * g.res_W + (wo >> 1) : ((long long)g.b * g.Ho + ho) * g.Wo + wo);

@@ -1,4 +1,4 @@
-"""`MonoFlex` / `KM3D` — DLA-34 + DCNv2 up-sampling + CenterNet-style heads on the GPU
+"""`MonoFlex` / `KM3D` — DLA-34 + DCNv2 up-sampling, or ResNet-18 / 34 + three transposed convs, + CenterNet-style heads on the GPU
 (drop-ins for R/detectors/KM3D.py:16-96, core R/detectors/KM3D_core.py:10-58, heads R/heads/km3d_head.py, monoflex_head.py).
 
 Protocol: ``module([image[1,3,H,W], P2[1,3,4]])`` -> ``(scores[K], bboxes[K,11], cls[K])``; a 3-element list is the training
@@ -19,6 +19,7 @@ from ..plugin import DETECTOR_DICT
 from . import modules as M
 from .base import NativeDetector, synth_load
 from .dla import DLAP, DLARunner, DLASegUpsampleP, DLAUpRunner
+from .stereo3d import ResNetRunner
 
 
 def _peak_capacity(n_cells: int) -> int:
@@ -32,16 +33,42 @@ def _peak_capacity(n_cells: int) -> int:
 
 
 class KM3DCoreP(M.Holder):
-    """keys of KM3DCore (R/detectors/KM3D_core.py:10-50) for the DLA backbone."""
+    """keys of KM3DCore (R/detectors/KM3D_core.py:10-50).  The backbone follows the reference's `build_backbone`
+    (R/backbones/__init__.py:5-13): `name` missing means 'resnet'.
+      * 'dla' / 'dlanet' (Monoflex_example): DLA-34, then DLASegUpsample (DCNv2 IDAUp) to 64 channels at 1/4 resolution.
+      * 'resnet' (KM3D_example, which names no backbone; Monoflex_example's commented-out alternative): ResNet-18 / 34 whose last stage
+        (512 channels at 1/32) feeds the "baseline" up-sampling `deconv_layers` = three ConvTranspose2d(4, stride 2, padding 1, no bias)
+        + BatchNorm2d + ReLU, 512 -> 256 -> 256 -> 256, to 1/4 resolution (KM3D_core.py:34-47).
+    The reference's own KM3DCore reads backbone_arguments['name'] directly, so it needs the name spelled out; a name-less config builds
+    here exactly what it builds with name='resnet'.  ResNet deeper than 34 is refused: the reference wires 2024 input channels into the
+    first transposed conv for it (KM3D_core.py:19-20), which cannot take the 2048-channel last stage."""
 
     def __init__(self, backbone_arguments):
         super().__init__()
         args = dict(backbone_arguments)
-        name = str(args.get("name", "dlanet")).lower()
-        if name not in ("dla", "dlanet"):
-            raise NotImplementedError("KM3DCore on the B200 path supports the DLA backbone (the shipped KM3D / MonoFlex configs)")
-        self.backbone = DLAP(**args)
-        self.deconv_layers = DLASegUpsampleP(input_channels=[16, 32, 64, 128, 256, 512], down_ratio=4, final_kernel=1, last_level=5, out_channel=64)
+        name = str(args.get("name", "resnet")).lower()
+        self.backbone_name = "resnet" if name == "resnet" else "dla"
+        if name in ("dla", "dlanet"):
+            self.backbone = DLAP(**args)
+            self.deconv_layers = DLASegUpsampleP(input_channels=[16, 32, 64, 128, 256, 512], down_ratio=4, final_kernel=1, last_level=5, out_channel=64)
+        elif name == "resnet":
+            args.pop("name", None)
+            depth = int(args.get("depth", 0))
+            if depth > 34:
+                raise ValueError(f"KM3DCore with ResNet-{depth}: the reference's core gives the first transposed conv 2024 input channels "
+                                 "for depth > 34 (KM3D_core.py:19-20) and cannot run the 2048-channel last stage; use depth 18 or 34")
+            out_indices = tuple(args.get("out_indices", (-1, 0, 1, 2, 3)))
+            if not out_indices or out_indices[-1] != 3:
+                raise ValueError(f"KM3DCore with ResNet: the last out_indices entry must be stage 3 (the core up-samples the last returned "
+                                 f"map, which must be the 512-channel stage 3), got {out_indices}")
+            self.backbone = M.ResNetP(**args)
+            feat = 256
+            self.deconv_layers = M.seq(
+                nn.ConvTranspose2d(self.backbone.out_channels(3), feat, 4, stride=2, padding=1, bias=False), nn.BatchNorm2d(feat), nn.ReLU(inplace=True),
+                nn.ConvTranspose2d(feat, feat, 4, stride=2, padding=1, bias=False), nn.BatchNorm2d(feat), nn.ReLU(inplace=True),
+                nn.ConvTranspose2d(feat, feat, 4, stride=2, padding=1, bias=False), nn.BatchNorm2d(feat), nn.ReLU(inplace=True))
+        else:
+            raise NotImplementedError(f"KM3DCore on the native path takes the DLA-34 or ResNet-18 / 34 backbone, not {name!r}")
         for m in self.deconv_layers.modules():
             if isinstance(m, nn.ConvTranspose2d):
                 nn.init.normal_(m.weight, std=0.001)
@@ -95,7 +122,13 @@ class _CenterNetBase(NativeDetector):
         self.topk = 100
 
     def build_plan(self, dev) -> dict:
-        pl = dict(dla=DLARunner(self.core.backbone, dev, first_used_level=self.core.deconv_layers.first_level), up=DLAUpRunner(self.core.deconv_layers, dev))
+        if self.core.backbone_name == "resnet":
+            dl = self.core.deconv_layers
+            pl = dict(resnet=ResNetRunner(self.core.backbone, dev),
+                      deconv=[E.ConvTransposeLayer(dl[i].weight, E.bn_dict(dl[i + 1]), relu=True, device=dev) for i in (0, 3, 6)])
+        else:
+            pl = dict(dla=DLARunner(self.core.backbone, dev, first_used_level=self.core.deconv_layers.first_level),
+                      up=DLAUpRunner(self.core.deconv_layers, dev))
         hl = self.bbox_head.head_layers
         names = list(hl.keys())
         # one stem conv for all heads: weights / biases concatenated along Cout
@@ -127,9 +160,12 @@ class _CenterNetBase(NativeDetector):
         ar = self._arena
         B, _, H, W = images.shape
         if H % 32 or W % 32:
-            raise Vd3dError(f"{type(self).__name__}: image size {H}x{W} must be a multiple of 32 (DLA-34 has 5 stride-2 levels)")
-        ys = pl["dla"].run(images, ar)
-        feat = pl["up"].run(ys, ar)                       # [B, H/4, W/4, 64]
+            raise Vd3dError(f"{type(self).__name__}: image size {H}x{W} must be a multiple of 32 (the backbone has 5 stride-2 levels)")
+        if "resnet" in pl:
+            feat = self._resnet_core(pl, images, ar)      # [B, H/4, W/4, 256]
+        else:
+            ys = pl["dla"].run(images, ar)
+            feat = pl["up"].run(ys, ar)                   # [B, H/4, W/4, 64]
         self._hook("features", feat)
         dev = images.device
         if pl["stem"].engine != "simt":
@@ -147,6 +183,22 @@ class _CenterNetBase(NativeDetector):
             layer(stem.slice(cin_off, self.bbox_head.head_features), out.slice(cout_off, n_pad))
         self._hook("heads", out)
         return out
+
+    def _resnet_core(self, pl, images, ar) -> E.Act:
+        """KM3DCore.forward for a ResNet backbone (KM3D_core.py:52-58): deconv_layers(backbone(image)[-1]).  The transposed convs read and
+        (in planes mode) write fp16 planes only: each one's consumer is the next transposed conv or the head stem, all tensor-core convs."""
+        rn, dc = pl["resnet"], pl["deconv"]
+        B, dev = images.shape[0], images.device
+        planes = E.planes_mode_ok()
+        x = rn.run(images, ar, tag="bb", f32_outputs=[not planes] * len(rn.p.out_indices))[-1]
+        if rn.out_lo_stale[-1]:
+            E.split_lo(x)
+        for i, layer in enumerate(dc):
+            last = i == len(dc) - 1
+            f32 = not planes or (last and pl["stem"].engine != "tc16")
+            Ho, Wo = layer.out_hw(x.H, x.W)
+            x = layer(x, ar.act(f"core.deconv{i}", (B, Ho, Wo, layer.Cout), dev, lo=True), f32_out=f32)
+        return x
 
     def launch(self, images, P2):
         images, P2 = self._device_inputs((images, "image"), (P2, "P2"))
@@ -243,9 +295,44 @@ def monoflex_cfg(obj_types=("Car", "Pedestrian", "Cyclist"), name: str = "MonoFl
     return det
 
 
-def build_synthetic_monoflex(seed: int = 0, name: str = "MonoFlex"):
-    """Random-init (seeded, de-degenerated) MonoFlex / KM3D: returns (detector, state_dict, cfg)."""
-    cfg = km3d_cfg() if name == "KM3D" else monoflex_cfg(name=name)
+def km3d_example_cfg(obj_types=("Car", "Pedestrian", "Cyclist"), score_thr: float = 0.3):
+    """cfg.detector of R/config/KM3D_example:127-165 as shipped, with pretrained=False: no backbone name (a ResNet-18 whose stage 3 feeds
+    the transposed-conv up-sampling), 256 head input features, 64 head features."""
+    from ..synth import AttrDict
+    obj_types = list(obj_types)
+    det = AttrDict(obj_types=obj_types, name="KM3D")
+    det.backbone = AttrDict(depth=18, pretrained=False, frozen_stages=-1, num_stages=4, out_indices=(3,), norm_eval=False,
+                            dilations=(1, 1, 1, 1))
+    det.head = AttrDict(num_classes=len(obj_types), num_joints=9, max_objects=32,
+                        layer_cfg=AttrDict(input_features=256, head_features=64,
+                                           head_dict={"hm": len(obj_types), "wh": 2, "hps": 18, "rot": 8, "dim": 3, "prob": 1, "reg": 2,
+                                                      "hm_hp": 9, "hp_offset": 2}),
+                        loss_cfg=AttrDict(gamma=2.0, rampup_length=100, output_w=1280 // 4),
+                        test_cfg=AttrDict(score_thr=score_thr))
+    det.loss = det.head.loss_cfg
+    return det
+
+
+def monoflex_resnet_cfg(obj_types=("Car", "Pedestrian", "Cyclist")):
+    """cfg.detector of R/config/Monoflex_example with its commented-out ResNet-18 backbone (name='resnet', depth=18, out_indices=(3,))
+    and the 256 head input features the transposed-conv up-sampling produces."""
+    from ..synth import AttrDict
+    det = monoflex_cfg(obj_types)
+    det.backbone = AttrDict(name="resnet", depth=18, out_indices=(3,), pretrained=False)
+    det.head.layer_cfg.input_features = 256
+    return det
+
+
+def build_synthetic_monoflex(seed: int = 0, name: str = "MonoFlex", backbone: str = "dla34"):
+    """Random-init (seeded, de-degenerated) MonoFlex / KM3D: returns (detector, state_dict, cfg).  backbone 'dla34': `km3d_cfg` /
+    `monoflex_cfg`; 'resnet18': `km3d_example_cfg` (score_thr 0.1, as `km3d_cfg`, to keep detections with the synthetic weights) /
+    `monoflex_resnet_cfg`."""
+    if backbone == "resnet18":
+        cfg = km3d_example_cfg(score_thr=0.1) if name == "KM3D" else monoflex_resnet_cfg()
+    elif backbone == "dla34":
+        cfg = km3d_cfg() if name == "KM3D" else monoflex_cfg(name=name)
+    else:
+        raise ValueError(f"backbone must be 'dla34' or 'resnet18', got {backbone!r}")
     det = DETECTOR_DICT[name](cfg)
     sd = synth_load(det, seed)
     return det, sd, cfg

@@ -359,6 +359,75 @@ class ConvLayer:
         return out
 
 
+def fold_bn_transposed(weight, bias, bn: Optional[Dict[str, torch.Tensor]], eps: float = 1e-5):
+    """ConvTranspose2d (+bias) followed by eval-mode BatchNorm -> (weight', bias') in float64.  The transposed weight is [Cin, Cout, KH, KW]:
+    the BN scale multiplies dim 1 (the output channel), not dim 0 as in `fold_bn`."""
+    w, b = fold_bn(weight.detach().transpose(0, 1), bias, bn, eps)
+    return w.transpose(0, 1).contiguous(), b
+
+
+def convtranspose_phase_matrix(w: torch.Tensor, cin_pad: int) -> torch.Tensor:
+    """Folded float64 ConvTranspose2d(4, stride 2, padding 1) weight [Cin, Cout, 4, 4] -> the four sub-pixel phase convs as one
+    [4 Cout][4 cin_pad] matrix (the weight operand of vd3d_convtranspose2d_tc16): output pixel (2m + r, 2n + s) is the 2x2 conv
+    y = sum_{a, c} x[m + r - 1 + a, n + s - 1 + c] . w[:, :, 3 - r - 2a, 3 - s - 2c], so row (2r + s) Cout + co, column (2a + c) cin_pad + ci
+    holds w[ci, co, 3 - r - 2a, 3 - s - 2c] (zero for ci >= Cin)."""
+    Cin, Cout, KH, KW = w.shape
+    assert (KH, KW) == (4, 4) and cin_pad >= Cin
+    m = torch.zeros(4, Cout, 4, cin_pad, dtype=torch.float64)
+    for r in (0, 1):
+        for s in (0, 1):
+            for a in (0, 1):
+                for c in (0, 1):
+                    m[2 * r + s, :, 2 * a + c, :Cin] = w[:, :, 3 - r - 2 * a, 3 - s - 2 * c].t().double()
+    return m.reshape(4 * Cout, 4 * cin_pad)
+
+
+class ConvTransposeLayer:
+    """ConvTranspose2d(kernel 4, stride 2, padding 1) + folded eval-mode BatchNorm [+ ReLU] (the CenterNet up-sampling of the ResNet KM3D /
+    MonoFlex core, R/detectors/KM3D_core.py:37-47) as its four sub-pixel phase convs in one launch of the fp16-split engine
+    (vd3d_convtranspose2d_tc16): 2x2 taps per output pixel.  Runs on that engine only; under any other VD3D_CONV_ENGINE the layer
+    refuses to build."""
+
+    def __init__(self, weight, bn=None, bias=None, relu=True, device="cuda"):
+        Cin, Cout, KH, KW = weight.shape
+        eng = conv_engine_default()
+        if eng != "tc16":
+            raise _lib.Vd3dError(f"ConvTransposeLayer: the transposed conv runs on the fp16-split tensor-core engine only "
+                                 f"(VD3D_CONV_ENGINE=tc16), not {eng!r}")
+        if (KH, KW) != (4, 4) or Cin % 8 or Cout % 16:
+            raise _lib.Vd3dError(f"ConvTransposeLayer: needs a 4x4 kernel, Cin % 8 == 0 and Cout % 16 == 0 (got {Cin} -> {Cout}, {KH}x{KW})")
+        w, b = fold_bn_transposed(weight, bias, bn)
+        self.Cin, self.Cout, self.relu = Cin, Cout, relu
+        self.engine = "tc16"
+        hi, lo, self.out_scale = fp16_split_scaled(convtranspose_phase_matrix(w, (Cin + 63) // 64 * 64))
+        self.w_hi, self.w_lo = hi.to(device), lo.to(device)
+        self.b = b.float().to(device)
+        # 128-column tiles: the widest the engine runs, and the planes-only epilogue keeps its registers there (as the head stem's)
+        self.bn_tile = 128 if Cout % 128 == 0 else 0
+
+    @staticmethod
+    def out_hw(H, W):
+        return 2 * H, 2 * W
+
+    def __call__(self, x: Act, out: Act, f32_out: bool = True):
+        """out = relu(bn(conv_transpose(x))) at twice the size of x.  x must carry fresh fp16 (hi, lo) planes; f32_out=False writes the
+        output planes only (legal when every consumer is a tensor-core conv)."""
+        assert x.C == self.Cin and out.C == self.Cout and out.B == x.B and (out.H, out.W) == self.out_hw(x.H, x.W)
+        if not x.h16:
+            raise _lib.Vd3dError("transposed conv: input activation has no fp16 (hi, lo) planes (plan bug: missing split_lo)")
+        if CHECK_LO:
+            check_lo(x)
+        if not f32_out and not out.h16:
+            raise _lib.Vd3dError("transposed conv: a planes-only output needs an activation with fp16 (hi, lo) planes")
+        xh, xl = x.h16_ptrs
+        oh, ol = out.h16_ptrs
+        call("vd3d_convtranspose2d_tc16", xh, xl, x.B, x.H, x.W, self.Cin, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(),
+             self.out_scale, self.b.data_ptr(), out.ptr if f32_out else None, oh, ol, self.Cout, out.cs, out.co, 1 if self.relu else 0,
+             self.bn_tile, _stream())
+        out.f32, out.lo_fresh = bool(f32_out), out.h16
+        return out
+
+
 class StemLayer:
     """Few-channel KxK strided stem conv (conv1 7x7 s2 + BN + ReLU, R/backbones/resnet.py:120-122,186-188) on the tensor cores:
     the NCHW image is converted straight into zero-padded fp16 (hi, lo) row planes and the conv runs as a KHx1 convolution

@@ -74,6 +74,10 @@ def synth_state_dict(shapes: Mapping[str, Sequence[int]], seed: int = 0, gain: f
                 std = 0.6 / math.sqrt(fan_in)
             elif "head_layers." in k and k.endswith(".2.weight"):      # CenterNet head outputs (zero-ish in the reference init)
                 std = 1.2 / math.sqrt(fan_in)
+            elif "deconv_layers." in k and len(shp) == 4 and shp[1] > 1 and shp[2:] == (4, 4):
+                # dense ConvTranspose2d(4, stride 2) of the ResNet CenterNet core, [Cin, Cout, 4, 4]: every output pixel sums Cin x 2 x 2 taps
+                # (not Cout x 16), so He-scale to that fan-in and the three layers keep activations O(1)
+                std = gain * math.sqrt(2.0 / (shp[0] * 4))
             if (stem + ".conv_offset.weight") in names:              # DCNv2 main weights: the sigmoid mask (~0.5) halves the response
                 std = std * 2.0
             if ".up_" in k and len(shp) == 4 and shp[1] == 1:          # depthwise ConvTranspose2d of IDAUp: bilinear-like, positive
