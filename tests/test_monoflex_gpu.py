@@ -4,37 +4,12 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from conftest import GOLDEN, load_fixture, subsample_like
 import torch_port as tp
 from detector_harness import match_dets, run_with_stages
 
 pytestmark = pytest.mark.gpu
-
-
-def nhwc(x):
-    return x.permute(0, 2, 3, 1).contiguous()
-
-
-def test_maxpool2x2_and_dw_convtranspose():
-    from visualdet3d_b200 import engine as E
-    from visualdet3d_b200._lib import call
-    g = torch.Generator().manual_seed(0)
-    x = torch.randn(2, 24, 10, 14, generator=g)
-    xa = E.Act(nhwc(x).cuda())
-    o = E.Act(torch.empty(2, 5, 7, 24, device="cuda"))
-    call("vd3d_maxpool2x2s2_nhwc", xa.ptr, 2, 10, 14, 24, 24, 0, o.ptr, 24, 0, None)
-    assert torch.equal(o.to_nchw().cpu(), F.max_pool2d(x, 2, 2))
-    for f in (2, 4):
-        w = torch.randn(24, 1, 2 * f, 2 * f, generator=g)
-        add = torch.randn(2, 24, 10 * f, 14 * f, generator=g)
-        ref = F.conv_transpose2d(x, w, None, stride=f, padding=f // 2, groups=24) + add
-        wk = w.reshape(24, -1).t().contiguous().cuda()
-        aa = E.Act(nhwc(add).cuda())
-        out = E.Act(torch.empty(2, 10 * f, 14 * f, 24, device="cuda"))
-        call("vd3d_dw_convtranspose_nhwc", xa.ptr, 2, 10, 14, 24, 24, 0, wk.data_ptr(), f, aa.ptr, 24, 0, out.ptr, 24, 0, None)
-        np.testing.assert_allclose(out.to_nchw().cpu().numpy(), ref.numpy(), rtol=1e-5, atol=1e-5)
 
 
 @pytest.fixture(scope="module")

@@ -73,24 +73,6 @@ def test_conv_bn_folding_matches_conv_then_bn():
     np.testing.assert_allclose(out.to_nchw().cpu().numpy(), ref.numpy(), rtol=1e-4, atol=2e-5)
 
 
-def test_pools_dwconv_copy():
-    E = _E()
-    g = torch.Generator().manual_seed(2)
-    x = torch.randn(2, 24, 18, 26, generator=g)
-    xa = E.Act(nhwc(x).cuda())
-    mp = E.maxpool3x3s2(xa, E.Act(torch.empty(2, 9, 13, 24, device="cuda")))
-    assert torch.equal(mp.to_nchw().cpu(), F.max_pool2d(x, 3, 2, 1))
-    ap = E.avgpool2(xa, E.Act(torch.empty(2, 9, 13, 24, device="cuda")))
-    np.testing.assert_allclose(ap.to_nchw().cpu().numpy(), F.avg_pool2d(x, 2).numpy(), atol=1e-6)
-    w = torch.randn(24, 1, 3, 3, generator=g)
-    dw = E.DwConvLayer(w, None, relu=True, device="cuda")
-    o = dw(xa, E.Act(torch.empty(2, 18, 26, 24, device="cuda")))
-    np.testing.assert_allclose(o.to_nchw().cpu().numpy(), F.relu(F.conv2d(x, w, None, padding=1, groups=24)).numpy(), atol=1e-5)
-    big = E.Act(torch.zeros(2, 18, 26, 40, device="cuda"))
-    E.copy_channels(xa, big.slice(8, 24))
-    assert torch.equal(big.slice(8, 24).to_nchw().cpu(), x) and float(big.t[..., :8].abs().max()) == 0
-
-
 @pytest.mark.parametrize("shape", [(2, 64, 5, 80), (1, 128, 3, 40), (1, 64, 4, 200), (2, 32, 3, 50), (1, 64, 2, 20), (1, 128, 2, 7)])
 def test_psm_cosine_vs_oracle(shape):
     """PSMCosine (R/lib/PSM_cost_volume.py:76-91): tiled kernel (C = 64/128, D = 24), generic kernel, ragged widths,
