@@ -423,21 +423,24 @@ int vd3d_nms_bev(const float* boxes, int N, float thresh, int rotated, void* ws,
  * boxes [N][5], qboxes [K][5] = (x, y, dx, dy, angle) f32; iou [N][K] f32 = devRotateIoUEval(qboxes[k], boxes[n], criterion),
  * criterion -1 IoU, 0 / 1 intersection over the query / box area, 2 intersection area.
  *
- * vd3d_kitti_eval replaces eval.py eval_class (:476-594) for the three metrics of do_eval_v3 (:650-673) with difficulties 0, 1, 2:
+ * vd3d_kitti_eval replaces eval.py eval_class (:476-594) for the three metrics of do_eval_v3 (:650-673) with difficulties 0, 1, 2 and
+ * any number n_mo >= 1 of min-overlap rows (2 for get_official_eval_result, 10 for do_coco_style_eval :676-703, in one call):
  * calculate_iou_partly, clean_data, compute_statistics_jit, get_thresholds and fused_compute_statistics, per image.
  *   gt [n_gt][15] f64 = bbox x1 y1 x2 y2, alpha, dims l h w, location x y z, rotation_y, truncated, occluded, class code;
  *   dt [n_dt][16] f64 = the same columns + score.  Class code: index into the reference's CLASS_NAMES of the lower-cased name
  *   ('car' 0, 'pedestrian' 1, 'cyclist' 2, 'van' 3, 'person_sitting' 4, 'tractor' 6, 'trailer' 7), -2 for "DontCare", else -1.
  *   offs [4][n_img+1] i64 = CSR offsets of gt rows, dt rows, [dt][gt] overlap blocks (n_pairs in all) and 32-bit detection-flag
- *   words (ceil(dt rows / 32) per image, n_words in all); classes [n_cls] i32; min_overlaps [2][3][n_cls] f64.
- * Outputs, configuration cfg = ((metric * n_cls + class) * 3 + difficulty) * 2 + min_overlap index:
- *   overlaps [3][n_pairs] (bbox, BEV, 3-D), precision / thresholds [18 n_cls][41], n_thresh [18 n_cls], orientation [6 n_cls][41]
- *   (metric 0 only; zeros unless compute_aos).  A configuration with n_thresh > 41 (the reference raises) has truncated thresholds.
- * workspace: vd3d_kitti_eval_workspace_bytes(...) bytes of device memory (a negative return is an error code). */
+ *   words (ceil(dt rows / 32) per image, n_words in all); classes [n_cls] i32; min_overlaps [n_mo][3][n_cls] f64.
+ * Outputs, configuration cfg = ((metric * n_cls + class) * 3 + difficulty) * n_mo + row:
+ *   overlaps [3][n_pairs] (bbox, BEV, 3-D), precision / thresholds [9 n_mo n_cls][41], n_thresh [9 n_mo n_cls], orientation
+ *   [3 n_mo n_cls][41] (metric 0 only; zeros unless compute_aos).  A configuration with n_thresh > 41 (the reference raises) has
+ *   truncated thresholds.  The overlaps and the ignore flags are computed once, whatever n_mo.
+ * workspace: vd3d_kitti_eval_workspace_bytes(...) bytes of device memory (a negative return is an error code, also when
+ * 9 n_mo n_cls configurations are too many to index). */
 int vd3d_kitti_rotate_iou(const float* boxes, int N, const float* qboxes, int K, int criterion, float* iou, void* stream);
-long long vd3d_kitti_eval_workspace_bytes(int n_img, long long n_gt, long long n_dt, long long n_words, int n_cls);
+long long vd3d_kitti_eval_workspace_bytes(int n_img, long long n_gt, long long n_dt, long long n_words, int n_cls, int n_mo);
 int vd3d_kitti_eval(const double* gt, const double* dt, const long long* offs, int n_img, long long n_gt, long long n_dt,
-                    long long n_pairs, long long n_words, const int* classes, int n_cls, const double* min_overlaps, int compute_aos,
+                    long long n_pairs, long long n_words, const int* classes, int n_cls, const double* min_overlaps, int n_mo, int compute_aos,
                     double* overlaps, double* precision, double* orientation, double* thresholds, int* n_thresh,
                     void* workspace, long long workspace_bytes, void* stream);
 

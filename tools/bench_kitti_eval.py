@@ -1,11 +1,13 @@
 """Time the native KITTI evaluator (visualdet3d_b200/kitti_eval.py) on a seeded KITTI-val-sized set, and the reference evaluator on the
 same files where it can run with a real numba CUDA device.
 
-    python tools/bench_kitti_eval.py [--images 3769] [--iters 5] [--no-reference]
+    python tools/bench_kitti_eval.py [--images 3769] [--iters 5] [--no-reference] [--coco]
 
 Writes the label / result files to a temporary directory and prints one JSON line: the wall time of evaluate() split into parse /
 device / format, the device part alone from CUDA events after a warm-up, the card and its power limit, and the reference's wall time
-with a check that its strings are equal ("not measured" where the reference or numba's CUDA target is missing)."""
+with a check that its strings are equal ("not measured" where the reference or numba's CUDA target is missing).  --coco adds "coco":
+the same split and CUDA-event timing for get_coco_eval_result's device part (one vd3d_kitti_eval call per class over ten min-overlap
+rows) next to the official evaluation's."""
 import argparse
 import json
 import os
@@ -76,28 +78,22 @@ def write_set(root, n_img, seed):
     return lab, res, split
 
 
-def native(lab, res, split, classes, iters):
-    """evaluate() step by step (the same calls it makes), timed per stage; then the device part alone with CUDA events."""
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    dt_annos = kitti_eval.get_label_annos(res)
-    gt_annos = kitti_eval.get_label_annos(lab, kitti_eval._read_imageset_file(split))
-    t1 = time.perf_counter()
+def device_part(gt_annos, dt_annos, classes, min_overlaps_of, format_result, iters):
+    """One DeviceEval per class (pack, upload, run, download) and its text, timed; then the launches alone with CUDA events."""
     t_dev = t_fmt = 0.0
     texts, evals = [], []
     for c in classes:
         cls = kitti_eval._class_indices(c)
         aos = kitti_eval._compute_aos(dt_annos)
         ta = time.perf_counter()
-        ev = kitti_eval.DeviceEval(gt_annos, dt_annos, cls, kitti_eval.MIN_OVERLAPS[:, :, cls], aos)
+        ev = kitti_eval.DeviceEval(gt_annos, dt_annos, cls, min_overlaps_of(cls), aos)
         metrics = ev.run().collect()
         tb = time.perf_counter()
-        texts.append(kitti_eval.format_official_result(metrics, cls, aos))
+        texts.append(format_result(metrics, cls, aos))
         tc = time.perf_counter()
         t_dev += tb - ta
         t_fmt += tc - tb
         evals.append(ev)
-    assert texts == kitti_eval.evaluate(lab, res, split, classes, gpu=torch.cuda.current_device())
     for ev in evals:                       # warm-up done above; now the launches alone
         ev.run()
     torch.cuda.synchronize()
@@ -108,9 +104,33 @@ def native(lab, res, split, classes, iters):
             ev.run()
     end.record()
     end.synchronize()
-    return texts, {"parse_s": t1 - t0, "device_s": t_dev, "format_s": t_fmt, "total_s": t1 - t0 + t_dev + t_fmt,
-                   "device_events_ms": start.elapsed_time(end) / iters, "n_gt": int(sum(len(a["name"]) for a in gt_annos)),
-                   "n_dt": int(sum(len(a["name"]) for a in dt_annos))}
+    return texts, t_dev, t_fmt, start.elapsed_time(end) / iters
+
+
+def native(lab, res, split, classes, iters, coco):
+    """evaluate() step by step (the same calls it makes), timed per stage; then the device part alone with CUDA events.  With coco,
+    get_coco_eval_result's device part on the same parsed annos, timed the same way."""
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    dt_annos = kitti_eval.get_label_annos(res)
+    gt_annos = kitti_eval.get_label_annos(lab, kitti_eval._read_imageset_file(split))
+    t1 = time.perf_counter()
+    texts, t_dev, t_fmt, ev_ms = device_part(gt_annos, dt_annos, classes, lambda cls: kitti_eval.MIN_OVERLAPS[:, :, cls],
+                                             kitti_eval.format_official_result, iters)
+    assert texts == kitti_eval.evaluate(lab, res, split, classes, gpu=torch.cuda.current_device())
+    out = {"parse_s": t1 - t0, "device_s": t_dev, "format_s": t_fmt, "total_s": t1 - t0 + t_dev + t_fmt,
+           "device_events_ms": ev_ms, "n_gt": int(sum(len(a["name"]) for a in gt_annos)),
+           "n_dt": int(sum(len(a["name"]) for a in dt_annos))}
+    if coco:
+        coco_texts, c_dev, c_fmt, c_ms = device_part(
+            gt_annos, dt_annos, classes, lambda cls: kitti_eval.coco_min_overlaps(kitti_eval._coco_overlap_ranges(cls)),
+            kitti_eval.format_coco_result, iters)
+        assert coco_texts == [kitti_eval.get_coco_eval_result(gt_annos, dt_annos, c) for c in classes]
+        out["coco"] = {"device_s": c_dev, "format_s": c_fmt, "device_events_ms": c_ms, "official_device_events_ms": ev_ms,
+                       "min_overlap_rows": 10,
+                       "reference": "not measured: its get_coco_eval_result raises TypeError on numpy >= 1.18 (np.linspace num as float64)"}
+        texts = texts + coco_texts
+    return texts, out
 
 
 REF_CODE = """
@@ -151,6 +171,7 @@ def main():
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--no-reference", action="store_true")
     ap.add_argument("--reference-timeout", type=int, default=900)
+    ap.add_argument("--coco", action="store_true", help="also time the COCO-style evaluation's device part")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_kitti_eval needs a CUDA device")
@@ -158,13 +179,15 @@ def main():
     classes = [0, 1, 2]
     with tempfile.TemporaryDirectory() as root:
         lab, res, split = write_set(root, args.images, args.seed)
-        texts, out = native(lab, res, split, classes, args.iters)
+        texts, out = native(lab, res, split, classes, args.iters, args.coco)
         ref = {"status": "not measured: --no-reference"} if args.no_reference else reference(lab, res, split, classes, args.reference_timeout)
     if "texts" in ref:
-        ref["strings_equal"] = ref.pop("texts") == texts
+        ref["strings_equal"] = ref.pop("texts") == texts[:len(classes)]
     out.update({"images": args.images, "classes": classes, "gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 else "unknown",
                 "reference": ref})
     print(texts[0])
+    if args.coco:
+        print(texts[len(classes)])
     print(json.dumps(out))
 
 

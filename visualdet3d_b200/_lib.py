@@ -102,8 +102,8 @@ _SIGS = {
     "vd3d_retina_decode_workspace": (c_longlong, [I, I, I]),
     "vd3d_retina_decode": (I, [I, P, P, P, I, I, P, I, I, I, I, I, P, P, F, c_double, I, P, P, P, P, P, P, P, P]),
     "vd3d_kitti_rotate_iou": (I, [P, I, P, I, I, P, P]),
-    "vd3d_kitti_eval_workspace_bytes": (c_longlong, [I, c_longlong, c_longlong, c_longlong, I]),
-    "vd3d_kitti_eval": (I, [P, P, P, I, c_longlong, c_longlong, c_longlong, c_longlong, P, I, P, I, P, P, P, P, P, P, c_longlong, P]),
+    "vd3d_kitti_eval_workspace_bytes": (c_longlong, [I, c_longlong, c_longlong, c_longlong, I, I]),
+    "vd3d_kitti_eval": (I, [P, P, P, I, c_longlong, c_longlong, c_longlong, c_longlong, P, I, P, I, I, P, P, P, P, P, P, c_longlong, P]),
     "vd3d_anchor_loss_workspace_bytes": (c_longlong, [I, I, I]),
     "vd3d_anchor_loss_forward": (I, [P, P, P, P, P, P, I, I, I, I, P, I, I, P, c_longlong, P, P, P, P, P, P]),
     "vd3d_anchor_loss_backward": (I, [P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P]),

@@ -3,8 +3,8 @@
 //
 // Data (all device, float64 as parsed): ground truth [n_gt][KE_GT_COLS], detections [n_dt][KE_DT_COLS] (the same columns + score),
 // CSR offsets offs[4][n_img+1] = ground truth, detections, [dt x gt] overlap blocks, 32-bit detection-flag words.
-// Configuration index cfg = ((metric * n_cls + class) * 3 + difficulty) * 2 + min_overlap: the reference's
-// precision[class][difficulty][min_overlap][41] per metric, flattened.
+// Configuration index cfg = ((metric * n_cls + class) * 3 + difficulty) * n_mo + row, over the n_mo min-overlap rows: the reference's
+// precision[class][difficulty][row][41] per metric, flattened.  The official evaluation has n_mo = 2, the COCO-style one 10.
 //
 // Compiled with -fmad=false: the bbox overlaps and all float64 statistics then round every product and sum separately, like numba.
 #include "common.cuh"
@@ -175,10 +175,10 @@ struct EvalArgs {
     const long long* dt_off;
     const long long* ov_off;
     const long long* word_off;
-    int n_img, n_cls;
+    int n_img, n_cls, n_mo;
     long long n_gt, n_dt, n_pairs, n_words;
     const int* classes;           // [n_cls] class indices of the reference's CLASS_NAMES
-    const double* min_overlaps;   // [2][3][n_cls]
+    const double* min_overlaps;   // [n_mo][3][n_cls]
     int compute_aos;
     double* overlaps;             // [3][n_pairs]: per image [dt][gt] row-major
     signed char* ign_gt;          // [n_cls][3][n_gt]
@@ -192,9 +192,9 @@ struct EvalArgs {
     int* n_thresh;                // [n_cfg]
     unsigned* flags2;             // [n_cfg][41][n_words]
     int* counts;                  // [n_cfg][41][3] tp, fp, fn
-    double* sims;                 // [n_cls*6][41][n_img]
+    double* sims;                 // [3 n_mo n_cls][41][n_img]
     double* precision;            // [n_cfg][41]
-    double* orientation;          // [n_cls*6][41]
+    double* orientation;          // [3 n_mo n_cls][41]
 };
 
 // ---- overlaps of the three metrics, one thread per (metric, dt, gt) pair of one image ------------------------------------------
@@ -357,9 +357,9 @@ __device__ Stats compute_statistics(const EvalArgs& a, int metric, int cd, int i
 }
 
 __device__ __forceinline__ void decode_cfg(const EvalArgs& a, int cfg, int& metric, int& cd, double& min_overlap) {
-    const int k = cfg % 2;
-    cd = (cfg / 2) % (a.n_cls * 3);
-    metric = cfg / (2 * a.n_cls * 3);
+    const int k = cfg % a.n_mo;
+    cd = (cfg / a.n_mo) % (a.n_cls * 3);
+    metric = cfg / (a.n_mo * a.n_cls * 3);
     min_overlap = a.min_overlaps[(k * 3 + metric) * a.n_cls + cd / 3];
 }
 
@@ -383,7 +383,7 @@ __global__ void thresholds_kernel(EvalArgs a, int n_cfg) {
     const int cfg = blockIdx.x * blockDim.x + threadIdx.x;
     if (cfg >= n_cfg) return;
     const int n = a.n_tp[cfg];
-    const int num_gt = a.n_valid[(cfg / 2) % (a.n_cls * 3)];
+    const int num_gt = a.n_valid[(cfg / a.n_mo) % (a.n_cls * 3)];
     const double* sc = a.tp_sorted + cfg * a.n_gt;
     double* thr = a.thresholds + cfg * kPts;
     double current_recall = 0;
@@ -477,8 +477,9 @@ struct Layout {
 
 size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
 
-int make_layout(int n_img, long long n_gt, long long n_dt, long long n_words, int n_cls, Layout& L) {
-    const long long n_cfg = 18LL * n_cls;
+int make_layout(int n_img, long long n_gt, long long n_dt, long long n_words, int n_cls, int n_mo, Layout& L) {
+    if ((long long)n_mo * n_cls > 0x7fffffffLL / (9 * kPts * 3)) return VD3D_EINVAL;   // the kernels index counts [n_cfg][41][3] with int
+    const long long n_cfg = 9LL * n_mo * n_cls;
     size_t o = 0;
     auto take = [&](size_t bytes) { const size_t at = o; o = align_up(o + bytes); return at; };
     L.ign_gt = take(n_cls * 3 * n_gt);
@@ -491,7 +492,7 @@ int make_layout(int n_img, long long n_gt, long long n_dt, long long n_words, in
     L.n_thresh = take(n_cfg * sizeof(int));
     L.flags2 = take(n_cfg * kPts * n_words * sizeof(unsigned));
     L.counts = take(n_cfg * kPts * 3 * sizeof(int));
-    L.sims = take(n_cls * 6LL * kPts * n_img * sizeof(double));
+    L.sims = take(3LL * n_mo * n_cls * kPts * n_img * sizeof(double));
     L.seg = take((n_cfg + 1) * sizeof(int));
     L.cub_bytes = 0;
     if (n_cfg * n_gt > 0) {
@@ -518,38 +519,40 @@ extern "C" int vd3d_kitti_rotate_iou(const float* boxes, int N, const float* qbo
     return VD3D_OK;
 }
 
-extern "C" long long vd3d_kitti_eval_workspace_bytes(int n_img, long long n_gt, long long n_dt, long long n_words, int n_cls) {
-    if (n_img < 0 || n_gt < 0 || n_dt < 0 || n_words < 0 || n_cls <= 0) {
+extern "C" long long vd3d_kitti_eval_workspace_bytes(int n_img, long long n_gt, long long n_dt, long long n_words, int n_cls, int n_mo) {
+    if (n_img < 0 || n_gt < 0 || n_dt < 0 || n_words < 0 || n_cls <= 0 || n_mo <= 0) {
         vd3d::set_error("kitti_eval_workspace_bytes: bad args");
         return VD3D_EINVAL;
     }
     Layout L;
-    const int rc = make_layout(n_img, n_gt, n_dt, n_words, n_cls, L);
+    const int rc = make_layout(n_img, n_gt, n_dt, n_words, n_cls, n_mo, L);
     if (rc != VD3D_OK) {
-        vd3d::set_error("kitti_eval_workspace_bytes: %s", rc == VD3D_EINVAL ? "too many scores for one segmented sort" : "cub query failed");
+        vd3d::set_error("kitti_eval_workspace_bytes: %s", rc == VD3D_EINVAL ? "too many configurations or scores for one segmented sort"
+                                                                           : "cub query failed");
         return rc;
     }
     return (long long)L.total;
 }
 
 extern "C" int vd3d_kitti_eval(const double* gt, const double* dt, const long long* offs, int n_img, long long n_gt, long long n_dt,
-                               long long n_pairs, long long n_words, const int* classes, int n_cls, const double* min_overlaps, int compute_aos,
+                               long long n_pairs, long long n_words, const int* classes, int n_cls, const double* min_overlaps, int n_mo,
+                               int compute_aos,
                                double* overlaps, double* precision, double* orientation, double* thresholds, int* n_thresh,
                                void* workspace, long long workspace_bytes, void* stream) {
-    VD3D_REQUIRE(n_img > 0 && n_cls > 0 && n_gt >= 0 && n_dt >= 0 && n_pairs >= 0 && n_words >= 0, "kitti_eval: bad sizes");
+    VD3D_REQUIRE(n_img > 0 && n_cls > 0 && n_mo > 0 && n_gt >= 0 && n_dt >= 0 && n_pairs >= 0 && n_words >= 0, "kitti_eval: bad sizes");
     VD3D_REQUIRE(offs && classes && min_overlaps && precision && orientation && thresholds && n_thresh && workspace,
                  "kitti_eval: null pointer");
     VD3D_REQUIRE((n_gt == 0 || gt) && (n_dt == 0 || dt) && (n_pairs == 0 || overlaps), "kitti_eval: null box or overlap pointer");
     Layout L;
-    VD3D_REQUIRE(make_layout(n_img, n_gt, n_dt, n_words, n_cls, L) == VD3D_OK, "kitti_eval: workspace layout failed");
+    VD3D_REQUIRE(make_layout(n_img, n_gt, n_dt, n_words, n_cls, n_mo, L) == VD3D_OK, "kitti_eval: workspace layout failed");
     VD3D_REQUIRE((size_t)workspace_bytes >= L.total, "kitti_eval: workspace of %lld bytes, %zu needed", workspace_bytes, L.total);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    const int n_cfg = 18 * n_cls;
+    const int n_cfg = 9 * n_mo * n_cls;   // make_layout bounded n_cfg * 41 * 3 by INT_MAX
     EvalArgs a;
     a.gt = gt; a.dt = dt;
     a.gt_off = offs; a.dt_off = offs + (n_img + 1); a.ov_off = offs + 2 * (n_img + 1); a.word_off = offs + 3 * (n_img + 1);
-    a.n_img = n_img; a.n_cls = n_cls; a.n_gt = n_gt; a.n_dt = n_dt; a.n_pairs = n_pairs; a.n_words = n_words;
+    a.n_img = n_img; a.n_cls = n_cls; a.n_mo = n_mo; a.n_gt = n_gt; a.n_dt = n_dt; a.n_pairs = n_pairs; a.n_words = n_words;
     a.classes = classes; a.min_overlaps = min_overlaps; a.compute_aos = compute_aos;
     a.overlaps = overlaps;
     a.ign_gt = (signed char*)(ws + L.ign_gt); a.ign_dt = (signed char*)(ws + L.ign_dt); a.n_valid = (int*)(ws + L.n_valid);
