@@ -762,13 +762,14 @@ extern "C" int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* con
                      "conv2d_tc16: level %d: 16-byte aligned input planes and a non-empty size are required", l);
         s.in[l] = in_hi[l]; s.in_lo[l] = in_lo[l]; s.H[l] = H[l]; s.W[l] = W[l];
         s.res_H[l] = res_H ? res_H[l] : 0; s.res_W[l] = res_W ? res_W[l] : 0;
-        // every output form of level l sits at the same pixel offset from level 0's (one allocation per form, levels concatenated)
-        const long long o32 = out ? level_pix_off(out[0], out[l], 4, out_cs) : 0;
+        // every output form of level l sits at the same pixel offset from level 0's (one allocation per form, levels concatenated); a form
+        // that is not written takes the offset of one that is (planes-only launches have no fp32 output)
+        const long long o32 = out ? level_pix_off(out[0], out[l], 4, out_cs) : level_pix_off(out_hi16[0], out_hi16[l], 2, out_cs);
         const long long oh = out_hi16 ? level_pix_off(out_hi16[0], out_hi16[l], 2, out_cs) : o32;
         const long long ol = out_lo16 ? level_pix_off(out_lo16[0], out_lo16[l], 2, out_cs) : o32;
         VD3D_REQUIRE(o32 == oh && oh == ol && (out ? out[l] != nullptr : true) && o32 > (-1LL << 62),
                      "conv2d_tc16: level %d: the output forms must lie at one common pixel offset from level 0's", l);
-        s.out_off[l] = out ? o32 : oh;
+        s.out_off[l] = o32;
         VD3D_REQUIRE((!res || res[l]) && (!res_hi16 || (res_hi16[l] && res_lo16[l])), "conv2d_tc16: level %d has no residual", l);
         if (res) {
             s.res_off[l] = level_pix_off(res[0], res[l], 4, res_cs);
