@@ -107,6 +107,17 @@ int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* const* in_lo, 
 int vd3d_convtranspose2d_tc16(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
                               const void* w_hi, const void* w_lo, float out_scale, const float* bias,
                               float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn, void* stream);
+/* The conv of vd3d_conv2d_tc16 computed only at listed output pixels, one 96-column group of the output channels at a time (the anchor
+ * head's regression conv on the pixels whose anchors the decoder reads, vd3d_reg_candidates).  Stride 1, output size = input size
+ * (2 pad = dil (K - 1)), fp32 output + bias, no residual / ReLU.
+ *   list [groups][B*H*W] i32 : counts[g] output pixels b*H*W + h*W + w (in any order) for columns 96 g .. 96 g + 95 of group g
+ *   counts [groups] i32      : read on the device (no host synchronisation); groups = ceil(Cout / 96) <= 32
+ * Bit-identical to vd3d_conv2d_tc16 at the listed pixels and columns; no other element of `out` is written.  Inputs / weights as
+ * vd3d_conv2d_tc16 (Cin % 8 == 0, Cout % 4 == 0). */
+int vd3d_conv2d_tc16_gather(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                            const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
+                            const int32_t* list, const int32_t* counts, int groups,
+                            float* out, int Cout, int out_cs, int out_co, void* stream);
 /* Few-channel KHxKW convolution (the ResNet / DLA stem: conv1 7x7 stride 2, R/backbones/resnet.py:120,186) on the tensor cores.
  * The image is held as fp16 (hi, lo) planes [B][H][Wp][4] (pixel x at column x + pad, zeros elsewhere: the buffer must be
  * zero-initialised once); Wp = vd3d_stem_row_pitch(W, KW, stride, pad).  vd3d_image_to_h16_rows fills the planes from an
@@ -210,6 +221,14 @@ int vd3d_concat_volume_conv3d(const float* lf, const float* rf, int B, int H, in
  *   anchors [N][4] f32, means_z [T][N] f32 (prior z mean per type), P2 [B][3][4] f32 -> mask [B][N] u8 */
 int vd3d_anchor_mask(const float* anchors, const float* means_z, const float* P2, int B, int N, int T,
                      float y_min, float y_max, float x_thr, uint8_t* mask, void* stream);
+
+/* The rows of the regression conv the decoder may read (vd3d_conv2d_tc16_gather's list): pair (b, pixel, group) when some anchor
+ * a of the group (group_anchors consecutive anchors of the pixel, anchor n = pixel * A + a) has mask[b][n] and the decoder's first-max
+ * sigmoid score > score_thr.  A superset of the anchors vd3d_decode_nms decodes (its prior z_mean > 0 test is not applied).
+ *   cls [B][P*A][ncls+1], mask [B][P*A] u8 -> list [groups][B*P] i32 (b*P + pixel), counts [groups] i32, groups = ceil(A / group_anchors);
+ *   counts are zeroed here; the list cannot overflow */
+int vd3d_reg_candidates(const float* cls, const uint8_t* mask, int B, int P, int A, int ncls, float score_thr, int group_anchors,
+                        int32_t* list, int32_t* counts, void* stream);
 
 /* AnchorBasedDetection3DHead.get_bboxes (R/heads/detection_3d_head.py:341-400) + _decode (:218-263) +
  * ClipBoxes (R/utils/utils.py:181-196) + torchvision.ops.nms (class-agnostic, IoU > thr suppresses), batched.

@@ -413,6 +413,197 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     }
 }
 
+// ----------------------------------------------------------------------------------------------------------------
+// Gathered-row conv (vd3d_conv2d_tc16_gather): the M rows of a tile are 128 entries of a device list of output pixels, not a rectangle, and
+// its N tile is one 96-column group of the output channels.  The anchor head's regression conv runs on the pixels whose anchors of that
+// group the decoder reads (vd3d_reg_candidates), instead of on the whole map.
+//   warps 0..7   two consumer warpgroups: the same wg_tile_kloop as conv2d_tcp_kernel (k-block order, chunk promotion, three products in
+//                the same order), so every output element carries the bits the dense conv gives it (tile widths are bit-identical); the
+//                epilogue (the dense one's arithmetic: scale, + 0 residual, + bias) stores straight from the accumulator registers, so no
+//                staging tile takes shared memory from the operand ring
+//   warp 8       weight producer: TMA boxes [64 k][96] of the (hi, lo) weight matrix, one per k-block
+//   warps 9..12  gather: per k-block (tap, 64-channel chunk) 16-byte cp.async of every row's (hi, lo) channels into the SWIZZLE_128B K-major
+//                stage (layout as dcn_fused.cu); a tap outside the image, a channel beyond Cin and a row beyond the list's count copy zero
+//                bytes (zero fill), as the dense conv's TMA out-of-bounds fill does.  Each gather thread keeps TCG_LAG k-blocks of copies in
+//                flight and signals a stage once its copies have landed.
+// The tile count is read from the device (the list's per-group counts): the launch needs no host synchronisation.
+// ----------------------------------------------------------------------------------------------------------------
+constexpr int TCG_BN = 96;
+constexpr int TCG_GATHER_WARPS = 4;
+constexpr int TCG_THREADS = TC_CONSUMERS + 32 + 32 * TCG_GATHER_WARPS;
+constexpr int TCG_STAGES = 4;
+// k-blocks of copies a gather thread keeps in flight.  The consumers release a stage only after they have acquired the next one, so before
+// the gather warps reuse the stage of k-block k - TCG_STAGES they must have signalled k-block k - TCG_STAGES + 1: TCG_LAG <= TCG_STAGES - 2.
+constexpr int TCG_LAG = TCG_STAGES - 2;
+constexpr int TCG_MAX_GROUPS = 32;
+
+struct TcgParams {
+    const __half* in_hi; const __half* in_lo;     // input planes [B][H][W][in_cs], channels in_co ..
+    int H, W, in_cs, in_co;
+    const int* list; const int* counts;           // list [groups][cap]: output pixel b * H * W + h * W + w; counts [groups]
+    int groups, cap;
+    int KW, taps, pad, dil;
+};
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+
+__global__ void __launch_bounds__(TCG_THREADS, 1)
+conv2d_tcg_kernel(const __grid_constant__ CUtensorMap mapWhi, const __grid_constant__ CUtensorMap mapWlo, const TcParams p, const TcgParams g) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    constexpr int BN = TCG_BN;
+    constexpr uint32_t a_bytes = 128u * 128u, b_bytes = (uint32_t)BN * 128u, stage_bytes = 2u * a_bytes + 2u * b_bytes;
+    uint64_t* fullA = reinterpret_cast<uint64_t*>(smem + (size_t)TCG_STAGES * stage_bytes);   // [stages] gather warps -> consumers
+    uint64_t* fullB = fullA + TCG_STAGES;                                                 // [stages] weight TMA -> consumers
+    uint64_t* empty = fullB + TCG_STAGES;                                                 // [stages] consumers (8 warps) -> producers
+    int* first = reinterpret_cast<int*>(empty + TCG_STAGES);                              // [groups + 1] first tile of each group
+
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
+    const int KB = g.taps * (p.cin_pad / 64);
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < TCG_STAGES; ++s) { mbar_init(&fullA[s], TCG_GATHER_WARPS); mbar_init(&fullB[s], 1); mbar_init(&empty[s], TC_CONSUMERS / 32); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    pdl_launch_dependents();
+    pdl_wait();                            // (PDL launches only) the list and the input planes are complete
+    if (threadIdx.x == 0) {
+        int t = 0;
+        for (int q = 0; q < g.groups; ++q) { first[q] = t; t += (__ldg(g.counts + q) + 127) / 128; }
+        first[g.groups] = t;
+    }
+    __syncthreads();
+    const int units = first[g.groups];
+    // tile u -> group, its first list entry and the number of entries of the group
+    auto tile_of = [&](int u, int& grp, int& e0, int& cnt) {
+        grp = 0;
+        while (u >= first[grp + 1]) ++grp;
+        e0 = (u - first[grp]) * 128;
+        cnt = __ldg(g.counts + grp);
+    };
+    // k-block kb = (64-channel chunk, tap), chunk outermost: the K order of conv2d_tcp_kernel
+    auto kcol = [&](int kb, int& tap, int& c0) { tap = kb % g.taps; c0 = (kb / g.taps) * 64; };
+
+    if (warp == TC_CONSUMERS / 32) {
+        // ================= weight producer =================
+        int it = 0;
+        for (int u = (int)blockIdx.x; u < units; u += (int)gridDim.x) {
+            int grp, e0, cnt;
+            tile_of(u, grp, e0, cnt);
+            for (int kb = 0; kb < KB; ++kb, ++it) {
+                const int s = it % TCG_STAGES, ph = (it / TCG_STAGES) & 1;
+                mbar_wait(&empty[s], ph ^ 1);
+                if (elect_one()) {
+                    int tap, c0;
+                    kcol(kb, tap, c0);
+                    uint8_t* st = smem + (size_t)s * stage_bytes + 2 * a_bytes;
+                    mbar_expect_tx(&fullB[s], 2u * b_bytes);
+                    tma_load_2d(st, &mapWhi, &fullB[s], tap * p.cin_pad + c0, grp * BN);
+                    tma_load_2d(st + b_bytes, &mapWlo, &fullB[s], tap * p.cin_pad + c0, grp * BN);
+                }
+                __syncwarp();
+            }
+        }
+    } else if (warp < TC_CONSUMERS / 32) {
+        // ================= consumer warpgroups =================
+        const int wg = warp >> 2;
+        int it = 0;
+        auto acquire = [&]() {
+            const int s = it % TCG_STAGES, ph = (it / TCG_STAGES) & 1;
+            mbar_wait(&fullB[s], ph);
+            mbar_wait(&fullA[s], ph);
+            const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+            const uint32_t aw = sa + (uint32_t)wg * 64u * 128u;
+            ++it;
+            return KbOperands{make_sdesc(aw), make_sdesc(aw + a_bytes), make_sdesc(sa + 2 * a_bytes), make_sdesc(sa + 2 * a_bytes + b_bytes), s};
+        };
+        auto release = [&](int st) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[st]);
+        };
+        auto issued = [] {};
+        float tot[BN / 2], c[BN / 2];
+        // accumulator fragment (wg_stage): rows 64 wg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 i + 2 (lane % 4) (+ 1)
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+        for (int u = (int)blockIdx.x; u < units; u += (int)gridDim.x) {
+            int grp, e0, cnt;
+            tile_of(u, grp, e0, cnt);
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+            wg_tile_kloop<BN, true, 0, 4>(tot, c, KB, p.chunk, acquire, release, issued);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (e0 + r0 + 8 * h >= cnt) continue;
+                const long long pix = __ldg(g.list + (long long)grp * g.cap + e0 + r0 + 8 * h);
+                float* op = p.out + pix * p.out_cs + p.out_co;
+#pragma unroll
+                for (int i = 0; i < BN / 8; ++i) {
+                    const int n = grp * BN + 8 * i + c0;
+                    if (n < p.Cout) {                             // (n even, Cout % 4 == 0: both columns exist)
+                        const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.f, 0.f);
+                        float a0 = tot[4 * i + 2 * h] * p.out_scale + 0.f, a1 = tot[4 * i + 2 * h + 1] * p.out_scale + 0.f;   // tcp_epi_out, no residual
+                        a0 += bb.x; a1 += bb.y;
+                        *reinterpret_cast<float2*>(op + n) = make_float2(a0, a1);
+                    }
+                }
+            }
+        }
+    } else {
+        // ================= gather warps =================
+        const int gt = (int)threadIdx.x - (TC_CONSUMERS + 32);
+        const int j = gt & 7;                                  // 16-byte chunk (8 channels) of the 64-channel k-block
+        const int m0 = gt >> 3;                                // rows m0 + 16 r, r = 0 .. 7
+        constexpr int ROWS = 128 / (TCG_GATHER_WARPS * 4);
+        const int HW = g.H * g.W;
+        int it = 0;
+        auto signal = [&](int k) {                             // the copies of k-block k (and every earlier one) have landed
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> the tensor core's async-proxy reads
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&fullA[k % TCG_STAGES]);
+        };
+        for (int u = (int)blockIdx.x; u < units; u += (int)gridDim.x) {
+            int grp, e0, cnt;
+            tile_of(u, grp, e0, cnt);
+            int pix[ROWS], ph_[ROWS], pw_[ROWS];               // output pixel of each row (-1: beyond the count), its row / column
+#pragma unroll
+            for (int r = 0; r < ROWS; ++r) {
+                const int e = e0 + m0 + 16 * r;
+                pix[r] = e < cnt ? __ldg(g.list + (long long)grp * g.cap + e) : -1;
+                const int pi = pix[r] < 0 ? 0 : pix[r] % HW;
+                ph_[r] = pi / g.W; pw_[r] = pi - ph_[r] * g.W;
+            }
+            for (int kb = 0; kb < KB; ++kb, ++it) {
+                const int s = it % TCG_STAGES, ph = (it / TCG_STAGES) & 1;
+                mbar_wait(&empty[s], ph ^ 1);
+                int tap, c0;
+                kcol(kb, tap, c0);
+                const int kh = tap / g.KW, kw = tap - kh * g.KW;
+                const int dy = kh * g.dil - g.pad, dx = kw * g.dil - g.pad;
+                const int ch = c0 + 8 * j;
+                const uint32_t sa = smem_u32(smem + (size_t)s * stage_bytes);
+#pragma unroll
+                for (int r = 0; r < ROWS; ++r) {
+                    const int m = m0 + 16 * r;
+                    const int hi = ph_[r] + dy, wi = pw_[r] + dx;
+                    const bool ok = pix[r] >= 0 && (unsigned)hi < (unsigned)g.H && (unsigned)wi < (unsigned)g.W && ch < p.Cin;
+                    const long long off = ok ? (long long)(pix[r] + dy * g.W + dx) * g.in_cs + g.in_co + ch : 0;
+                    const uint32_t so = (uint32_t)(m >> 3) * 1024u + (uint32_t)(m & 7) * 128u + (uint32_t)((j ^ (m & 7)) * 16);
+                    cp_async16(sa + so, g.in_hi + off, ok ? 16u : 0u);
+                    cp_async16(sa + a_bytes + so, g.in_lo + off, ok ? 16u : 0u);
+                }
+                asm volatile("cp.async.commit_group;" ::: "memory");
+                if (it >= TCG_LAG) {
+                    asm volatile("cp.async.wait_group %0;" ::"n"(TCG_LAG) : "memory");
+                    signal(it - TCG_LAG);
+                }
+            }
+        }
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        for (int k = it - TCG_LAG < 0 ? 0 : it - TCG_LAG; k < it; ++k) signal(k);
+    }
+}
+
 // lo = v - (v & 0xFFFFE000): the part of v the tf32 MMA does not see.  Elementwise, float4, channel-slice aware.
 __global__ void split_lo_kernel(const float* __restrict__ in, float* __restrict__ lo, long long npix, int C4, int cs, int co) {
     long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -810,6 +1001,51 @@ extern "C" int vd3d_convtranspose2d_tc16(const void* in_hi, const void* in_lo, i
     s.out = out; s.out_h16_hi = out_hi16; s.out_h16_lo = out_lo16;
     s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = 3; s.bn = bn;
     return conv2d_tc_launch(s, stream);
+}
+
+// The conv of vd3d_conv2d_tc16 (stride 1, output size = input size, fp32 output, bias, no residual / ReLU) computed only at the listed output
+// pixels of each 96-column group: list [groups][B * H * W] holds counts[g] pixels b * H * W + h * W + w for group g (columns 96 g ..).
+// Bit-identical to the dense conv at those pixels and columns; nothing else of `out` is written.
+extern "C" int vd3d_conv2d_tc16_gather(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                                       const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
+                                       const int32_t* list, const int32_t* counts, int groups,
+                                       float* out, int Cout, int out_cs, int out_co, void* stream) {
+    VD3D_REQUIRE(in_hi && in_lo && w_hi && w_lo && list && counts && out && B > 0 && H > 0 && W > 0, "conv2d_tc16_gather: null pointer or empty input");
+    VD3D_REQUIRE(KH >= 1 && KW >= 1 && dil >= 1 && 2 * pad == dil * (KH - 1) && 2 * pad == dil * (KW - 1),
+                 "conv2d_tc16_gather: the output must have the input's size (2 pad = dil (K - 1), stride 1)");
+    VD3D_REQUIRE(Cout % 4 == 0 && Cout >= 16 && groups == cdiv(Cout, TCG_BN) && groups <= TCG_MAX_GROUPS,
+                 "conv2d_tc16_gather: Cout %d must be a multiple of 4 covered by %d groups of %d columns (<= %d groups)", Cout, groups, TCG_BN, TCG_MAX_GROUPS);
+    VD3D_REQUIRE(Cin % 8 == 0 && in_cs % 8 == 0 && in_co % 8 == 0 && Cin + in_co <= in_cs && ((((uintptr_t)in_hi | (uintptr_t)in_lo) & 15) == 0),
+                 "conv2d_tc16_gather: 16-byte aligned input planes with Cin, pitch and offset multiples of 8");
+    VD3D_REQUIRE(out_cs % 4 == 0 && out_co % 4 == 0 && Cout + out_co <= out_cs && ((uintptr_t)out & 15) == 0 && (!bias || ((uintptr_t)bias & 7) == 0),
+                 "conv2d_tc16_gather: output pitch / offset must be multiples of 4, pointers 16-byte aligned");
+    VD3D_REQUIRE((long long)B * H * W < (1LL << 31), "conv2d_tc16_gather: too many pixels for the 32-bit list");
+    TcParams p;
+    memset(&p, 0, sizeof(p));
+    p.B = B; p.H = H; p.W = W; p.Ho = H; p.Wo = W; p.Cin = Cin; p.KH = KH; p.KW = KW; p.pad = pad; p.dil = dil; p.stride = 1;
+    p.Cout = Cout; p.BN = TCG_BN; p.passes = 3; p.f16 = 1; p.bk = 64; p.cin_pad = (Cin + 63) / 64 * 64; p.out_scale = out_scale;
+    p.cout_pad = (Cout + 15) / 16 * 16;
+    p.out_cs = out_cs; p.out_co = out_co; p.bias = bias; p.out = out;
+    {
+        const char* e = getenv("VD3D_TC_CHUNK");            // the dense conv's promotion chunk: the same bits
+        p.chunk = e ? atoi(e) : 4;
+        if (p.chunk < 1) p.chunk = 1;
+    }
+    TcgParams g;
+    g.in_hi = (const __half*)in_hi; g.in_lo = (const __half*)in_lo; g.H = H; g.W = W; g.in_cs = in_cs; g.in_co = in_co;
+    g.list = list; g.counts = counts; g.groups = groups; g.cap = B * H * W;
+    g.KW = KW; g.taps = KH * KW; g.pad = pad; g.dil = dil;
+    CUtensorMap mWhi, mWlo;
+    int rc;
+    if ((rc = make_map_wgt(&mWhi, w_hi, Cout, KH * KW * p.cin_pad, TCG_BN, 2))) return rc;
+    if ((rc = make_map_wgt(&mWlo, w_lo, Cout, KH * KW * p.cin_pad, TCG_BN, 2))) return rc;
+    const long long max_tiles = (long long)groups * cdiv((long long)B * H * W, 128);
+    const int grid = max_tiles < kNumSMs ? (int)max_tiles : kNumSMs;
+    const size_t smem = (size_t)TCG_STAGES * (2 * 128 * 128 + 2 * TCG_BN * 128) + 3 * TCG_STAGES * sizeof(uint64_t) + (TCG_MAX_GROUPS + 1) * sizeof(int) + 1024;
+    const cudaError_t le = tc_launch<conv2d_tcg_kernel>(grid, TCG_THREADS, smem, stream, mWhi, mWlo, p, g);
+    if (le != cudaSuccess) { set_error("conv2d_tc16_gather: launch failed: %s", cudaGetErrorString(le)); return VD3D_ECUDA; }
+    VD3D_CHECK_LAUNCH("conv2d_tc16_gather");
+    return VD3D_OK;
 }
 
 // ----------------------------------------------------------------------------------------------------------------

@@ -49,6 +49,40 @@ struct DecodeWs {
     int* ncand;                 // [B]
 };
 
+// The candidate test of the decoder: the first maximum over the classes of sigmoid(cls) (torch.max over dim) and whether it clears the
+// score threshold.  decode_candidates_kernel and reg_candidates_kernel both call it, so the regression rows computed for the decoder are
+// always a superset of the rows it reads.
+__device__ __forceinline__ bool anchor_score(const float* cp, int ncls, float score_thr, float& best, int& label) {
+    best = -1.f; label = 0;
+    for (int c = 0; c < ncls; ++c) {
+        float p = sigmoid_ref(__ldg(cp + c));
+        if (p > best) { best = p; label = c; }     // first maximum wins (torch.max over dim)
+    }
+    return best > score_thr;
+}
+
+// The (pixel, anchor group) pairs whose regression values the decoder may read: some anchor of the group is inside the anchor mask and
+// passes anchor_score.  The decoder's z_mean > 0 test is not applied: the list is a superset of what it reads, never a subset.
+// One thread per (image, pixel, group); pair -> list[group][slot] = b * P + pixel, counts[group] (zeroed by the caller) = slots used.
+// The capacity of each group is B * P, so the list cannot overflow.  The order of the slots is not fixed: the gathered conv computes
+// every row on its own.
+__global__ void reg_candidates_kernel(const float* __restrict__ cls, const uint8_t* __restrict__ mask, int B, int P, int A, int ncls,
+                                      float score_thr, int ga, int groups, int32_t* __restrict__ list, int32_t* __restrict__ counts) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= (long long)B * P * groups) return;
+    const int grp = (int)(idx % groups);
+    const long long pix = idx / groups;                       // b * P + pixel
+    bool any = false;
+    for (int a = grp * ga; a < min(A, (grp + 1) * ga) && !any; ++a) {
+        const long long n = pix * A + a;                      // b * N + anchor
+        float best; int label;
+        any = mask[n] && anchor_score(cls + n * (ncls + 1), ncls, score_thr, best, label);
+    }
+    if (!any) return;
+    const int slot = atomicAdd(counts + grp, 1);
+    list[(long long)grp * B * P + slot] = (int32_t)pix;
+}
+
 __global__ void decode_candidates_kernel(const float* __restrict__ cls, const float* __restrict__ reg, const float* __restrict__ anchors,
                                          const float* __restrict__ mean_std, const uint8_t* __restrict__ mask,
                                          int B, int N, int ncls, int T, float score_thr, float img_w, float img_h, int cap, DecodeWs ws) {
@@ -57,12 +91,8 @@ __global__ void decode_candidates_kernel(const float* __restrict__ cls, const fl
     int n = (int)(idx % N), b = (int)(idx / N);
     if (!mask[idx]) return;
     const float* cp = cls + idx * (ncls + 1);
-    float best = -1.f; int label = 0;
-    for (int c = 0; c < ncls; ++c) {
-        float p = sigmoid_ref(__ldg(cp + c));
-        if (p > best) { best = p; label = c; }     // first maximum wins (torch.max over dim)
-    }
-    if (!(best > score_thr)) return;
+    float best; int label;
+    if (!anchor_score(cp, ncls, score_thr, best, label)) return;
     const float* ms = mean_std + ((long long)n * T + label) * 12;   // [6][2]
     float z_mean = __ldg(ms + 0);
     if (!(z_mean > 0.f)) return;                                    // `mask = selected_mean_std[:,0,0] > 0` (:242)
@@ -343,6 +373,18 @@ extern "C" int vd3d_anchor_mask(const float* anchors, const float* means_z, cons
     VD3D_REQUIRE(anchors && means_z && P2 && mask && B > 0 && N > 0 && T > 0, "anchor_mask: bad args");
     anchor_mask_kernel<<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(anchors, means_z, P2, B, N, T, y_min, y_max, x_thr, mask);
     VD3D_CHECK_LAUNCH("anchor_mask");
+    return VD3D_OK;
+}
+
+extern "C" int vd3d_reg_candidates(const float* cls, const uint8_t* mask, int B, int P, int A, int ncls, float score_thr, int group_anchors,
+                                   int32_t* list, int32_t* counts, void* stream) {
+    VD3D_REQUIRE(cls && mask && list && counts && B > 0 && P > 0 && A > 0 && ncls > 0 && group_anchors > 0, "reg_candidates: bad args");
+    VD3D_REQUIRE((long long)B * P * A < (1LL << 31), "reg_candidates: too many anchors for the 32-bit list");
+    const int groups = cdiv(A, group_anchors);
+    cudaStream_t st = (cudaStream_t)stream;
+    VD3D_CUDA(cudaMemsetAsync(counts, 0, sizeof(int32_t) * groups, st));
+    reg_candidates_kernel<<<cdiv((long long)B * P * groups, 256), 256, 0, st>>>(cls, mask, B, P, A, ncls, score_thr, group_anchors, groups, list, counts);
+    VD3D_CHECK_LAUNCH("reg_candidates");
     return VD3D_OK;
 }
 

@@ -4,6 +4,7 @@ batched decode + NMS of the anchor-based 3-D detectors Stereo3D, Yolo3D and Grou
 from __future__ import annotations
 
 import contextlib
+import os
 
 import torch
 import torch.nn as nn
@@ -153,23 +154,47 @@ class Anchor3DDetector(NativeDetector):
         return self._anchor_tables[key]
 
     # ---- head outputs -> detections -------------------------------------------------------------------------
-    def decode(self, cls: E.Act, reg: E.Act, P2: torch.Tensor, H: int, W: int) -> E.DecodeNms:
-        """get_anchor + get_bboxes (R/heads/detection_3d_head.py:310-321,341-400), batched, no host sync."""
+    def sparse_reg(self, reg_out: E.ConvLayer, B: int, h: int, w: int) -> bool:
+        """Run the regression output conv `reg_out` inside `decode`, on the rows the decoder reads only (`ConvLayer.gather`), instead of over
+        the whole [B, h, w] map: the inference path, unless a stage hook wants the full `reg_preds` map or VD3D_SPARSE_REG=0.  Only when the
+        dense conv takes more than one round of 128-pixel x 128-column tiles on the SMs: a gathered tile walks the whole K loop as a dense one
+        does, so a one-round dense conv is as fast (Yolo3D at batch 1, DESIGN §4).  The detections are bit-identical either way."""
+        if self.stage_hook is not None or os.environ.get("VD3D_SPARSE_REG", "1") == "0" or not reg_out.gather_ok():
+            return False
+        dense_tiles = B * -(-h // 8) * -(-w // 16) * -(-reg_out.Cout // 128)
+        return dense_tiles > torch.cuda.get_device_properties(reg_out.w_hi.device).multi_processor_count
+
+    def run_reg_out(self, reg_out: E.ConvLayer, x: E.Act) -> E.Act:
+        """The dense regression output conv (R/heads/detection_3d_head.py:509-530): `x` -> reg_preds."""
+        return reg_out(x, self._arena.act("REG", (x.B, x.H, x.W, reg_out.Cout), x.t.device))
+
+    def decode(self, cls: E.Act, reg: E.Act, P2: torch.Tensor, H: int, W: int, reg_out: E.ConvLayer = None) -> E.DecodeNms:
+        """get_anchor + get_bboxes (R/heads/detection_3d_head.py:310-321,341-400), batched, no host sync.  `reg` is the regression map, or
+        with `reg_out` (`sparse_reg`) the input of that last conv, which then runs on the (pixel, anchor group) pairs whose anchors pass the
+        mask and the score threshold (`vd3d_reg_candidates`, a superset of the rows the decode reads)."""
         dev = cls.t.device
         B = cls.B
         tab = self._anchor_table(H, W, dev)
         N = tab.N
-        assert cls.H * cls.W * cls.C == N * self.num_cls_output and reg.C * reg.H * reg.W == N * 12
-        assert cls.co == 0 and reg.co == 0 and cls.cs == cls.C and reg.cs == reg.C
         mask = self._arena.get("mask", (B, N), dev, dtype=torch.uint8)
         if self.filter_anchor:
             E.anchor_mask(tab.anchors, tab.means_z, P2, mask, *self.anchor_filter)
         else:
             mask.fill_(1)
         self._hook("mask", mask)
+        score_thr = self.test_cfg.get("score_thr", 0.5)
+        if reg_out is not None:
+            A = self.num_anchors
+            groups = -(-A // E.REG_GROUP_ANCHORS)
+            lst = self._arena.get("reg_list", (groups, B * reg.H * reg.W), dev, dtype=torch.int32)
+            counts = self._arena.get("reg_counts", (groups,), dev, dtype=torch.int32)
+            E.reg_candidates(cls.t, mask, A, self.num_classes, score_thr, lst, counts)
+            reg = reg_out.gather(reg, lst, counts, self._arena.act("REG", (B, reg.H, reg.W, reg_out.Cout), dev))
+        assert cls.H * cls.W * cls.C == N * self.num_cls_output and reg.C * reg.H * reg.W == N * 12
+        assert cls.co == 0 and reg.co == 0 and cls.cs == cls.C and reg.cs == reg.C
         dec = self._decoder((B, str(dev)), lambda: E.DecodeNms(B, self.max_detections, dev))
         dec.run(cls.t.view(B, N, self.num_cls_output), reg.t.view(B, N, 12), tab.anchors, tab.mean_std, mask,
-                self.num_classes, self.test_cfg.get("score_thr", 0.5), self.test_cfg.get("nms_iou_thr", 0.5), W, H)
+                self.num_classes, score_thr, self.test_cfg.get("nms_iou_thr", 0.5), W, H)
         if self.post_optimization:
             # head.test_cfg.post_optimization (R/heads/detection_3d_head.py:294-308): yaw hill climbing of the kept car boxes deeper than
             # 3 m, in place on the fixed-capacity NMS output, stream-ordered (the reference searches on the CPU with one `.item()` per box)

@@ -72,6 +72,7 @@ class _Mono3DBase(Anchor3DDetector):
         return pl
 
     def run_reg(self, pl, feat: E.Act, P2, arena) -> E.Act:  # pragma: no cover
+        """the reg tower up to the input of its output conv pl["reg_out"]"""
         raise NotImplementedError
 
     def launch(self, images, P2):
@@ -86,7 +87,10 @@ class _Mono3DBase(Anchor3DDetector):
             E.split_lo(feat)
         self._hook("features", feat)
         cls = run_cls_tower(pl["cls"], feat, ar)
-        reg = self.run_reg(pl, feat, P2, ar)
+        x = self.run_reg(pl, feat, P2, ar)
+        if self.sparse_reg(pl["reg_out"], B, x.H, x.W):
+            return self.decode(cls, x, P2, H, W, reg_out=pl["reg_out"])
+        reg = self.run_reg_out(pl["reg_out"], x)
         self._hook("cls_preds", cls), self._hook("reg_preds", reg)
         return self.decode(cls, reg, P2, H, W)
 
@@ -114,7 +118,7 @@ class Yolo3D(_Mono3DBase):
         a = pl["reg1"](a, ar.act("R2", (B, h, w, pl["reg1"].Cout), dev, lo=True))
         if tc(pl["reg_out"]) and not tc(pl["reg1"]):
             E.split_lo(a)
-        return pl["reg_out"](a, ar.act("REG", (B, h, w, pl["reg_out"].Cout), dev))
+        return a
 
 
 @DETECTOR_DICT.register_module
@@ -141,7 +145,7 @@ class GroundAwareYolo3D(_Mono3DBase):
             a = pl[k](a, ar.act(name, (B, h, w, pl[k].Cout), dev, lo=True))
             if tc(nxt) and not tc(pl[k]):
                 E.split_lo(a)
-        return pl["reg_out"](a, ar.act("REG", (B, h, w, pl["reg_out"].Cout), dev))
+        return a
 
 
 def build_synthetic_mono3d(kind: str = "Yolo3D", seed: int = 0, depth: Optional[int] = None, workdir: Optional[str] = None):

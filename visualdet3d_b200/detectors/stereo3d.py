@@ -235,8 +235,9 @@ class Stereo3D(Anchor3DDetector):
         return pl
 
     # ---- forward ------------------------------------------------------------------------------------------
-    def core_forward(self, left: torch.Tensor, right: torch.Tensor) -> Tuple[E.Act, E.Act, E.Act]:
-        """R/detectors/yolostereo3d_core.py:110-126 + StereoMerging :88-94.  Returns (features, cls_preds, reg_preds) Acts."""
+    def core_forward(self, left: torch.Tensor, right: torch.Tensor, reg_out: bool = True) -> Tuple[E.Act, E.Act, E.Act]:
+        """R/detectors/yolostereo3d_core.py:110-126 + StereoMerging :88-94.  Returns (features, cls_preds, reg_preds) Acts; with
+        reg_out=False the last one is the input of the regression output conv (`decode` runs that conv on the rows it reads)."""
         pl = self.prepare()
         ar = self._arena
         dev = left.device
@@ -333,7 +334,9 @@ class Stereo3D(Anchor3DDetector):
         ro = pl["reg_out"]
         if tc(ro) and not tc(c2):
             E.split_lo(r3)
-        reg = ro(r3, ar.act("REG", (B, h16, w16, ro.Cout), dev))
+        if not reg_out:
+            return FEAT, cls, r3
+        reg = self.run_reg_out(ro, r3)
         self._hook("cls_preds", cls), self._hook("reg_preds", reg)
         return FEAT, cls, reg
 
@@ -341,9 +344,11 @@ class Stereo3D(Anchor3DDetector):
         """Enqueue the whole forward (backbone .. NMS) on the current stream; no host synchronisation.
         Returns the DecodeNms object holding the fixed-capacity device outputs."""
         left, right, P2 = self._device_inputs((left, "left"), (right, "right"), (P2, "P2"))
-        _, _, H, W = left.shape
-        _, cls, reg = self.core_forward(left, right)
-        return self.decode(cls, reg, P2, H, W)
+        B, _, H, W = left.shape
+        ro = self.prepare()["reg_out"]
+        sparse = self.sparse_reg(ro, B, H // 16, W // 16)
+        _, cls, reg = self.core_forward(left, right, reg_out=not sparse)
+        return self.decode(cls, reg, P2, H, W, reg_out=ro if sparse else None)
 
     def forward_batch(self, left, right, P2, P3=None):
         """B stereo pairs -> list of B (scores[K], bboxes[K,11], cls_indexes[K]) triples (new API; no reference counterpart).

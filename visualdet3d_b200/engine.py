@@ -286,6 +286,23 @@ class ConvLayer:
              r0.cs if r0 is not None else 0, r0.co if r0 is not None else 0,
              P(*[t.ptr for t in outs]) if f32_out else None, oh, ol, self.Cout, o.cs, o.co, 1 if relu else 0, self.passes, self.bn_tile, _stream())
 
+    def gather_ok(self) -> bool:
+        """`gather` runs this layer: fp16-split engine, stride 1, an output of the input's size"""
+        return self.engine == "tc16" and self.passes == 3 and self.stride == 1 and 2 * self.pad == self.dil * (self.KH - 1) == self.dil * (self.KW - 1)
+
+    def gather(self, x: Act, lst: torch.Tensor, counts: torch.Tensor, out: Act) -> Act:
+        """The conv (with its bias, no ReLU) at the listed output pixels only, one 96-column group of `out` at a time
+        (`vd3d_conv2d_tc16_gather`): `lst` [groups, B * H * W] int32 holds counts[g] pixels b * H * W + h * W + w for group g.  Bit-identical
+        to the dense conv there; every other element of `out` is left as it was."""
+        assert self.gather_ok() and not self.relu and x.C == self.Cin and out.C == self.Cout and (out.B, out.H, out.W) == (x.B, x.H, x.W)
+        self._check_tc16_input(x, "gathered conv")
+        xh, xl = x.h16_ptrs
+        call("vd3d_conv2d_tc16_gather", xh, xl, x.B, x.H, x.W, self.Cin, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale,
+             self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, lst.data_ptr(), counts.data_ptr(), counts.shape[0],
+             out.ptr, self.Cout, out.cs, out.co, _stream())
+        out.f32 = True
+        return out
+
     def run_levels(self, xs: Sequence[Act], outs: Sequence[Act], res: Optional[Sequence[Act]] = None, res_up: bool = False):
         """The conv on several tensors of different sizes in ONE persistent launch (vd3d_conv2d_tc16 over L levels): outs[l] = conv(xs[l])
         [+ res[l], nearest-upsampled when res_up].  Each form of `outs` (fp32, fp16 planes) and `res` must be views of one allocation with the
@@ -792,6 +809,20 @@ def anchor_mask(anchors: torch.Tensor, means_z: torch.Tensor, P2: torch.Tensor, 
     call("vd3d_anchor_mask", anchors.data_ptr(), means_z.data_ptr(), P2.data_ptr(), B, N, T,
          float(np.float32(y_min)), float(np.float32(y_max)), float(np.float32(x_thr)), mask.data_ptr(), _stream())
     return mask
+
+
+# Anchors per row group of the gathered regression conv: 8 anchors x 12 regression values = the 96 output columns of one of its N tiles
+REG_GROUP_ANCHORS = 8
+
+
+def reg_candidates(cls_preds: torch.Tensor, mask: torch.Tensor, A: int, ncls: int, score_thr: float, lst: torch.Tensor, counts: torch.Tensor):
+    """The (image, pixel, anchor group) pairs whose regression values the decoder may read (`vd3d_reg_candidates`): `cls_preds` NHWC [B, H, W, A *
+    (ncls + 1)], `mask` [B, P * A] with P = H * W -> `lst` [groups, B * P] int32, `counts` [groups] int32 (device)."""
+    B = cls_preds.shape[0]
+    P = cls_preds.numel() // (B * A * (ncls + 1))
+    assert lst.dtype == counts.dtype == torch.int32 and lst.shape == (counts.shape[0], B * P) and counts.shape[0] == -(-A // REG_GROUP_ANCHORS)
+    call("vd3d_reg_candidates", cls_preds.data_ptr(), mask.data_ptr(), B, P, A, ncls, float(np.float32(score_thr)), REG_GROUP_ANCHORS,
+         lst.data_ptr(), counts.data_ptr(), _stream())
 
 
 RANGE_MSG = ("an activation left the fp16 range (|v| >= 65520) in front of a tensor-core conv: the fp16-split engine keeps activations "
