@@ -118,6 +118,16 @@ int vd3d_conv2d_tc16_gather(const void* in_hi, const void* in_lo, int B, int H, 
                             const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
                             const int32_t* list, const int32_t* counts, int groups,
                             float* out, int Cout, int out_cs, int out_co, void* stream);
+/* The conv of vd3d_conv2d_tc16 (one tensor, stride 1, fp32 or plane residual, fp32 and / or plane output) on a device list of 8 x 16 output tiles
+ * (the regression tower on the tiles its candidates reach, vd3d_reg_tower_tiles): tiles [cap][4] i32 = (b, y0, x0, 0), any origin, 16-byte
+ * aligned; tile_count [1] i32 read on the device.  Each tile runs the dense conv's K loop and epilogue, so every stored element is bit-identical
+ * to vd3d_conv2d_tc16's; only pixels whose store_map [B][Ho][Wo] u8 byte is set are stored and checked by the fp16-range guard, so the input
+ * may hold anything (stale, non-finite) where no stored pixel reads it. */
+int vd3d_conv2d_tc16_tiles(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                           const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
+                           const float* res, const void* res_hi16, const void* res_lo16, int res_cs, int res_co,
+                           float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn,
+                           const int32_t* tiles, const int32_t* tile_count, const uint8_t* store_map, void* stream);
 /* Few-channel KHxKW convolution (the ResNet / DLA stem: conv1 7x7 stride 2, R/backbones/resnet.py:120,186) on the tensor cores.
  * The image is held as fp16 (hi, lo) planes [B][H][Wp][4] (pixel x at column x + pad, zeros elsewhere: the buffer must be
  * zero-initialised once); Wp = vd3d_stem_row_pitch(W, KW, stride, pad).  vd3d_image_to_h16_rows fills the planes from an
@@ -226,9 +236,20 @@ int vd3d_anchor_mask(const float* anchors, const float* means_z, const float* P2
  * a of the group (group_anchors consecutive anchors of the pixel, anchor n = pixel * A + a) has mask[b][n] and the decoder's first-max
  * sigmoid score > score_thr.  A superset of the anchors vd3d_decode_nms decodes (its prior z_mean > 0 test is not applied).
  *   cls [B][P*A][ncls+1], mask [B][P*A] u8 -> list [groups][B*P] i32 (b*P + pixel), counts [groups] i32, groups = ceil(A / group_anchors);
- *   counts are zeroed here; the list cannot overflow */
+ *   counts are zeroed here; the list cannot overflow.
+ *   pixmap [B][P] u8 (optional, NULL to skip): zeroed here, then 1 at every pixel listed in some group */
 int vd3d_reg_candidates(const float* cls, const uint8_t* mask, int B, int P, int A, int ncls, float score_thr, int group_anchors,
-                        int32_t* list, int32_t* counts, void* stream);
+                        int32_t* list, int32_t* counts, uint8_t* pixmap, void* stream);
+
+/* Tile lists of the regression tower under the regression output conv (vd3d_conv2d_tc16_tiles).  For depth d = 1 .. D (the output conv reads
+ * the tower's last conv within one pixel of a candidate, that conv reads the one before it within one more pixel, ...):
+ *   smaps [D][B][H][W] u8   : S_d = the pixels within d 3x3 steps of a set pixel of cand [B][H][W] (clipped to the image)
+ *   tiles [D][cap][4] i32   : (b, y0, x0, 0) of the 8 x 16 tiles of each image whose rows start at the image's first row of S_d and that hold a
+ *                             pixel of S_d, in the order image, tile row, tile column; cap = vd3d_reg_tower_tile_cap(B, H, W) (cannot overflow)
+ *   counts [D] i32          : entries of each list
+ * One launch, no host synchronisation.  2 H W + 4 (ceil(H / 8) + 1) ceil(W / 16) <= 48 KB. */
+int vd3d_reg_tower_tile_cap(int B, int H, int W);
+int vd3d_reg_tower_tiles(const uint8_t* cand, int B, int H, int W, int D, uint8_t* smaps, int32_t* tiles, int32_t* counts, void* stream);
 
 /* AnchorBasedDetection3DHead.get_bboxes (R/heads/detection_3d_head.py:341-400) + _decode (:218-263) +
  * ClipBoxes (R/utils/utils.py:181-196) + torchvision.ops.nms (class-agnostic, IoU > thr suppresses), batched.

@@ -56,6 +56,7 @@ _SIGS = {
     "vd3d_conv2d_tc16": (I, [I, P, P, P, P, I, I, I, I, P, P, F, P, I, I, I, I, I, P, P, P, P, P, I, I, P, P, P, I, I, I, I, I, I, P]),
     "vd3d_convtranspose2d_tc16": (I, [P, P, I, I, I, I, I, I, P, P, F, P, P, P, P, I, I, I, I, I, P]),
     "vd3d_conv2d_tc16_gather": (I, [P, P, I, I, I, I, I, I, P, P, F, P, I, I, I, I, P, P, I, P, I, I, I, P]),
+    "vd3d_conv2d_tc16_tiles": (I, [P, P, I, I, I, I, I, I, P, P, F, P, I, I, I, I, P, P, P, I, I, P, P, P, I, I, I, I, I, P, P, P, P]),
     "vd3d_stem_row_pitch": (I, [I, I, I, I]),
     "vd3d_image_to_h16_rows": (I, [P, I, I, I, I, P, P, I, I, P]),
     "vd3d_conv2d_tc16_stem": (I, [P, P, I, I, I, I, I, I, I, I, I, P, P, F, P, P, P, P, I, I, I, I, P]),
@@ -98,7 +99,9 @@ _SIGS = {
     "vd3d_pack_records_geo": (I, [P, P, P, P, P, P, P, I, I, I, P, P]),
     "vd3d_look_ground_sample": (I, [P, I, I, I, I, I, I, P, I, I, P, F, F, P, P, I, P]),
     "vd3d_anchor_mask": (I, [P, P, P, I, I, I, F, F, F, P, P]),
-    "vd3d_reg_candidates": (I, [P, P, I, I, I, I, F, I, P, P, P]),
+    "vd3d_reg_candidates": (I, [P, P, I, I, I, I, F, I, P, P, P, P]),
+    "vd3d_reg_tower_tile_cap": (I, [I, I, I]),
+    "vd3d_reg_tower_tiles": (I, [P, I, I, I, I, P, P, P, P]),
     "vd3d_decode_nms_workspace": (c_longlong, [I, I]),
     "vd3d_decode_nms": (I, [P, P, P, P, P, I, I, I, I, F, c_double, F, F, I, P, P, P, P, P, P, P, P]),
     "vd3d_retina_decode_workspace": (c_longlong, [I, I, I]),

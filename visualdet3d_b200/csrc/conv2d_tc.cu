@@ -159,9 +159,9 @@ __device__ __forceinline__ float tcp_epi_tile(const TcParams& p, const float* ti
         for (int i = 0; i < U; ++i) {
             const int idx = i0 + i * TCP_EPI;
             const int r = idx / CG, g = idx - r * CG;
-            const int ho = geo.th * TC_TH + r / TC_TW, wo = geo.tw * TC_TW + r % TC_TW;
+            const int ho = geo.h0 + r / TC_TW, wo = geo.w0 + r % TC_TW;
             const int n = nt * BN + 8 * g;
-            rg[i] = (idx < ITEMS && ho < geo.Ho && wo < geo.Wo && 8 * g < ncols && n + 4 <= p.Cout) ? idx : -1;
+            rg[i] = (idx < ITEMS && 8 * g < ncols && n + 4 <= p.Cout && tcp_stores(p, geo, ho, wo)) ? idx : -1;
             pix[i] = tcp_out_pix(geo, ho, wo);
             if (rg[i] >= 0) tcp_epi_res(p, tcp_res_pix(geo, ho, wo), n, rr[i]);
         }
@@ -214,8 +214,6 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;      // (warp-uniform for the compiler)
     const int cchunks = p.cin_pad / kbc;
     const int KB = p.KH * p.KW * cchunks;
-    const int mt_units = p.m_tiles;
-    const int units = mt_units * p.n_tiles;
     const int u0 = (int)blockIdx.x, ustep = (int)gridDim.x;
     const int mode = tc_mma_mode(p);
 
@@ -228,7 +226,10 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
     }
     __syncthreads();
     pdl_launch_dependents();
-    pdl_wait();                            // (PDL launches only) the producer of the activations / residual has completed
+    pdl_wait();                            // (PDL launches only) the producer of the activations / residual (and of a tile list) has completed
+    // every role reads the same count: the producer, the consumers and the epilogue walk the same units
+    const int mt_units = tcp_m_tiles(p);
+    const int units = mt_units * p.n_tiles;
 
     if (warp >= TC_CONSUMERS / 32) {
         // (epilogue-warp tiles) every warp of a warpgroup executes the same setmaxnreg: before the producer / epilogue split
@@ -282,7 +283,7 @@ conv2d_tcp_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constan
                     unit_tile(p, u, mt_units, mu, nt);
                     const TcGeom geo = tile_geom(p, mu);
                     const int b = geo.b;
-                    const int wi0 = geo.tw * TC_TW * p.stride_w - geo.pad_w, hi0 = geo.th * TC_TH * p.stride - geo.pad_h;
+                    const int wi0 = geo.w0 * p.stride_w - geo.pad_w, hi0 = geo.h0 * p.stride - geo.pad_h;
                     const CUtensorMap* mA = &mapA;
                     const CUtensorMap* mAlo = &mapAlo;
                     if constexpr (LV) { mA = &lmaps.a[geo.lvl]; mAlo = &lmaps.alo[geo.lvl]; }
@@ -775,6 +776,7 @@ struct ConvSpec {
     float* out; float* out_lo; void* out_h16_hi; void* out_h16_lo;
     int Cout, out_cs, out_co, relu, passes, bn;
     int convt;
+    const int4* tlist; const int* tcount; const uint8_t* smap;     // tile-listed launch (TcParams::tlist)
 };
 
 // output size of level l: the conv's, or (convt) the input's -- each phase writes one pixel of every 2x2 output cell
@@ -884,6 +886,12 @@ static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
         p.res_up_H = res_up_H; p.res_up_W = res_up_W;
     }
     p.two_pass = two_pass;
+    if (s.tlist) {
+        // the list's origins are output pixels of a stride-1 conv over one tensor; the fused pool writes whole pooled tiles
+        VD3D_REQUIRE(s.L == 1 && stride == 1 && f16 && passes == 3 && !two_pass && !s.convt && s.res_W[0] == 0 && s.tcount && s.smap,
+                     "conv2d_tc16_tiles: a tile list needs a one-tensor, stride-1 fp16-split conv, its device count and a store map");
+        p.tlist = s.tlist; p.tcount = s.tcount; p.smap = s.smap;
+    }
     p.range_flag = s.out_h16_hi ? fp16_range_flag() : nullptr;
     {
         const char* e = getenv("VD3D_TC_CHUNK");
@@ -895,7 +903,7 @@ static int conv2d_tc_launch(const ConvSpec& s, void* stream) {
         // MMA-mode timing experiments (VD3D_TC_DEBUG bits 0 and 1), which only conv2d_tcp_kernel implements.
         const char* e = getenv("VD3D_ROW64");
         const char* d = getenv("VD3D_TC_DEBUG");
-        if (s.L == 1 && conv2d_row64_eligible(p) && !(e && atoi(e) == 0) && !(d && (atoi(d) & 3)))
+        if (s.L == 1 && !s.tlist && conv2d_row64_eligible(p) && !(e && atoi(e) == 0) && !(d && (atoi(d) & 3)))
             return conv2d_row64_launch(p, s.in[0], s.in_lo[0], s.in_cs, s.in_co, s.w_hi, s.w_lo, stream);
     }
     const int K = KH * KW * p.cin_pad;
@@ -973,6 +981,30 @@ extern "C" int vd3d_conv2d_tc16(int L, const void* const* in_hi, const void* con
     s.res_h16_hi = res_hi16 ? res_hi16[0] : nullptr; s.res_h16_lo = res_lo16 ? res_lo16[0] : nullptr;
     s.out = out ? (float*)out[0] : nullptr; s.out_h16_hi = out_hi16 ? (void*)out_hi16[0] : nullptr; s.out_h16_lo = out_lo16 ? (void*)out_lo16[0] : nullptr;
     s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = passes; s.bn = bn;
+    return conv2d_tc_launch(s, stream);
+}
+
+// The conv of vd3d_conv2d_tc16 (one tensor, stride 1) on a device list of 8 x 16 output tiles: tiles [cap] of (b, y0, x0, 0), tile_count[0] of
+// them, each computed by the dense conv's K loop and epilogue (the same bits), stored only where store_map [B][Ho][Wo] is set.
+extern "C" int vd3d_conv2d_tc16_tiles(const void* in_hi, const void* in_lo, int B, int H, int W, int Cin, int in_cs, int in_co,
+                                      const void* w_hi, const void* w_lo, float out_scale, const float* bias, int KH, int KW, int pad, int dil,
+                                      const float* res, const void* res_hi16, const void* res_lo16, int res_cs, int res_co,
+                                      float* out, void* out_hi16, void* out_lo16, int Cout, int out_cs, int out_co, int relu, int bn,
+                                      const int32_t* tiles, const int32_t* tile_count, const uint8_t* store_map, void* stream) {
+    VD3D_REQUIRE(in_hi && in_lo && tiles && tile_count && store_map && (out || out_hi16) && (!out_hi16 == !out_lo16) && (!res_hi16 == !res_lo16) &&
+                 B > 0 && H > 0 && W > 0, "conv2d_tc16_tiles: input planes, a tile list, its count, a store map and an output are required");
+    VD3D_REQUIRE(((((uintptr_t)in_hi | (uintptr_t)in_lo) & 15) == 0) && ((uintptr_t)tiles & 15) == 0,
+                 "conv2d_tc16_tiles: 16-byte aligned input planes and tile list are required");
+    ConvSpec s;
+    memset(&s, 0, sizeof(s));
+    s.f16 = 1; s.L = 1; s.B = B; s.Cin = Cin; s.in_cs = in_cs; s.in_co = in_co;
+    s.in[0] = in_hi; s.in_lo[0] = in_lo; s.H[0] = H; s.W[0] = W;
+    s.w_hi = w_hi; s.w_lo = w_lo; s.out_scale = out_scale; s.bias = bias;
+    s.KH = KH; s.KW = KW; s.pad = pad; s.dil = dil; s.stride = 1;
+    s.res = res; s.res_h16_hi = res_hi16; s.res_h16_lo = res_lo16; s.res_cs = res_cs; s.res_co = res_co;
+    s.out = out; s.out_h16_hi = out_hi16; s.out_h16_lo = out_lo16;
+    s.Cout = Cout; s.out_cs = out_cs; s.out_co = out_co; s.relu = relu; s.passes = 3; s.bn = bn;
+    s.tlist = reinterpret_cast<const int4*>(tiles); s.tcount = tile_count; s.smap = store_map;
     return conv2d_tc_launch(s, stream);
 }
 

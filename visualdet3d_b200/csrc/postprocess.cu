@@ -66,8 +66,10 @@ __device__ __forceinline__ bool anchor_score(const float* cp, int ncls, float sc
 // One thread per (image, pixel, group); pair -> list[group][slot] = b * P + pixel, counts[group] (zeroed by the caller) = slots used.
 // The capacity of each group is B * P, so the list cannot overflow.  The order of the slots is not fixed: the gathered conv computes
 // every row on its own.
+// pixmap (optional, zeroed by the caller): byte b * P + pixel set when the pixel is listed in some group.
 __global__ void reg_candidates_kernel(const float* __restrict__ cls, const uint8_t* __restrict__ mask, int B, int P, int A, int ncls,
-                                      float score_thr, int ga, int groups, int32_t* __restrict__ list, int32_t* __restrict__ counts) {
+                                      float score_thr, int ga, int groups, int32_t* __restrict__ list, int32_t* __restrict__ counts,
+                                      uint8_t* __restrict__ pixmap) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)B * P * groups) return;
     const int grp = (int)(idx % groups);
@@ -81,6 +83,66 @@ __global__ void reg_candidates_kernel(const float* __restrict__ cls, const uint8
     if (!any) return;
     const int slot = atomicAdd(counts + grp, 1);
     list[(long long)grp * B * P + slot] = (int32_t)pix;
+    if (pixmap) pixmap[pix] = 1;
+}
+
+// Tile lists of the regression tower (vd3d_reg_tower_tiles).  Block d - 1 builds depth d: S_d = the pixels within d 3x3 steps of a candidate
+// pixel (a (2 d + 1)^2 window, clipped to the image: separable, rows then columns, in shared memory), and per image the 8 x 16 tiles whose
+// rows start at the first row of S_d and which hold a pixel of S_d, listed in the order image, tile row, tile column (warp 0 compacts the
+// tile flags 32 at a time), so the list does not depend on the schedule.
+__global__ void reg_tower_tiles_kernel(const uint8_t* __restrict__ cand, int B, int H, int W, uint8_t* __restrict__ smaps,
+                                       int4* __restrict__ tiles, int cap, int32_t* __restrict__ counts) {
+    extern __shared__ uint8_t sh[];
+    const int d = (int)blockIdx.x + 1, HW = H * W, TW = (W + 15) / 16, TH = (H + 7) / 8 + 1;
+    uint8_t* rows = sh;                                       // [H][W] candidates dilated along the row
+    uint8_t* set = sh + HW;                                   // [H][W] S_d
+    int* flag = reinterpret_cast<int*>(sh + ((2 * HW + 15) & ~15));     // [TH][TW]
+    __shared__ int ymin;
+    int base = 0;                                             // (warp 0) entries listed so far
+    uint8_t* smap = smaps + (long long)blockIdx.x * B * HW;
+    int4* list = tiles + (long long)blockIdx.x * cap;
+    for (int b = 0; b < B; ++b) {
+        const uint8_t* c = cand + (long long)b * HW;
+        if (threadIdx.x == 0) ymin = H;
+        for (int i = threadIdx.x; i < TH * TW; i += blockDim.x) flag[i] = 0;
+        for (int i = threadIdx.x; i < HW; i += blockDim.x) {
+            const int y = i / W, x = i - y * W;
+            uint8_t v = 0;
+            for (int xx = max(0, x - d); xx <= min(W - 1, x + d); ++xx) v |= c[y * W + xx];
+            rows[i] = v;
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < HW; i += blockDim.x) {
+            const int y = i / W, x = i - y * W;
+            uint8_t v = 0;
+            for (int yy = max(0, y - d); yy <= min(H - 1, y + d); ++yy) v |= rows[yy * W + x];
+            v = v ? 1 : 0;
+            set[i] = v;
+            smap[(long long)b * HW + i] = v;
+            if (v) atomicMin(&ymin, y);
+        }
+        __syncthreads();
+        const int y0 = ymin;
+        for (int i = threadIdx.x; i < HW; i += blockDim.x) {
+            const int y = i / W, x = i - y * W;
+            if (set[i]) flag[((y - y0) >> 3) * TW + (x >> 4)] = 1;
+        }
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            for (int t0 = 0; t0 < TH * TW; t0 += 32) {
+                const int t = t0 + (int)threadIdx.x;
+                const bool on = t < TH * TW && flag[t];
+                const unsigned bal = __ballot_sync(0xffffffffu, on);
+                if (on) {
+                    const int ty = t / TW, tx = t - ty * TW;
+                    list[base + __popc(bal & ((1u << threadIdx.x) - 1u))] = make_int4(b, y0 + 8 * ty, 16 * tx, 0);
+                }
+                base += __popc(bal);
+            }
+        }
+        __syncthreads();                                      // rows / set / flag / ymin are reused by the next image
+    }
+    if (threadIdx.x == 0) counts[blockIdx.x] = base;
 }
 
 __global__ void decode_candidates_kernel(const float* __restrict__ cls, const float* __restrict__ reg, const float* __restrict__ anchors,
@@ -377,14 +439,31 @@ extern "C" int vd3d_anchor_mask(const float* anchors, const float* means_z, cons
 }
 
 extern "C" int vd3d_reg_candidates(const float* cls, const uint8_t* mask, int B, int P, int A, int ncls, float score_thr, int group_anchors,
-                                   int32_t* list, int32_t* counts, void* stream) {
+                                   int32_t* list, int32_t* counts, uint8_t* pixmap, void* stream) {
     VD3D_REQUIRE(cls && mask && list && counts && B > 0 && P > 0 && A > 0 && ncls > 0 && group_anchors > 0, "reg_candidates: bad args");
     VD3D_REQUIRE((long long)B * P * A < (1LL << 31), "reg_candidates: too many anchors for the 32-bit list");
     const int groups = cdiv(A, group_anchors);
     cudaStream_t st = (cudaStream_t)stream;
     VD3D_CUDA(cudaMemsetAsync(counts, 0, sizeof(int32_t) * groups, st));
-    reg_candidates_kernel<<<cdiv((long long)B * P * groups, 256), 256, 0, st>>>(cls, mask, B, P, A, ncls, score_thr, group_anchors, groups, list, counts);
+    if (pixmap) VD3D_CUDA(cudaMemsetAsync(pixmap, 0, (size_t)B * P, st));
+    reg_candidates_kernel<<<cdiv((long long)B * P * groups, 256), 256, 0, st>>>(cls, mask, B, P, A, ncls, score_thr, group_anchors, groups, list, counts,
+                                                                               pixmap);
     VD3D_CHECK_LAUNCH("reg_candidates");
+    return VD3D_OK;
+}
+
+extern "C" int vd3d_reg_tower_tile_cap(int B, int H, int W) { return B * (cdiv(H, 8) + 1) * cdiv(W, 16); }
+
+// shared memory of reg_tower_tiles_kernel: two [H][W] byte maps and the [cdiv(H, 8) + 1][cdiv(W, 16)] tile flags
+static size_t tower_tiles_smem(int H, int W) { return (size_t)((2 * H * W + 15) & ~15) + sizeof(int) * (cdiv(H, 8) + 1) * cdiv(W, 16); }
+
+extern "C" int vd3d_reg_tower_tiles(const uint8_t* cand, int B, int H, int W, int D, uint8_t* smaps, int32_t* tiles, int32_t* counts, void* stream) {
+    VD3D_REQUIRE(cand && smaps && tiles && counts && B > 0 && H > 0 && W > 0 && D >= 1 && D <= 16, "reg_tower_tiles: bad args");
+    VD3D_REQUIRE(((uintptr_t)tiles & 15) == 0, "reg_tower_tiles: the tile list must be 16-byte aligned");
+    VD3D_REQUIRE(tower_tiles_smem(H, W) <= 48 * 1024, "reg_tower_tiles: a %dx%d map does not fit the kernel's shared memory", H, W);
+    reg_tower_tiles_kernel<<<D, 512, tower_tiles_smem(H, W), (cudaStream_t)stream>>>(cand, B, H, W, smaps, reinterpret_cast<int4*>(tiles),
+                                                                                   vd3d_reg_tower_tile_cap(B, H, W), counts);
+    VD3D_CHECK_LAUNCH("reg_tower_tiles");
     return VD3D_OK;
 }
 

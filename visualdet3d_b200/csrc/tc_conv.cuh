@@ -60,6 +60,11 @@ struct TcParams {
     // its own tap origin, weight rows and interleaved output pixels (TcLevel::pad_h / pad_w / w_row / up).
     int n_levels;
     TcLevel lv[TC_MAX_LEVELS];
+    // Tile-listed launch (vd3d_conv2d_tc16_tiles; one level, stride 1): the M tiles are the entries (b, y0, x0, 0) of `tlist`, 8 x 16 output tiles
+    // whose origin may be any pixel, and there are tcount[0] of them (read on the device, so the list can be built by an earlier kernel of the
+    // stream); only the pixels whose byte of `smap` [B][Ho][Wo] is set are stored (and feed the fp16-range guard).  m_tiles stays the dense
+    // count: it sizes the grid and the L2 blocks.
+    const int4* tlist; const int* tcount; const uint8_t* smap;
 };
 
 // 8 consecutive channels (16-byte aligned)
@@ -201,15 +206,20 @@ template <int V> using tc_int = std::integral_constant<int, V>;
 // Epilogue arithmetic of the persistent kernels, per 8 output channels n .. n + 7 of one output pixel `pix` (n + 4 <= Cout; when n + 8 > Cout,
 // the Cout % 8 == 4 tail, only the first four are read and written).  Split in two so that an epilogue can have the residual loads of
 // several groups in flight before it computes the first.
-// Output geometry of M tile mu: tile column / row, image, the output size, and the pixel offsets of the output and the residual (the level's,
+// Output geometry of M tile mu: the output pixel of the tile's (0, 0) (a multiple of the tile size, or a list entry's origin), image, the output size, and the pixel offsets of the output and the residual (the level's,
 // in a multi-level launch; zero otherwise).  The level table is indexed with compile-time indices only, so it stays in parameter space.
 // Tap origin (pad_h, pad_w), first weight row (w_row) and output pixel map (up) of the tile's level: p.pad / p.pad_w, 0 and 0 outside
 // multi-level launches.
-struct TcGeom { int tw, th, b, Ho, Wo, lvl, res_H, res_W, pad_h, pad_w, w_row, up; long long pix_off, res_off; };
+struct TcGeom { int w0, h0, b, Ho, Wo, lvl, res_H, res_W, pad_h, pad_w, w_row, up; long long pix_off, res_off; };
 __device__ __forceinline__ TcGeom tile_geom(const TcParams& p, int mu) {
     TcGeom g;
     g.lvl = 0; g.Ho = p.Ho; g.Wo = p.Wo; g.res_H = p.res_up_H; g.res_W = p.res_up_W; g.pix_off = 0; g.res_off = 0;
     g.pad_h = p.pad; g.pad_w = p.pad_w; g.w_row = 0; g.up = 0;
+    if (p.tlist) {
+        const int4 e = __ldg(p.tlist + mu);
+        g.b = e.x; g.h0 = e.y; g.w0 = e.z;
+        return g;
+    }
     int tiles_w = p.tiles_w, tiles_h = p.tiles_h;
     if (p.n_levels > 0) {
 #pragma unroll
@@ -223,10 +233,16 @@ __device__ __forceinline__ TcGeom tile_geom(const TcParams& p, int mu) {
         for (int i = 0; i < TC_MAX_LEVELS; ++i)
             if (i == g.lvl) mu -= p.lv[i].m_begin;
     }
-    g.tw = mu % tiles_w; mu /= tiles_w;
-    g.th = mu % tiles_h; g.b = mu / tiles_h;
+    g.w0 = (mu % tiles_w) * TC_TW; mu /= tiles_w;
+    g.h0 = (mu % tiles_h) * TC_TH; g.b = mu / tiles_h;
     return g;
 }
+// Whether the epilogue stores output pixel (ho, wo) of the tile: inside the output and (tile-listed launches) set in the store map.
+__device__ __forceinline__ bool tcp_stores(const TcParams& p, const TcGeom& g, int ho, int wo) {
+    return ho < g.Ho && wo < g.Wo && (!p.smap || __ldg(p.smap + ((long long)g.b * g.Ho + ho) * g.Wo + wo));
+}
+// M tiles of a launch: the dense count, or the device count of a tile-listed launch (read after pdl_wait)
+__device__ __forceinline__ int tcp_m_tiles(const TcParams& p) { return p.tcount ? __ldg(p.tcount) : p.m_tiles; }
 // Output pixel of (b, ho, wo), and its residual pixel: the same pixel, or (res_W > 0) pixel (ho >> 1, wo >> 1) of the half-resolution
 // residual, i.e. the nearest-neighbour x2 upsampling of the FPN top-down path fused into the residual read.  A sub-pixel phase level (up = 1)
 // writes pixel (2 ho, 2 wo) of the [B][2 Ho][2 Wo] output; its pix_off (2 W r + s for phase (r, s)) picks the phase's pixel of each 2x2 cell.
@@ -327,9 +343,9 @@ __device__ __forceinline__ float tcp_store_tile(const TcParams& p, const float* 
     const int ncols = min(HALF, min(p.BN, p.cout_pad - nt * p.BN) - cb);      // valid columns of this thread in this tile (<= 0: none)
     const TcGeom g = tile_geom(p, mu);
     const int r = q * 32 + lane;
-    const int ho = g.th * TC_TH + r / TC_TW, wo = g.tw * TC_TW + r % TC_TW;
+    const int ho = g.h0 + r / TC_TW, wo = g.w0 + r % TC_TW;
     float amax = 0.f;
-    if (!(ho < g.Ho && wo < g.Wo) || ncols <= 0 || (p.dbg & 16)) return amax;
+    if (!tcp_stores(p, g, ho, wo) || ncols <= 0 || (p.dbg & 16)) return amax;
     const long long pix = tcp_out_pix(g, ho, wo);
     const long long rpix = tcp_res_pix(g, ho, wo);
     const float* acc = tile + r * ld;

@@ -164,14 +164,34 @@ class Anchor3DDetector(NativeDetector):
         dense_tiles = B * -(-h // 8) * -(-w // 16) * -(-reg_out.Cout // 128)
         return dense_tiles > torch.cuda.get_device_properties(reg_out.w_hi.device).multi_processor_count
 
+    def reg_tower(self, pl) -> list:
+        """The 3x3 convs at the end of the regression tower that `decode` may run on tile lists (its `tower`); none by default."""
+        return []
+
+    @staticmethod
+    def tower_tiles_ok(tower, reg_out: E.ConvLayer, h: int, w: int) -> bool:
+        """`decode` can run the regression tower `tower` on tile lists over an h x w map: every conv of it and the output conv read their
+        input within one pixel (`ConvLayer.tiles_ok`), and the map fits the list builder (`vd3d_reg_tower_tiles`)"""
+        return bool(tower) and reg_out.tiles_ok() and all(layer.tiles_ok() for layer, _, _ in tower) and E.tower_tiles_fit(h, w)
+
+    def tiled_tower(self, pl, sparse: bool, h: int, w: int):
+        """`decode`'s `tower` for a run with the `sparse_reg` decision `sparse` over an h x w map: `reg_tower(pl)` when it can run on tile
+        lists, else () (the caller runs the tower densely)."""
+        tower = self.reg_tower(pl) if sparse else []
+        return tower if self.tower_tiles_ok(tower, pl["reg_out"], h, w) else ()
+
     def run_reg_out(self, reg_out: E.ConvLayer, x: E.Act) -> E.Act:
         """The dense regression output conv (R/heads/detection_3d_head.py:509-530): `x` -> reg_preds."""
         return reg_out(x, self._arena.act("REG", (x.B, x.H, x.W, reg_out.Cout), x.t.device))
 
-    def decode(self, cls: E.Act, reg: E.Act, P2: torch.Tensor, H: int, W: int, reg_out: E.ConvLayer = None) -> E.DecodeNms:
+    def decode(self, cls: E.Act, reg: E.Act, P2: torch.Tensor, H: int, W: int, reg_out: E.ConvLayer = None, tower=()) -> E.DecodeNms:
         """get_anchor + get_bboxes (R/heads/detection_3d_head.py:310-321,341-400), batched, no host sync.  `reg` is the regression map, or
         with `reg_out` (`sparse_reg`) the input of that last conv, which then runs on the (pixel, anchor group) pairs whose anchors pass the
-        mask and the score threshold (`vd3d_reg_candidates`, a superset of the rows the decode reads)."""
+        mask and the score threshold (`vd3d_reg_candidates`, a superset of the rows the decode reads).
+        `tower` (with `reg_out`, `tower_tiles_ok`): the convs in front of `reg_out` as (layer, arena name, index of the earlier tower output
+        added as residual or None); `reg` is then the tower's input.  Conv j of D runs on the 8 x 16 tiles holding the pixels within D - j
+        steps of a candidate pixel (`vd3d_reg_tower_tiles`), which is where `reg_out` reads it through the later convs: bit-identical
+        detections, the tower's outputs stale elsewhere."""
         dev = cls.t.device
         B = cls.B
         tab = self._anchor_table(H, W, dev)
@@ -188,7 +208,10 @@ class Anchor3DDetector(NativeDetector):
             groups = -(-A // E.REG_GROUP_ANCHORS)
             lst = self._arena.get("reg_list", (groups, B * reg.H * reg.W), dev, dtype=torch.int32)
             counts = self._arena.get("reg_counts", (groups,), dev, dtype=torch.int32)
-            E.reg_candidates(cls.t, mask, A, self.num_classes, score_thr, lst, counts)
+            pix = self._arena.get("reg_pix", (B, reg.H, reg.W), dev, dtype=torch.uint8) if tower else None
+            E.reg_candidates(cls.t, mask, A, self.num_classes, score_thr, lst, counts, pix)
+            if tower:
+                reg = self._run_tower(tower, reg, pix)
             reg = reg_out.gather(reg, lst, counts, self._arena.act("REG", (B, reg.H, reg.W, reg_out.Cout), dev))
         assert cls.H * cls.W * cls.C == N * self.num_cls_output and reg.C * reg.H * reg.W == N * 12
         assert cls.co == 0 and reg.co == 0 and cls.cs == cls.C and reg.cs == reg.C
@@ -200,6 +223,22 @@ class Anchor3DDetector(NativeDetector):
             # 3 m, in place on the fixed-capacity NMS output, stream-ordered (the reference searches on the CPU with one `.item()` per box)
             dec.post_opt(P2)
         return dec
+
+    def _run_tower(self, tower, x: E.Act, pix: torch.Tensor) -> E.Act:
+        """The regression tower (`decode`'s `tower`) on the tile lists built from the candidate pixel map `pix` [B, h, w]."""
+        B, h, w, dev = x.B, x.H, x.W, x.t.device
+        D = len(tower)
+        smaps = self._arena.get("tower_smap", (D, B, h, w), dev, dtype=torch.uint8)
+        tiles = self._arena.get("tower_tiles", (D, E.tower_tile_cap(B, h, w), 4), dev, dtype=torch.int32)
+        tcount = self._arena.get("tower_count", (D,), dev, dtype=torch.int32)
+        E.tower_tiles(pix, smaps, tiles, tcount)
+        outs = []
+        for j, (layer, name, res) in enumerate(tower):
+            d = D - j
+            x = layer(x, self._arena.act(name, (B, h, w, layer.Cout), dev, lo=True), res=outs[res] if res is not None else None,
+                      tiles=(tiles[d - 1], tcount[d - 1:d], smaps[d - 1]))
+            outs.append(x)
+        return x
 
 
 def synth_load(det: nn.Module, seed: int):

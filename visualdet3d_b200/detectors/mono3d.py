@@ -71,8 +71,8 @@ class _Mono3DBase(Anchor3DDetector):
         pl.update(self.reg_plan(dev))
         return pl
 
-    def run_reg(self, pl, feat: E.Act, P2, arena) -> E.Act:  # pragma: no cover
-        """the reg tower up to the input of its output conv pl["reg_out"]"""
+    def run_reg(self, pl, feat: E.Act, P2, arena, tower: bool = True) -> E.Act:  # pragma: no cover
+        """the reg tower up to the input of its output conv pl["reg_out"]; tower=False: up to the input of `reg_tower(pl)`"""
         raise NotImplementedError
 
     def launch(self, images, P2):
@@ -87,9 +87,11 @@ class _Mono3DBase(Anchor3DDetector):
             E.split_lo(feat)
         self._hook("features", feat)
         cls = run_cls_tower(pl["cls"], feat, ar)
-        x = self.run_reg(pl, feat, P2, ar)
-        if self.sparse_reg(pl["reg_out"], B, x.H, x.W):
-            return self.decode(cls, x, P2, H, W, reg_out=pl["reg_out"])
+        sparse = self.sparse_reg(pl["reg_out"], B, feat.H, feat.W)
+        tower = self.tiled_tower(pl, sparse, feat.H, feat.W)
+        x = self.run_reg(pl, feat, P2, ar, tower=not tower)
+        if sparse:
+            return self.decode(cls, x, P2, H, W, reg_out=pl["reg_out"], tower=tower)
         reg = self.run_reg_out(pl["reg_out"], x)
         self._hook("cls_preds", cls), self._hook("reg_preds", reg)
         return self.decode(cls, reg, P2, H, W)
@@ -109,7 +111,7 @@ class Yolo3D(_Mono3DBase):
             reg1=E.ConvLayer(rt[3].weight, rt[3].bias, E.bn_dict(rt[4]), pad=1, relu=True, device=dev),
             reg_out=E.ConvLayer(rt[6].weight, rt[6].bias, None, pad=1, relu=False, device=dev))
 
-    def run_reg(self, pl, feat, P2, ar):
+    def run_reg(self, pl, feat, P2, ar, tower=True):
         B, h, w, dev = feat.B, feat.H, feat.W, feat.t.device
         tc = lambda l: l.engine != "simt"
         a = pl["dcn"](feat, ar.act("R1", (B, h, w, pl["dcn"].Cout), dev, lo=True), ar, "dcn")
@@ -133,13 +135,18 @@ class GroundAwareYolo3D(_Mono3DBase):
                     reg1=E.ConvLayer(rt[4].weight, rt[4].bias, E.bn_dict(rt[5]), pad=1, relu=True, device=dev),
                     reg_out=E.ConvLayer(rt[7].weight, rt[7].bias, None, pad=1, relu=False, device=dev))
 
-    def run_reg(self, pl, feat, P2, ar):
+    def reg_tower(self, pl):
+        return [(pl["reg0"], "R1", None), (pl["reg1"], "R2", None)]
+
+    def run_reg(self, pl, feat, P2, ar, tower=True):
         B, h, w, dev = feat.B, feat.H, feat.W, feat.t.device
         tc = lambda l: l.engine != "simt"
         a = pl["gac"].run(feat, P2, ar)
         self._hook("gac", a)
         if tc(pl["reg0"]) and not tc(pl["gac"].extract):
             E.split_lo(a)
+        if not tower:
+            return a
         for k, name in (("reg0", "R1"), ("reg1", "R2")):
             nxt = pl["reg1"] if k == "reg0" else pl["reg_out"]
             a = pl[k](a, ar.act(name, (B, h, w, pl[k].Cout), dev, lo=True))

@@ -235,9 +235,10 @@ class Stereo3D(Anchor3DDetector):
         return pl
 
     # ---- forward ------------------------------------------------------------------------------------------
-    def core_forward(self, left: torch.Tensor, right: torch.Tensor, reg_out: bool = True) -> Tuple[E.Act, E.Act, E.Act]:
+    def core_forward(self, left: torch.Tensor, right: torch.Tensor, reg_out: bool = True, reg_tower: bool = True) -> Tuple[E.Act, E.Act, E.Act]:
         """R/detectors/yolostereo3d_core.py:110-126 + StereoMerging :88-94.  Returns (features, cls_preds, reg_preds) Acts; with
-        reg_out=False the last one is the input of the regression output conv (`decode` runs that conv on the rows it reads)."""
+        reg_out=False the last one is the input of the regression output conv (`decode` runs that conv on the rows it reads), with
+        reg_tower=False the features again: the regression tower is left to `decode` too (`reg_tower`)."""
         pl = self.prepare()
         ar = self._arena
         dev = left.device
@@ -322,6 +323,8 @@ class Stereo3D(Anchor3DDetector):
         self._hook("features", FEAT)
         # head towers (R/heads/detection_3d_head.py:509-530); AnchorFlatten == the NHWC layout itself
         cls = run_cls_tower(pl["cls"], FEAT, ar)
+        if not reg_tower:
+            return FEAT, cls, FEAT
         r0 = pl["reg0"]
         r1 = r0(FEAT, ar.act("R1", (B, h16, w16, r0.Cout), dev, lo=True))
         c1, c2 = pl["reg_bb"]
@@ -340,15 +343,22 @@ class Stereo3D(Anchor3DDetector):
         self._hook("cls_preds", cls), self._hook("reg_preds", reg)
         return FEAT, cls, reg
 
+    def reg_tower(self, pl) -> list:
+        """The regression tower in front of reg_out as `decode` takes it: reg0 -> R1, the BasicBlock's c1 -> R2 and c2 (+ R1) -> R3."""
+        c1, c2 = pl["reg_bb"]
+        return [(pl["reg0"], "R1", None), (c1, "R2", None), (c2, "R3", 0)]
+
     def launch(self, left, right, P2, P3=None):
         """Enqueue the whole forward (backbone .. NMS) on the current stream; no host synchronisation.
         Returns the DecodeNms object holding the fixed-capacity device outputs."""
         left, right, P2 = self._device_inputs((left, "left"), (right, "right"), (P2, "P2"))
         B, _, H, W = left.shape
-        ro = self.prepare()["reg_out"]
+        pl = self.prepare()
+        ro = pl["reg_out"]
         sparse = self.sparse_reg(ro, B, H // 16, W // 16)
-        _, cls, reg = self.core_forward(left, right, reg_out=not sparse)
-        return self.decode(cls, reg, P2, H, W, reg_out=ro if sparse else None)
+        tower = self.tiled_tower(pl, sparse, H // 16, W // 16)
+        _, cls, reg = self.core_forward(left, right, reg_out=not sparse, reg_tower=not tower)
+        return self.decode(cls, reg, P2, H, W, reg_out=ro if sparse else None, tower=tower)
 
     def forward_batch(self, left, right, P2, P3=None):
         """B stereo pairs -> list of B (scores[K], bboxes[K,11], cls_indexes[K]) triples (new API; no reference counterpart).

@@ -33,7 +33,7 @@ class Act:
       * float16, shape [2, B, H, W, cs]: planes hi = rn16(t) and lo = rn16(t - hi) ("tc16" engine, the default).
     The wgmma conv engine consumes and produces these; other producers leave them stale and the plan calls `split_lo`
     before a tensor-core consumer."""
-    __slots__ = ("t", "co", "C", "lo", "f32", "lo_fresh")
+    __slots__ = ("t", "co", "C", "lo", "f32", "lo_fresh", "valid")
 
     def __init__(self, t: torch.Tensor, co: int = 0, C: Optional[int] = None, lo: Optional[torch.Tensor] = None, f32: bool = True):
         assert t.dim() == 4 and t.dtype == torch.float32 and t.is_contiguous()
@@ -42,6 +42,7 @@ class Act:
         # tensor-core convs / plane residuals): the fp16 (hi, lo) planes are the tensor, `t` only carries the shape
         self.f32 = f32
         self.lo_fresh = False      # True once a kernel that writes the companion together with the tensor (tensor-core conv, fused DCN, row conv) produced THIS view
+        self.valid = None          # [B, H, W] uint8 map of the pixels the producer wrote (a tile-listed conv); None: every pixel
         self.C = (t.shape[3] - co) if C is None else C
         assert 0 <= co and co + self.C <= t.shape[3]
         assert lo is None or (lo.dtype == torch.float32 and lo.shape == t.shape) or \
@@ -286,9 +287,29 @@ class ConvLayer:
              r0.cs if r0 is not None else 0, r0.co if r0 is not None else 0,
              P(*[t.ptr for t in outs]) if f32_out else None, oh, ol, self.Cout, o.cs, o.co, 1 if relu else 0, self.passes, self.bn_tile, _stream())
 
+    def _tc16_tiles(self, x: Act, out: Act, res: Optional[Act], relu: bool, f32_out: bool, tiles):
+        """One vd3d_conv2d_tc16_tiles launch (the `tiles` form of `__call__`)."""
+        lst, cnt, smap = tiles
+        assert self.tiles_ok() and lst.dtype == cnt.dtype == torch.int32 and smap.dtype == torch.uint8 and lst.shape[-1] == 4
+        assert lst.is_contiguous() and smap.is_contiguous() and tuple(smap.shape) == (x.B, x.H, x.W)
+        oh, ol = out.h16_ptrs if out.h16 else (None, None)
+        rf = res is not None and res.f32
+        rh, rl = res.h16_ptrs if res is not None and not rf else (None, None)
+        xh, xl = x.h16_ptrs
+        call("vd3d_conv2d_tc16_tiles", xh, xl, x.B, x.H, x.W, self.Cin, x.cs, x.co, self.w_hi.data_ptr(), self.w_lo.data_ptr(), self.out_scale,
+             self.b.data_ptr(), self.KH, self.KW, self.pad, self.dil, res.ptr if rf else None, rh, rl,
+             res.cs if res is not None else 0, res.co if res is not None else 0,
+             out.ptr if f32_out else None, oh, ol, self.Cout, out.cs, out.co, 1 if relu else 0, self.bn_tile,
+             lst.data_ptr(), cnt.data_ptr(), smap.data_ptr(), _stream())
+
     def gather_ok(self) -> bool:
         """`gather` runs this layer: fp16-split engine, stride 1, an output of the input's size"""
         return self.engine == "tc16" and self.passes == 3 and self.stride == 1 and 2 * self.pad == self.dil * (self.KH - 1) == self.dil * (self.KW - 1)
+
+    def tiles_ok(self) -> bool:
+        """`__call__` with `tiles` runs this layer: a 3x3 / pad 1 / stride 1 conv of the fp16-split engine (each output pixel reads its input
+        within one pixel)"""
+        return self.gather_ok() and self.KH == self.KW == 3 and self.pad == self.dil == 1
 
     def gather(self, x: Act, lst: torch.Tensor, counts: torch.Tensor, out: Act) -> Act:
         """The conv (with its bias, no ReLU) at the listed output pixels only, one 96-column group of `out` at a time
@@ -321,16 +342,21 @@ class ConvLayer:
             o.f32, o.lo_fresh = True, o.h16
         return outs
 
-    def __call__(self, x: Act, out: Act, res: Optional[Act] = None, relu: Optional[bool] = None, f32_out: bool = True, res_up: bool = False):
+    def __call__(self, x: Act, out: Act, res: Optional[Act] = None, relu: Optional[bool] = None, f32_out: bool = True, res_up: bool = False,
+                 tiles: Optional[Tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = None):
         """f32_out=False (fp16-split engine only): write ONLY the fp16 (hi, lo) planes of the output; legal when every consumer is a
         tensor-core conv, a plane residual or the tensor-core PSMCosine kernel.  A residual whose fp32 tensor is not valid is read
         from its planes.  res_up=True (fp16-split engine, fp32 residual): `res` has half the output size and is added nearest-upsampled
-        (the FPN top-down add)."""
+        (the FPN top-down add).  tiles = (list [cap, 4] int32, count [1] int32, store map [B, H, W] uint8) on the device (`tower_tiles`,
+        `tiles_ok` layers): the conv runs on the listed 8 x 16 tiles only and stores the pixels of the map, bit-identical to the dense conv
+        there; `out.valid` becomes the map."""
         assert x.C == self.Cin, (x.C, self.Cin)
         assert out.C == self.Cout and out.B == x.B
         Ho, Wo = self.out_hw(x.H, x.W)
         assert (out.H, out.W) == (Ho, Wo), ((out.H, out.W), (Ho, Wo))
         r = self.relu if relu is None else relu
+        if tiles is not None and (res_up or not self.tiles_ok()):
+            raise _lib.Vd3dError("tile-listed conv: a 3x3 / pad 1 / stride 1 layer of the fp16-split engine without an upsampled residual only")
         if res_up:
             self._check_tc16_input(x, "conv with an upsampled residual")
             if not out.h16 or res is None:
@@ -361,8 +387,12 @@ class ConvLayer:
                 raise _lib.Vd3dError("the 2-pass experiment mode needs VD3D_PLANES=0 (fp32 residuals)")
             if res_planes and not res.h16:
                 raise _lib.Vd3dError("conv residual: neither an fp32 tensor nor fp16 planes are valid")
-            self._tc16([x], [out], [res] if res is not None else None, False, r, f32_out)
+            if tiles is not None:
+                self._tc16_tiles(x, out, res, r, f32_out, tiles)
+            else:
+                self._tc16([x], [out], [res] if res is not None else None, False, r, f32_out)
             out.lo_fresh = out.h16
+            out.valid = tiles[2] if tiles is not None else None
             return out
         passes = 3 if self.engine == "tc" else 1
         if passes == 3 and x.lo_ptr is None:
@@ -725,14 +755,19 @@ def split_lo_if_stale(x: Act) -> Act:
 
 
 def check_lo(x: Act):
-    """Debug (VD3D_CHECK_LO=1): assert the companion of the slice a tensor-core conv is about to read is fresh."""
+    """Debug (VD3D_CHECK_LO=1): assert the companion of the slice a tensor-core conv is about to read is fresh (at the pixels its producer
+    wrote, `Act.valid`: a tile-listed conv leaves the others stale, and no stored pixel of its consumer reads them)."""
     if not x.f32:
         return                      # planes-only tensor: the planes are the tensor
     t = x.t[..., x.co:x.co + x.C]
     if x.h16:
         hi = t.half()
         lo = (t - hi.float()).half()
-        if not (torch.equal(x.lo[0][..., x.co:x.co + x.C], hi) and torch.equal(x.lo[1][..., x.co:x.co + x.C], lo)):
+        ph, pl = x.lo[0][..., x.co:x.co + x.C], x.lo[1][..., x.co:x.co + x.C]
+        if x.valid is not None:
+            v = x.valid.bool()
+            hi, lo, ph, pl = hi[v], lo[v], ph[v], pl[v]
+        if not (torch.equal(ph, hi) and torch.equal(pl, lo)):
             raise _lib.Vd3dError("stale fp16 (hi, lo) planes in front of a tensor-core conv")
         return
     hi = (t.contiguous().view(torch.int32) & -8192).view(torch.float32)
@@ -815,14 +850,38 @@ def anchor_mask(anchors: torch.Tensor, means_z: torch.Tensor, P2: torch.Tensor, 
 REG_GROUP_ANCHORS = 8
 
 
-def reg_candidates(cls_preds: torch.Tensor, mask: torch.Tensor, A: int, ncls: int, score_thr: float, lst: torch.Tensor, counts: torch.Tensor):
+def reg_candidates(cls_preds: torch.Tensor, mask: torch.Tensor, A: int, ncls: int, score_thr: float, lst: torch.Tensor, counts: torch.Tensor,
+                   pixmap: Optional[torch.Tensor] = None):
     """The (image, pixel, anchor group) pairs whose regression values the decoder may read (`vd3d_reg_candidates`): `cls_preds` NHWC [B, H, W, A *
-    (ncls + 1)], `mask` [B, P * A] with P = H * W -> `lst` [groups, B * P] int32, `counts` [groups] int32 (device)."""
+    (ncls + 1)], `mask` [B, P * A] with P = H * W -> `lst` [groups, B * P] int32, `counts` [groups] int32 (device); `pixmap` (optional) [B, P]
+    uint8: 1 at the pixels listed in some group, 0 elsewhere."""
     B = cls_preds.shape[0]
     P = cls_preds.numel() // (B * A * (ncls + 1))
     assert lst.dtype == counts.dtype == torch.int32 and lst.shape == (counts.shape[0], B * P) and counts.shape[0] == -(-A // REG_GROUP_ANCHORS)
+    assert pixmap is None or (pixmap.dtype == torch.uint8 and pixmap.numel() == B * P and pixmap.is_contiguous())
     call("vd3d_reg_candidates", cls_preds.data_ptr(), mask.data_ptr(), B, P, A, ncls, float(np.float32(score_thr)), REG_GROUP_ANCHORS,
-         lst.data_ptr(), counts.data_ptr(), _stream())
+         lst.data_ptr(), counts.data_ptr(), pixmap.data_ptr() if pixmap is not None else None, _stream())
+
+
+def tower_tile_cap(B: int, H: int, W: int) -> int:
+    """entries of one depth's tile list (`tower_tiles`): B * (ceil(H / 8) + 1) * ceil(W / 16)"""
+    return B * (-(-H // 8) + 1) * -(-W // 16)
+
+
+def tower_tiles_fit(H: int, W: int) -> bool:
+    """`tower_tiles` takes an H x W map: its two byte maps and tile flags fit the 48 KB of shared memory of its one block per depth"""
+    return ((2 * H * W + 15) & ~15) + 4 * (-(-H // 8) + 1) * -(-W // 16) <= 48 * 1024
+
+
+def tower_tiles(cand: torch.Tensor, smaps: torch.Tensor, tiles: torch.Tensor, counts: torch.Tensor):
+    """`vd3d_reg_tower_tiles`: candidate pixel map `cand` [B, H, W] uint8 -> for depth d = 1 .. D, `smaps[d - 1]` [B, H, W] uint8 = the pixels
+    within d 3x3 steps of a candidate, `tiles[d - 1]` [cap, 4] int32 = the 8 x 16 tiles (b, y0, x0, 0) that hold them (per image from its first
+    such row), `counts[d - 1]` int32 = their number.  On the device, no host synchronisation."""
+    B, H, W = cand.shape
+    D = smaps.shape[0]
+    assert cand.dtype == smaps.dtype == torch.uint8 and tiles.dtype == counts.dtype == torch.int32
+    assert tuple(smaps.shape) == (D, B, H, W) and tuple(tiles.shape) == (D, tower_tile_cap(B, H, W), 4) and tuple(counts.shape) == (D,)
+    call("vd3d_reg_tower_tiles", cand.data_ptr(), B, H, W, D, smaps.data_ptr(), tiles.data_ptr(), counts.data_ptr(), _stream())
 
 
 RANGE_MSG = ("an activation left the fp16 range (|v| >= 65520) in front of a tensor-core conv: the fp16-split engine keeps activations "
